@@ -5,6 +5,7 @@
     python -m torch.distributed.run --nnodes=1 --nproc-per-node N --master-addr 127.0.0.1 --master-port P \
         bench.py --gpus N --steps K --warmup W
     python bench.py --impl reference ...       # the UNMODIFIED reference's generate() on the host cores
+    python bench.py --dump-outputs DIR ...     # also writes what the last timed step computed, DIR/<name>.npy
 
 One "step" = one full pass of the hot path (conditioning network + all T*hop autoregressive sample steps + mu-law
 decode/fade) over this rank's batch of synthetic 80-frame mels, on the SHIPPED checkpoint when its travel copy is present
@@ -56,7 +57,36 @@ def parse():
     ap.add_argument('--no-strong', action='store_true', help='skip the strong-scaling (global batch) measurement')
     ap.add_argument('--no-cpu-baseline', action='store_true')
     ap.add_argument('--no-e2e', action='store_true')
-    return ap.parse_args()
+    ap.add_argument('--dump-outputs', metavar='DIR', default=None,
+                    help='after the timed steps, write the arrays the last timed step returned as DIR/<name>.npy (float32 / float64, '
+                         '<= 64 MB in all: a fixed seeded sample of rows when larger), so that two builds can be compared output for output; '
+                         'default workload: labels of the global batch (gathered over the ranks) and rank 0\'s wave')
+    args = ap.parse_args()
+    if args.steps < 1:
+        ap.error('--steps must be at least 1 (the timed window)')
+    return args
+
+
+DUMP_BUDGET = 64 * 1024 * 1024
+
+
+def dump_outputs(out_dir, arrays):
+    """arrays: name -> array with the rows (utterances) first.  Integer arrays are written as float32, floating ones keep float32 /
+    float64.  When the arrays together exceed DUMP_BUDGET, every array keeps the same share of its rows, a fixed seeded sample
+    whose indices go to <name>_rows.npy."""
+    arrays = {k: np.asarray(v) for k, v in arrays.items()}
+    arrays = {k: v if v.dtype in (np.float32, np.float64) else v.astype(np.float32) for k, v in arrays.items()}
+    total = sum(v.nbytes for v in arrays.values())
+    if total > DUMP_BUDGET:
+        share = DUMP_BUDGET / total
+        for k in list(arrays):
+            n = arrays[k].shape[0]
+            rows = np.sort(np.random.RandomState(0).choice(n, size=max(1, int(n * share) - 1), replace=False))
+            arrays[k] = arrays[k][rows]
+            arrays[k + '_rows'] = rows.astype(np.float64)
+    os.makedirs(out_dir, exist_ok=True)
+    for k, v in arrays.items():
+        np.save(os.path.join(out_dir, k + '.npy'), np.ascontiguousarray(v))
 
 
 # ------------------------------------------------------------------------------------------------
@@ -66,12 +96,16 @@ class ClockSampler(threading.Thread):
     def __init__(self, index):
         super().__init__(daemon=True)
         self.index, self.samples, self.reasons, self._stop_evt, self.max_mhz = index, [], set(), threading.Event(), None
+        self.name, self.power_limit_w = None, None
         try:
             import pynvml
             pynvml.nvmlInit()
             self.nv = pynvml
             self.h = pynvml.nvmlDeviceGetHandleByIndex(index)
             self.max_mhz = pynvml.nvmlDeviceGetMaxClockInfo(self.h, pynvml.NVML_CLOCK_SM)
+            name = pynvml.nvmlDeviceGetName(self.h)
+            self.name = name.decode() if isinstance(name, bytes) else name
+            self.power_limit_w = pynvml.nvmlDeviceGetEnforcedPowerLimit(self.h) / 1000.0
         except Exception:
             self.nv = None
 
@@ -101,7 +135,8 @@ class ClockSampler(threading.Thread):
         self._stop_evt.set()
         self.join(timeout=2)
         med = float(np.median(self.samples)) if self.samples else None
-        return {'sm_mhz': med, 'sm_max_mhz': self.max_mhz, 'reasons': sorted(self.reasons), 'samples': len(self.samples)}
+        return {'sm_mhz': med, 'sm_max_mhz': self.max_mhz, 'reasons': sorted(self.reasons), 'samples': len(self.samples),
+                'gpu': self.name, 'power_limit_w': self.power_limit_w}
 
 
 # ------------------------------------------------------------------------------------------------
@@ -442,8 +477,8 @@ def run_tacotron(args):
             'us_per_decoder_step': 1e6 * dt / max(1, nst),
             'decoder_loop_only': {'us_per_step': 1e3 * float(np.mean(loop_ms)) / max(1, loop_steps), 'steps': loop_steps,
                                   'kernel': 'taco_grid_kernel (128 blocks, weights resident in shared memory) unless B200TTS_TACO_GRID=0'},
-            'roofline': {'bound': 'hbm', 'achieved': step_bytes * nst / dt / 1e9, 'peak': float(peaks.get('hbm_gbs', 6650.0)), 'unit': 'GB/s',
-                         'frac': step_bytes * nst / dt / 1e9 / float(peaks.get('hbm_gbs', 6650.0)), 'traffic': None,
+            'roofline': {'bound': 'hbm', 'achieved': step_bytes * nst / dt / 1e9, 'peak': float(peaks.get('hbm_gbs', 3350.0)), 'unit': 'GB/s',
+                         'frac': step_bytes * nst / dt / 1e9 / float(peaks.get('hbm_gbs', 3350.0)), 'traffic': None,
                          'algorithmic_bytes_per_step': step_bytes,
                          'note': 'single sentence: weights are shared-memory resident across 128 blocks (taco_grid.cuh), so neither HBM nor L2 '
                                  're-streams them; the step is bound by the six L2-mediated exchanges of its dependency chain'}}
@@ -460,6 +495,8 @@ def run_tacotron(args):
 
 def main():
     args = parse()
+    if args.dump_outputs and (args.impl == 'reference' or args.workload != 'config3'):
+        raise SystemExit('--dump-outputs is implemented for the default workload (config3) on the GPU')
     if args.impl == 'reference':
         return run_reference(args)
     if args.workload == 'text2audio':
@@ -475,7 +512,7 @@ def main():
     rank = int(os.environ.get('RANK', '0'))
     local = int(os.environ.get('LOCAL_RANK', '0'))
     if not torch.cuda.is_available():
-        raise SystemExit('bench.py needs a CUDA device: the B200 path has no CPU fallback')
+        raise SystemExit('bench.py needs a CUDA device: the generation path has no CPU fallback')
     torch.cuda.set_device(local)
     dev = torch.device('cuda', local)
     if world > 1:
@@ -487,7 +524,7 @@ def main():
 
     sd, wdesc = load_weights(args.weights)
     eng = WaveRNNEngine(sd, synth.DEFAULT_DIMS, device=local)
-    flush = torch.empty(256 * 1024 * 1024 // 4, device=dev, dtype=torch.float32)   # > 126 MB L2
+    flush = torch.empty(256 * 1024 * 1024 // 4, device=dev, dtype=torch.float32)   # 5x the 50 MB L2 of an H100
 
     def sync_all():
         torch.cuda.synchronize(dev)
@@ -515,10 +552,13 @@ def main():
         ev0, ev1 = torch.cuda.Event(enable_timing=True), torch.cuda.Event(enable_timing=True)
         ev0.record()
         for i in range(steps):
-            one_step(i)
+            last = one_step(i)
         ev1.record()
         sync_all()
         eng.check()
+        if args.dump_outputs:        # what the last timed step hands its caller: all ranks' labels (gathered), this rank's wave
+            labels = torch.cat([g.view(torch.int16) for g in gathered]) if N > 1 else last['labels']
+            measure.outputs = {'labels': labels.cpu().numpy(), 'wave': last['wave'].float().cpu().numpy()}
         ms = ev0.elapsed_time(ev1)
         launches = eng.launch_count - launches0 + steps           # + the L2 flush fill per step
         kms = []
@@ -535,6 +575,8 @@ def main():
     sampler.start()
     ms, gen_ms, launches = measure(B, rank * B, args.steps, args.warmup)
     weak_kernel = measure.kernel
+    if args.dump_outputs and rank == 0:
+        dump_outputs(args.dump_outputs, measure.outputs)
     clocks = sampler.stop()
     value = N * B * S * args.steps / (ms / 1e3)
 
@@ -576,12 +618,12 @@ def main():
             peaks = json.load(open(os.path.join(ROOT, 'MEASURED_PEAKS.json')))
         except Exception:
             pass
-        hbm_peak = float(peaks.get('hbm_gbs', 6650.0))
-        peak_src = 'measured (MEASURED_PEAKS.json hbm_gbs)' if 'hbm_gbs' in peaks else 'fallback 6650 GB/s'
+        hbm_peak = float(peaks.get('hbm_gbs', 3350.0))
+        peak_src = 'measured (MEASURED_PEAKS.json hbm_gbs)' if 'hbm_gbs' in peaks else 'H100 SXM data sheet, 3350 GB/s'
         alg_bytes = S * (STEP_WEIGHT_BYTES + B * COND_BYTES_PER_UTT)       # per launch of the generation kernel
         achieved = alg_bytes / (gen_ms / 1e3) / 1e9
-        sm_mhz = clocks.get('sm_mhz') or 1965.0
-        nominal_fp32 = 148 * 128 * 2 * sm_mhz * 1e6 / 1e12
+        sm_mhz = clocks.get('sm_mhz') or 1980.0
+        nominal_fp32 = torch.cuda.get_device_properties(dev).multi_processor_count * 128 * 2 * sm_mhz * 1e6 / 1e12
         try:
             fp32_measured = eng.fp32_peak_tflops()
         except Exception:
@@ -594,18 +636,18 @@ def main():
         except Exception:
             pass
         fpeak = fp32_measured or nominal_fp32
-        # tensor-core pipeline (wavernn_tc_kernel): every fp32 operand is two fp16 planes and a dot product is three kind::f16
-        # MMA products, so the tensor cores EXECUTE 3x the algorithmic GEMM work (6656 x 512 MAC per sample; the conditioning
+        # tensor-core pipeline (wavernn_tc_kernel): every fp32 operand is two fp16 planes and a dot product is three f16
+        # wgmma products, so the tensor cores EXECUTE 3x the algorithmic GEMM work (6656 x 512 MAC per sample; the conditioning
         # and the fed-back sample column stay on the CUDA cores).  The kernel is bound by the latency of its five-exchange
         # dependency chain, not by either ceiling; both forms are reported.
         tensor_form = None
         if weak_kernel == 'wavernn_tc_kernel':
             tf = 3 * 2 * 6656 * 512 * B * S / (gen_ms / 1e3) / 1e12
-            tpeak = float(peaks.get('bf16_tflops_sustained', peaks.get('bf16_tflops', 1437.7)))
-            tensor_form = {'executed': tf, 'peak': tpeak, 'unit': 'TFLOP/s (kind::f16 tcgen05.mma, fp32 accumulate)', 'frac': tf / tpeak,
+            tpeak = float(peaks.get('bf16_tflops_sustained', peaks.get('bf16_tflops', 989.0)))
+            tensor_form = {'executed': tf, 'peak': tpeak, 'unit': 'TFLOP/s (f16 wgmma, fp32 accumulate)', 'frac': tf / tpeak,
                            'peak_source': 'measured (MEASURED_PEAKS.json bf16_tflops_sustained)' if 'bf16_tflops_sustained' in peaks
-                           else 'fallback', 'products_per_dot': 3,
-                           'note': 'latency-bound pipeline: 2 groups of 128 rows in flight over 144 layer-stationary CTAs'}
+                           else 'H100 SXM data sheet, dense', 'products_per_dot': 3,
+                           'note': 'latency-bound pipeline: 2 groups of 128 rows in flight over 128 layer-stationary CTAs'}
         line = {
             'metric': 'wavernn_audio_samples_per_sec', 'value': value, 'unit': 'samples/s', 'n_gpus': N,
             'steps': args.steps, 'warmup': args.warmup, 'ms_per_step': ms / args.steps, 'higher_is_better': True,
@@ -622,8 +664,8 @@ def main():
                          'kernel': weak_kernel, 'kernel_ms': gen_ms, 'algorithmic_bytes_per_launch': alg_bytes, 'tensor_form': tensor_form,
                          'flop_form': {'achieved': flops, 'peak': fpeak, 'unit': 'TFLOP/s fp32 CUDA-core',
                                        'frac': flops / fpeak,
-                                       'peak_source': 'measured: register-only FFMA2 loop on all SMs (b200tts_debug_fp32_peak)'
-                                       if fp32_measured else 'nominal 148 SM x 128 FMA/clk x 2 x SM clock',
+                                       'peak_source': 'measured: register-only FFMA loop on all SMs (b200tts_debug_fp32_peak)'
+                                       if fp32_measured else 'nominal SMs x 128 FMA/clk x 2 x SM clock',
                                        'nominal_peak': nominal_fp32, 'frac_of_nominal': flops / nominal_fp32}},
             'clocks': clocks,
             'gpu_launches': int(launches),

@@ -1,5 +1,5 @@
 /*
- * b200tts.h -- C ABI of libb200tts.so: the sm_100a replacement for the hot paths of
+ * b200tts.h -- C ABI of libb200tts.so: the sm_90a replacement for the hot paths of
  * lturing/tacotronv2_wavernn_chinese.
  *
  * The reference is pure Python and has no FFI of its own (SURVEY.md section 8b); the
@@ -90,7 +90,7 @@ enum {
   B200TTS_KERNEL_AUTO = 0,
   B200TTS_KERNEL_UTTERANCE = 1, /* one CTA per group of utterances, weights streamed from L2      */
   B200TTS_KERNEL_GRID = 2,      /* weight-stationary persistent cooperative grid, all SMs per step */
-  B200TTS_KERNEL_TC = 3         /* layer-stationary tensor-core pipeline (tcgen05, split-fp16 operands), 33-256 rows */
+  B200TTS_KERNEL_TC = 3         /* layer-stationary tensor-core pipeline (wgmma, split-fp16 operands), 33-256 rows */
 };
 typedef struct {
   int32_t kernel;             /* B200TTS_KERNEL_*                                                      */

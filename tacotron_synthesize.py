@@ -1,5 +1,5 @@
 #!/usr/bin/env python
-"""Text (pinyin tokens) -> mel `.npy` with Tacotron-2 on a B200 -- drop-in for the reference's `tacotron_synthesize.py`.
+"""Text (pinyin tokens) -> mel `.npy` with Tacotron-2 on an H100 -- drop-in for the reference's `tacotron_synthesize.py`.
 
     python tacotron_synthesize.py --text 'm ao2 h a2 d eng3 b ei4 l ei4 。'
 

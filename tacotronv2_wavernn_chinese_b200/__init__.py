@@ -1,4 +1,4 @@
-"""B200-native (sm_100a) WaveRNN sample-generation loop and Tacotron-2 decoder step.
+"""H100-native (sm_90a) WaveRNN sample-generation loop and Tacotron-2 decoder step.
 
 Drop-in for the hot paths of lturing/tacotronv2_wavernn_chinese behind that
 project's own Python surface (`wavernn_gen.py --file`, `WaveRNN.generate`).

@@ -1,8 +1,8 @@
-"""Builds csrc/libb200tts.so for sm_100a with nvcc (cross-compiles without a GPU).
+"""Builds csrc/libb200tts.so for sm_90a with nvcc (cross-compiles without a GPU).
 
     python -m tacotronv2_wavernn_chinese_b200.build [--force]
 
-The library is built IN-TREE (git-ignored, but it travels to the GPU box with the snapshot).
+The library is built IN-TREE (git-ignored).
 """
 from __future__ import annotations
 
@@ -15,7 +15,7 @@ PKG = os.path.dirname(os.path.abspath(__file__))
 CSRC = os.path.join(PKG, 'csrc')
 LIB = os.path.join(CSRC, 'libb200tts.so')
 SOURCES = ['b200tts_api.cu']
-NVCC_FLAGS = ['-gencode', 'arch=compute_100a,code=sm_100a', '-lineinfo', '-O3', '-std=c++17',
+NVCC_FLAGS = ['-gencode', 'arch=compute_90a,code=sm_90a', '-lineinfo', '-O3', '-std=c++17',
               '-shared', '-Xcompiler', '-fPIC', '--expt-relaxed-constexpr']
 
 

@@ -502,7 +502,7 @@ extern "C" int b200tts_wavernn_create(b200tts_wavernn** out, int device, const b
         ctx->pcw.ncta = g.ncta; ctx->pcw.feat = FEAT; ctx->pcw.aux = AUX;
 
         // ---- tensor-core pipeline (wavernn_tc.cuh): per-CTA B-operand images, every weight split into two fp16 planes
-        //      (hi, lo' = (w - hi) * 2048) in the UMMA K-major no-swizzle layout [plane][k-step 32][k half 2][N/8][8 cols][8 halves]
+        //      (hi, lo' = (w - hi) * 2048) in the wgmma K-major no-swizzle layout [plane][k-step 32][k half 2][N/8][8 cols][8 halves]
         if (NC == 1024 && ctx->sm_count >= kTcCtas) {
           std::vector<uint16_t> img((size_t)kTcCtas * kTcWimgBytes / 2, 0);
           std::vector<float> prm((size_t)kTcCtas * kTcPrm, 0.f);
@@ -541,16 +541,16 @@ extern "C" int b200tts_wavernn_create(b200tts_wavernn** out, int device, const b
                   pr[gate * 8 + i] = b[pm.obhh2 + gate * 4 + j];
                 }
               }
-            } else if (cta < 128) {                           // fc1 / fc2: 32 units
-              const bool first = cta < 112;
-              const int ci = first ? cta - 96 : cta - 112;
-              for (int i = 0; i < 32; ++i) {
-                const int unit = 32 * ci + i, j = unit & 3;
+            } else if (cta < 112) {                           // fc1 / fc2: 64 units
+              const bool first = cta < 104;
+              const int ci = first ? cta - 96 : cta - 104;
+              for (int i = 0; i < 64; ++i) {
+                const int unit = 64 * ci + i, j = unit & 3;
                 const float* b = unit_blob(unit);
-                put(wi, 32, i, b + (first ? pm.ofc1 : pm.ofc2) + (size_t)j * R);
+                put(wi, 64, i, b + (first ? pm.ofc1 : pm.ofc2) + (size_t)j * R);
               }
             } else {                                          // fc3: 64 classes
-              const int ci = cta - 128;
+              const int ci = cta - 112;
               for (int i = 0; i < 64; ++i) {
                 const int cls = 64 * ci + i;
                 const float* b = &pb[(size_t)(cls >> 3) * pm.blob];
@@ -837,8 +837,8 @@ static void launch_push_t(b200tts_wavernn* ctx, PushArgs& a, cudaStream_t st) {
   ctx->launches++;
 }
 
-// rows per group of the push kernels.  Measured (profiles/r02_push_v3_phase_cycles.txt): 8 rows 9.2 us per step, 4 rows 14.5 us
-// (64 hot L2 lines polled by 65 536 threads) -- so up to 8 rows run the 8-row variant; env B200TTS_PUSH_MIN_G is an A/B switch.
+// rows per group of the push kernels: up to 8 rows run the 8-row variant (on the previous GPU the 4-row variant was slower, its
+// 64 hot L2 lines being polled by 65 536 threads; not re-measured on the H100); env B200TTS_PUSH_MIN_G is an A/B switch.
 static inline int push_rows(int B) {
   static const int min_g = getenv("B200TTS_PUSH_MIN_G") ? atoi(getenv("B200TTS_PUSH_MIN_G")) : 8;
   const int g = B <= 4 ? 4 : (B <= 8 ? 8 : (B <= 16 ? 16 : 32));
@@ -849,7 +849,7 @@ static inline int push_rows(int B) {
 static bool push_eligible(const b200tts_wavernn* ctx, int rows) {
   static const bool off = getenv("B200TTS_PUSH") != nullptr && getenv("B200TTS_PUSH")[0] == '0';
   // Default 32: the multi-group form (wavernn_pushmg.cuh, 33 ... 256 rows) is parity-green but MEASURED SLOWER than the round-1 wide
-  // mapping (144 vs 68 us per lock-step at 256 rows, profiles/r02_pushmg_time.txt), so it only runs when asked for.
+  // mapping (twice as slow at 256 rows on the previous GPU), so it only runs when asked for.
   static const int max_rows = getenv("B200TTS_PUSH_MAX_ROWS") ? atoi(getenv("B200TTS_PUSH_MAX_ROWS")) : kMgG;
   return ctx->pm.ok && ctx->gm.ok && rows <= max_rows && rows <= kMgG * kMgMaxGroups && !off;
 }
@@ -975,20 +975,6 @@ static void launch_tc(b200tts_wavernn* ctx, const float* d_mel, GenArgs& ua, cud
   a.NT = ctx->NT; a.B = rows; a.S = ua.S; a.T = T; a.hop = hop; a.steps = ua.steps; a.ng = ng; a.NC = ctx->NC;
   a.rng_mode = ua.rng_mode; a.seed = ua.seed; a.utt_offset = ua.utt_offset; a.utt_ids = ua.utt_ids; a.q = ua.q;
   a.teacher = ua.teacher; a.logits_out = ua.logits_out; a.labels = ua.labels;
-  a.prof = nullptr;
-  const bool prof = getenv("B200TTS_TC_PROF") != nullptr;
-  a.prof_mode = prof ? atoi(getenv("B200TTS_TC_PROF")) : 0;
-#ifndef B200TTS_TC_CHAIN_PROF
-  if (a.prof_mode == 2) {      // the chain-event probe is a compile-time option (wavernn_tc.cuh): fall back to the cycle accounting
-    fprintf(stderr, "libb200tts: B200TTS_TC_PROF=2 needs a build with -DB200TTS_TC_CHAIN_PROF; printing the cycle accounting instead\n");
-    a.prof_mode = 1;
-  }
-#endif
-  if (prof) {
-    ctx->push_prof.ensure((size_t)kTcCtas * 12 * sizeof(long long));
-    B200_CUDA(cudaMemsetAsync(ctx->push_prof.p, 0, (size_t)kTcCtas * 12 * sizeof(long long), st));
-    a.prof = ctx->push_prof.as<long long>();
-  }
   ctx->last_push_ncta = 0;
   ctx->last_grid_ncta = 0;
   B200_CUDA(cudaFuncSetAttribute(wavernn_tc_kernel, cudaFuncAttributeMaxDynamicSharedMemorySize, kTcSmemBytes));
@@ -1000,38 +986,6 @@ static void launch_tc(b200tts_wavernn* ctx, const float* d_mel, GenArgs& ua, cud
   B200_CUDA(cudaLaunchCooperativeKernel((const void*)wavernn_tc_kernel, dim3(kTcCtas), dim3(kTcThreads), args, (size_t)kTcSmemBytes, st));
   ctx->launches++;
   B200_CUDA(cudaEventRecord(ctx->ev1, st));
-  if (prof) {      // development aid: mean cycles per lock-step and role, to stderr
-    B200_CUDA(cudaStreamSynchronize(st));
-    std::vector<long long> h((size_t)kTcCtas * 12);
-    B200_CUDA(cudaMemcpy(h.data(), ctx->push_prof.p, h.size() * sizeof(long long), cudaMemcpyDeviceToHost));
-    static const char* names[12] = {"ld:cnt", "ld:empty+issue", "mma:accfree", "mma:full", "mma:issue", "epi:wait-main", "epi:wait-other",
-                                    "epi:tmem", "epi:math+store", "epi:publish", "cond:wait", "cond:compute"};
-    static const char* roles[5] = {"GRU1", "GRU2", "fc1", "fc2", "fc3"};
-    const int lo[6] = {0, 32, 96, 112, 128, 144};
-    if (a.prof_mode == 2 && ua.steps > 2) {    // chain events of group 0 (first CTA of every role), mean ns between consecutive events
-      const double n = (double)(ua.steps - 1);
-      auto ev = [&](int cta, int slot) { return (double)h[(size_t)cta * 12 + slot] / n; };
-      const double a0 = ev(0, 5), b0 = ev(0, 6), a2 = ev(0, 7);
-      double prev = b0;
-      fprintf(stderr, "tc chain (ns, group 0): GRU1 winners->published %.0f", b0 - a0);
-      for (int r = 1; r < 5; ++r) {
-        const double c0 = ev(lo[r], 0), d0 = ev(lo[r], 5), e0 = ev(lo[r], 6);
-        fprintf(stderr, " | hop %.0f  %s GEMM %.0f (first stage %.0f, last stage %.0f, last MMA issued %.0f, accumulator seen %.0f) epilogue %.0f", c0 - prev,
-                roles[r], d0 - c0, ev(lo[r], 2) - c0, ev(lo[r], 3) - c0, ev(lo[r], 4) - c0, d0 - c0, e0 - d0);
-        prev = e0;
-      }
-      fprintf(stderr, " | hop %.0f  (step %.0f)\n", a2 - prev, a2 - a0);
-    } else
-    for (int r = 0; r < 5; ++r) {
-      fprintf(stderr, "tc prof %-4s (cycles per lock-step):", roles[r]);
-      for (int i = 0; i < 12; ++i) {
-        double s = 0;
-        for (int cta = lo[r]; cta < lo[r + 1]; ++cta) s += (double)h[(size_t)cta * 12 + i];
-        fprintf(stderr, " %s=%.0f", names[i], s / (lo[r + 1] - lo[r]) / ua.steps);
-      }
-      fprintf(stderr, "\n");
-    }
-  }
 }
 
 // After the stream has been synchronised: did the last grid launch abandon a barrier?
@@ -1058,8 +1012,8 @@ static void run_generate(b200tts_wavernn* ctx, const float* d_mel, int B, int T,
   const bool debug_bufs = (rng && rng->mode == B200TTS_RNG_EXT_EXPONENTIAL) || (opts && opts->d_logits);
   const bool folding = opts && opts->fold_target > 0;
   const bool packing = opts && opts->d_pack_utt;
-  // kernel=auto and more than 256 rows: launches of 256 rows through the tensor-core pipeline (50 us per lock-step each) beat the
-  // wide mapping on the whole batch (68 us per 256 rows); the noise is keyed by the global row, so the result does not change
+  // kernel=auto and more than 256 rows: launches of 256 rows through the tensor-core pipeline (66 us per lock-step each on an H100)
+  // beat the wide mapping on the whole batch (91 us per 256 rows); the noise is keyed by the global row, so the result does not change
   const bool tc_off = getenv("B200TTS_TC") != nullptr && getenv("B200TTS_TC")[0] == '0';
   const bool tc_slices = B > kTcRows * kTcMaxGroups && !tc_off && (!opts || opts->kernel == B200TTS_KERNEL_AUTO) && !debug_bufs && d_labels &&
                          tc_eligible(ctx, kTcRows * kTcMaxGroups, folding, packing);
@@ -1144,16 +1098,17 @@ static void run_generate_rows(b200tts_wavernn* ctx, const float* d_mel, int B, i
     labels = ctx->labels.as<int16_t>();
   }
   bool use_tc = false;
-  // kernel=auto: the tensor-core pipeline costs ~50 us per lock-step whatever the row count (1 or 2 groups of 128 rows in flight),
-  // the wide CUDA-core mapping 33.8 / 41.4 / 68.0 us at 64 / 128 / 256 rows -> the crossover is near 160 rows (env
-  // B200TTS_TC_MIN_ROWS; B200TTS_TC=0 keeps the CUDA-core mappings).  Fold mode and packed rows stay on the other kernels.
-  static const int tc_min_rows = getenv("B200TTS_TC_MIN_ROWS") ? atoi(getenv("B200TTS_TC_MIN_ROWS")) : 161;
+  // kernel=auto: on an H100 (80GB HBM3, 700 W) the tensor-core pipeline costs 62-66 us per lock-step whatever the row count
+  // (1 or 2 groups of 128 rows in flight), the wide CUDA-core mapping 37.5 us at 64 rows, 60.9 at 96-128 and 90-91 from 129
+  // rows on (a second tile of 128) -> the tensor cores take 129 rows and more (env B200TTS_TC_MIN_ROWS; B200TTS_TC=0 keeps the
+  // CUDA-core mappings).  Fold mode and packed rows stay on the other kernels.
+  static const int tc_min_rows = getenv("B200TTS_TC_MIN_ROWS") ? atoi(getenv("B200TTS_TC_MIN_ROWS")) : 129;
   static const bool tc_off = getenv("B200TTS_TC") != nullptr && getenv("B200TTS_TC")[0] == '0';
   if (o.kernel == B200TTS_KERNEL_AUTO && kernel == B200TTS_KERNEL_GRID && !tc_off && GB >= tc_min_rows && tc_eligible(ctx, GB, folding, packing))
     kernel = B200TTS_KERNEL_TC;
   if (kernel == B200TTS_KERNEL_TC) {
     REQUIRE(tc_eligible(ctx, GB, folding, packing), B200TTS_EINVAL,
-            "kernel=tc needs rnn_dims = fc_dims = 512, 10-bit classes, >= 144 SMs, 1..256 rows, no folding / packing");
+            "kernel=tc needs rnn_dims = fc_dims = 512, 10-bit classes, >= 128 SMs, 1..256 rows, no folding / packing");
     use_tc = true;
     kernel = B200TTS_KERNEL_GRID;
   }
@@ -1302,7 +1257,7 @@ __global__ void fp32_peak_kernel(float* out, int iters) {
 #pragma unroll
     for (int r = 0; r < 4; ++r)
 #pragma unroll
-      for (int i = 0; i < 8; ++i) a[i] = __ffma2_rn(a[i], x, y);
+      for (int i = 0; i < 8; ++i) a[i] = fma2_rn(a[i], x, y);
   }
   float s = 0.f;
 #pragma unroll
@@ -1380,7 +1335,7 @@ extern "C" int b200tts_philox_exponential(int device, uint64_t seed, uint64_t ut
   REQUIRE(d_q && B >= 1 && n_steps >= 1 && n_classes >= 4 && n_classes % 4 == 0 && step0 >= 0, B200TTS_EINVAL, "bad argument");
   DeviceGuard dg(device);
   size_t total = (size_t)n_steps * B * (n_classes / 4);
-  unsigned grid = (unsigned)std::min<size_t>((total + 255) / 256, 148 * 16);
+  unsigned grid = (unsigned)std::min<size_t>((total + 255) / 256, 132 * 16);
   philox_dump_kernel<<<grid, 256, 0, (cudaStream_t)stream>>>(seed, utterance_offset, B, step0, n_steps, n_classes, d_q);
   B200_CUDA(cudaGetLastError());
   API_END
@@ -1725,7 +1680,7 @@ extern "C" int b200tts_taco_philox_masks(int device, uint64_t seed, uint64_t utt
   REQUIRE(d_masks && B >= 1 && steps >= 1 && prenet_units >= 4, B200TTS_EINVAL, "bad argument");
   DeviceGuard dg(device);
   size_t total = (size_t)B * steps * 2 * prenet_units;
-  unsigned grid = (unsigned)std::min<size_t>((total + 255) / 256, 148 * 16);
+  unsigned grid = (unsigned)std::min<size_t>((total + 255) / 256, 132 * 16);
   taco_philox_masks_kernel<<<grid, 256, 0, (cudaStream_t)stream>>>(seed, utterance_offset, B, steps, prenet_units, d_masks);
   B200_CUDA(cudaGetLastError());
   API_END

@@ -88,6 +88,11 @@ __device__ __forceinline__ float warp_sum(float v) {
 
 __device__ __forceinline__ float sigmoidf_acc(float x) { return 1.0f / (1.0f + expf(-x)); }
 
+// two independent fp32 FMAs, round to nearest (the pairwise form the CUDA-core kernels are written in)
+__device__ __forceinline__ float2 fma2_rn(float2 a, float2 b, float2 c) {
+  return make_float2(__fmaf_rn(a.x, b.x, c.x), __fmaf_rn(a.y, b.y, c.y));
+}
+
 // `2 * label.float() / (n_classes - 1.) - 1.` in fp32, same operation order as fatchord_version.py:235
 __device__ __forceinline__ float label_to_float(int label, float ncls_m1) {
   return 2.0f * (float)label / ncls_m1 - 1.0f;

@@ -1,7 +1,7 @@
 // Tacotron-2 forward-attention decoder loop, WEIGHT-STATIONARY over 128 thread blocks (one sentence; BASELINE config 4).
 //
 // taco_decoder_kernel (taco_decoder.cuh) runs a sentence in ONE block and re-streams the 6.9 MB of decoder weights from L2
-// every step: 73 us per step measured, floor 41 us.  Here the weights are resident chip-wide, the way the WaveRNN grid is:
+// every step.  Here the weights are resident chip-wide, the way the WaveRNN grid is:
 // block c of 128 (cooperative launch, 512 threads) keeps in shared memory the columns that produce
 //     prenet units 2c, 2c+1 (both layers)   .   LSTM-1 and LSTM-2 units 2c, 2c+1 (all four gates)   .   attention dimension c
 //     context columns 4c ... 4c+3           .   mel column c (c < 80)

@@ -186,7 +186,7 @@ struct Gemm {           // rows x (sum of segs) weight block in shared memory
 };
 
 // acc[r][u] += sum_{c4 in [lo,hi)} W[r][4*(col4+c4) .. +3] . act[4*c4 .. +3][u0 .. u0+U)
-// The activation loads come from L2 (~1 us under load) and only 3 warps share a scheduler, so they are software
+// The activation loads come from L2 (about a microsecond under load) and only 3 warps share a scheduler, so they are software
 // pipelined two iterations (8 k rows) ahead in registers: three rotating buffers, loads of c4+2 issued before the
 // FMAs of c4.
 #ifndef B200_GRID_RS2_FULL
@@ -202,16 +202,15 @@ __device__ __forceinline__ void wide_fma4(float (&acc)[RT][U], const float4* __r
   for (int r = 0; r < RT; ++r) {
     float4 w = W4[r * ldw4 + c4];
     if constexpr (B200_GRID_FFMA2 && U % 2 == 0) {
-      // sm_100 packed fp32: one FFMA2 does two utterances (a 64-bit register pair) against ONE weight register, which
-      // the instruction broadcasts (`FFMA2 Rd, Ra.F32x2.HI_LO, Rw.F32, Rd.F32x2.HI_LO`) -- half the issue slots of
-      // scalar FFMA for bit-identical results (same rounding, same summation order per lane).
+      // two utterances against ONE weight register per step (fma2_rn: two scalar FFMAs on Hopper, which has no packed
+      // fp32 FMA) -- bit-identical to the scalar loop below (same rounding, same summation order per lane).
 #pragma unroll
       for (int u = 0; u < U; u += 2) {
         float2 s = make_float2(acc[r][u], acc[r][u + 1]);
-        s = __ffma2_rn(make_float2(a[0][u], a[0][u + 1]), make_float2(w.x, w.x), s);
-        s = __ffma2_rn(make_float2(a[1][u], a[1][u + 1]), make_float2(w.y, w.y), s);
-        s = __ffma2_rn(make_float2(a[2][u], a[2][u + 1]), make_float2(w.z, w.z), s);
-        s = __ffma2_rn(make_float2(a[3][u], a[3][u + 1]), make_float2(w.w, w.w), s);
+        s = fma2_rn(make_float2(a[0][u], a[0][u + 1]), make_float2(w.x, w.x), s);
+        s = fma2_rn(make_float2(a[1][u], a[1][u + 1]), make_float2(w.y, w.y), s);
+        s = fma2_rn(make_float2(a[2][u], a[2][u + 1]), make_float2(w.z, w.z), s);
+        s = fma2_rn(make_float2(a[3][u], a[3][u + 1]), make_float2(w.w, w.w), s);
         acc[r][u] = s.x; acc[r][u + 1] = s.y;
       }
     } else {
@@ -275,15 +274,15 @@ __device__ __forceinline__ void wide_accumulate_pd(float (&acc)[RT][U], const fl
 template <int U, int RT>
 __device__ __forceinline__ void wide_accumulate(float (&acc)[RT][U], const float* __restrict__ W, int ldw, int col4,
                                                 const float* __restrict__ act, int Bp, int u0, int lo, int hi) {
-  // measured on B200: 3-4 columns ahead on the 4/8-row tiles is SLOWER (19.0k vs 15.5k cycles for fc1)
+  // measured on the previous GPU: 3-4 columns ahead on the 4/8-row tiles is slower
   constexpr int PD = (B200_GRID_NW_WIDE >= 16) ? ((RT * U <= 32) ? B200_GRID_PD16_SMALL : B200_GRID_PD16) : 2;
   wide_accumulate_pd<U, RT, PD>(acc, W, ldw, col4, act, Bp, u0, lo, hi);
 }
 
 // Wide mapping: NG GEMMs of RT rows each; 8 warps = NG x UW (utterance warps) x KS (k slices).
 // Partial sums land in part[((g*KS + ks)*RT + r)*BT + ul].
-// (Measured: sharing one __noinline__ copy of this body between phases to shrink the ~65 KB kernel is SLOWER, 104.9 vs
-// 97.8 us per lock-step at B=256 -- the call/stack traffic costs more than the instruction-fetch stalls it removes.)
+// (Measured on the previous GPU: sharing one __noinline__ copy of this body between phases to shrink the ~65 KB kernel is
+// slower -- the call/stack traffic costs more than the instruction-fetch stalls it removes.)
 template <int NW, int U, int UW, int RT, int NG, int RS = 1>
 __device__ __forceinline__ void wide_partials(float* part, const Gemm& g0, const Gemm& g1, int tile_base, int Bp, int warp,
                                               int lane) {
@@ -475,9 +474,8 @@ __global__ void __launch_bounds__(MapTraits<U, UW, GROUPS>::NW * 32, 1) wavernn_
   unsigned int nbar = 0;
   const unsigned int ncta = gridDim.x;
   __shared__ int s_ok[2];                             // outcome of the group's last barrier wait
-  // Split barriers pay off when ONE group owns the SM (B <= 128: 18.7 -> 17.7 us per step at B = 1, 30.4 -> 29.4 at 32,
-  // 42.4 -> 41.9 at 128).  With two groups the other group already fills the barrier bubble and the split is slower
-  // (68.2 -> 74.5 us at B = 256 measured), so it is off there.
+  // Split barriers paid off on the previous GPU when ONE group owns the SM (B <= 128); with two groups the other group
+  // already fills the barrier bubble and the split was slower, so it is off there.  Not re-measured on the H100.
   constexpr int kSplit = (GROUPS == 1) ? B200_GRID_SPLIT_BARRIER : 0;
   bool pending = false;                               // arrived at the sampling barrier of the previous step, not yet waited
   unsigned int pend_target = 0;

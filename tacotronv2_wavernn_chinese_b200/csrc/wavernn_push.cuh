@@ -3,9 +3,9 @@
 // Same decomposition as wavernn_grid.cuh -- 128 co-resident CTAs (cooperative launch), CTA c keeps the rows of every layer
 // that produce hidden units / fc rows [4c, 4c+4) and classes [8c, 8c+8) in shared memory for the whole launch -- but the
 // five exchanges of a sample step (reference loop wavernn/models/fatchord_version.py:201-237) no longer go through a
-// grid barrier followed by a load of the activations.  At B <= 32 a step is pure latency (FMA floor 4 us at 32 rows), and
-// the barrier round (bar.sync + red.release + spin on ld.acquire + bar.sync = 1.27 us measured) plus the L2 pull after it
-// was ~75 % of the 17.7 us (B <= 4) / 29.4 us (B = 32) step of the round-1 kernel.  Here:
+// grid barrier followed by a load of the activations.  At B <= 32 a step is pure latency, and on the GPU this kernel was
+// first written for the barrier round (bar.sync + red.release + spin on ld.acquire + bar.sync) plus the L2 pull after it
+// took about three quarters of a step of the grid kernel.  Here:
 //
 //   * FLAG-IN-DATA exchange.  Every exchanged activation vector lives in L2 as [producer CTA][row][4 units] fp32, two
 //     parity copies, pre-filled with a sentinel bit pattern (0xFFFFFFFF, a NaN no arithmetic here can produce).  A
@@ -144,28 +144,23 @@ struct PollGuard {
 };
 
 // ---- exchange protocol ------------------------------------------------------------------------------------------
-// Measured in isolation (tools/exchange_bench.cu -> profiles/r02_exchange_bench.txt, cycles per all-to-all exchange of
-// a [128][G][4] vector by 128 CTAs, G = 4 / 8 / 32):  counter barrier + loads 3511 / 3600 / 4106;  every thread
-// spinning on its own entries 1558 / 2033 / 4140;  one canary warp (on the data or on replicated hint words) releasing
-// the block through a barrier 2928-3761 / 3780-4545 / 6754-7465.  The direct spin wins: detection and delivery are the
-// same L2 round trip.  Every thread issues ALL its loads first and re-polls only what still carries a sentinel.
+// Compared in isolation on the previous GPU (tools/exchange_bench.cu; all-to-all exchange of a [128][G][4] vector by 128
+// CTAs): every thread spinning on its own entries beat a counter barrier followed by loads and a canary warp releasing the
+// block through a barrier -- detection and delivery are the same L2 round trip.  Not re-measured on the H100.  Every
+// thread issues ALL its loads first and re-polls only what still carries a sentinel.
 template <int NL>
 __device__ __forceinline__ void poll_entries(const float* base, const int (&off)[NL], float4 (&a)[NL], PollGuard& g) {
 #pragma unroll
   for (int i = 0; i < NL; ++i) a[i] = ld_relaxed_f4(base + off[i]);
-  unsigned pending = 0;
+  // Then each entry in turn until it carries no sentinel.  (Written as one loop per entry: the earlier form with a bit mask
+  // of pending entries was compiled by nvcc 12.9 for sm_90a, at two entries per thread, into a test that skipped the re-poll
+  // exactly when BOTH entries were still pending -- stale sentinels went on as data, without a timeout.)
+  g.begin();
 #pragma unroll
-  for (int i = 0; i < NL; ++i) pending |= f4_ready(a[i]) ? 0u : (1u << i);
-  if (pending) {
-    g.begin();
-    while (pending && !g.aborted) {
-#pragma unroll
-      for (int i = 0; i < NL; ++i)
-        if (pending & (1u << i)) {
-          a[i] = ld_relaxed_f4(base + off[i]);
-          if (f4_ready(a[i])) pending &= ~(1u << i);
-        }
-      if (pending && g.expired()) break;
+  for (int i = 0; i < NL; ++i) {
+    while (!f4_ready(a[i]) && !g.aborted) {
+      if (g.expired()) break;
+      a[i] = ld_relaxed_f4(base + off[i]);
     }
   }
 }
@@ -215,8 +210,8 @@ __device__ __forceinline__ void push_load(const float* vecbase, float4 (&a)[Push
     for (int j = 0; j < UT; ++j) off[i * UT + j] = ((kq * NKB + i) * G + ul + NU * j) * 4;
   poll_entries<NL>(vecbase, off, a, pg);
 }
-// (settling and multiplying block by block, so that the FMAs of block i overlap the loads of block i+1, was measured SLOWER:
-//  19.4 vs 14.4 us per step at 16 rows, 24.9 vs 21.7 at 32 -- the per-block leaves no longer fit the register file)
+// (settling and multiplying block by block, so that the FMAs of block i overlap the loads of block i+1, was measured slower
+//  on the previous GPU: the per-block leaves no longer fit the register file)
 template <int G, int ROWS>
 __device__ __forceinline__ void push_mma(const float* __restrict__ W /*[ROWS][512] smem*/, const float4 (&a)[PushTraits<G>::NL], float* part,
                                          int ul, int kq, int warp, int lane) {
@@ -233,10 +228,10 @@ __device__ __forceinline__ void push_mma(const float* __restrict__ W /*[ROWS][51
       if constexpr (UT == 2) {
         // packed fp32: both rows of this thread against one broadcast weight (bit-identical to two scalar FMA chains)
         const float4 v0 = a[i * 2], v1 = a[i * 2 + 1];
-        float2 s2 = __ffma2_rn(make_float2(v0.x, v1.x), make_float2(w.x, w.x), make_float2(0.f, 0.f));
-        s2 = __ffma2_rn(make_float2(v0.y, v1.y), make_float2(w.y, w.y), s2);
-        s2 = __ffma2_rn(make_float2(v0.z, v1.z), make_float2(w.z, w.z), s2);
-        s2 = __ffma2_rn(make_float2(v0.w, v1.w), make_float2(w.w, w.w), s2);
+        float2 s2 = fma2_rn(make_float2(v0.x, v1.x), make_float2(w.x, w.x), make_float2(0.f, 0.f));
+        s2 = fma2_rn(make_float2(v0.y, v1.y), make_float2(w.y, w.y), s2);
+        s2 = fma2_rn(make_float2(v0.z, v1.z), make_float2(w.z, w.z), s2);
+        s2 = fma2_rn(make_float2(v0.w, v1.w), make_float2(w.w, w.w), s2);
         leaf[i][0] = s2.x; leaf[i][1] = s2.y;
       } else {
         const float4 v = a[i];

@@ -13,10 +13,10 @@
 // activation word is loaded ONCE per block straight into the register of the thread that multiplies it (there: once per
 // row-slice warp through L1), there are no grid barriers and no k-slice partial sums of the conditioning columns.
 //
-// STATUS (round 2): parity-green against the oracle on the shipped checkpoint at 64 / 100 / 128 / 256 rows, but NOT the default: measured
-// 36.4 / 71.4 / 144.4 us per lock-step at 64 / 128 / 256 rows against 33.8 / 41.4 / 67.8 for the wide mapping of wavernn_grid.cuh
-// (profiles/r02_pushmg_time.txt).  A group's L2 loads, FMAs, cross-warp reduction and gate math are serialised by its block
-// barriers (~18 us per group and step, flat in the number of groups): latency is hidden, issue slots are not filled.  It runs
+// STATUS: parity-green against the oracle on the shipped checkpoint at 64 / 100 / 128 / 256 rows, but NOT the default: on the
+// previous GPU it was slower than the wide mapping of wavernn_grid.cuh at 64 / 128 / 256 rows (twice as slow at 256; not
+// re-measured on the H100).  A group's L2 loads, FMAs, cross-warp reduction and gate math are serialised by its block
+// barriers (a fixed cost per group and step, flat in the number of groups): latency is hidden, issue slots are not filled.  It runs
 // only with B200TTS_PUSH_MAX_ROWS=256 in the environment; its one advantage is the batch-size-invariant arithmetic.
 //
 // Shared memory (ng = 8): weights 104 KB, two partial-sum buffers 48 KB, per group gh1/gh2 3 KB + conditioning rows 16-35

@@ -1,43 +1,42 @@
-// WaveRNN per-sample recurrence on the 5th-generation tensor cores (tcgen05.mma, accumulators in TMEM): the large-batch
+// WaveRNN per-sample recurrence on the Hopper tensor cores (wgmma, fp32 accumulators in registers): the large-batch
 // (33 ... 256 rows per GPU) form of the reference loop wavernn/models/fatchord_version.py:201-237.
 //
-// LAYER-STATIONARY decomposition.  144 co-resident CTAs, each keeps a [N x 512] slice of ONE layer's weights in shared
-// memory for the whole launch as the B operand of the MMA (K-major, no swizzle):
+// LAYER-STATIONARY decomposition.  128 co-resident CTAs (one per SM; H100 has 132), each keeps a [N x 512] slice of ONE
+// layer's weights in shared memory for the whole launch as the B operand of the MMA (K-major, no swizzle):
 //     CTAs   0- 31  GRU-1 recurrent  W_hh1, 16 hidden units x (r, z, n) = 48 columns
 //     CTAs  32- 95  GRU-2            W_ih2 and W_hh2, 8 units x (r, z, n) (+ 8 zero columns) = 32 + 32 columns
-//     CTAs  96-111  fc1, 32 units    CTAs 112-127  fc2, 32 units    CTAs 128-143  fc3, 64 classes
-// The batch is cut into groups of 128 rows = the 128 TMEM lanes of an M = 128 MMA; a group's activation vector [128 x 512] is
-// the A operand.  The two groups of a 256-row batch flow through the layers as a pipeline: while group 0 is in fc1, group 1
-// is in GRU-2, and so on -- a CTA works on whichever group has reached its layer.
+//     CTAs  96-103  fc1, 64 units    CTAs 104-111  fc2, 64 units    CTAs 112-127  fc3, 64 classes
+// The batch is cut into groups of 128 rows; a group's activation vector [128 x 512] is the A operand.  Two consumer
+// warpgroups per CTA each own 64 rows of a group (one M = 64 wgmma) and hold that slice of the accumulators in registers, so
+// the thread that issues the MMA also does the gate math of the rows it accumulated.  The two groups of a 256-row batch flow
+// through the layers as a pipeline: while group 0 is in fc1, group 1 is in GRU-2, and so on -- a CTA works on whichever group
+// has reached its layer.
 //
 // EXACTNESS.  The tensor core has no fp32 operands; every fp32 value v (weights on the host, activations by the thread that
 // produces them) is split into two fp16 planes, v = hi + lo' / 2048 with hi = fp16(v), lo' = fp16((v - hi) * 2048) (the scaling
 // keeps lo' out of the fp16 subnormals), 22 mantissa bits in all.  a.w = hi.hi + (hi.lo' + lo'.hi) / 2048 (+ lo'.lo' / 2^22,
-// dropped: below fp32 resolution): three kind::f16 MMAs per k-step with fp32 accumulation.  The accumulator TRUNCATES on every
-// add (tools/umma_split_bench.cu), so the dominant hi.hi product is accumulated in TMEM only over 8 k-steps (K = 128) per
-// accumulator; the four chunk accumulators and the cross-term accumulator are added in fp32 registers (round to nearest).
-// CPU model of exactly this arithmetic: 2.6e-7 of max|out| against float64 where an fp32 FMA loop has 8.1e-7.
+// dropped: below fp32 resolution): three f16 wgmma per k-step with fp32 accumulation.  The tensor-core accumulator does not
+// round to nearest on every add, so the dominant hi.hi product is accumulated only over 8 k-steps (K = 128) at a time; the four
+// chunk sums and the cross-term accumulator are added in fp32 registers (round to nearest).
 //
-// DATA FLOW.  An epilogue thread owns one batch row (its TMEM lane) and a quarter of the CTA's columns (16 epilogue warps, 4 threads
-// per row): it reads its accumulators with tcgen05.ld, does the gate math, and stores the result ALREADY SPLIT and ALREADY in the
-// UMMA canonical layout into the vector's image in global memory (L2): [K/32 stages][plane][k-step][k half][16 row groups][8 rows]
-// [8 halves] -- rows of a warp are contiguous.  Every epilogue warp then releases one arrival on the per-(vector, group) counter
-// (red.release.gpu, cumulative over the warp barrier; no block barrier on the critical path).  A consumer CTA's loader thread spins
-// on the counter (ld.acquire.gpu), executes fence.proxy.async, and streams the 256 KB image through a ring of 16 KB shared-memory
-// stages with cp.async.bulk; the MMA thread issues six tcgen05.mma per stage and commits to the stage's mbarrier.  Vectors are
-// double-buffered by step parity; the dependency chain of the recurrence itself guarantees that a buffer is rewritten only after
-// every reader of its previous content has finished (DESIGN.md 3.6).
+// DATA FLOW.  A consumer thread owns two batch rows and a quarter of the CTA's columns (the wgmma accumulator fragment: rows
+// r, r + 8, column pairs 8i + 2(lane % 4)).  After the gate math it stores its results ALREADY SPLIT and ALREADY in the
+// canonical K-major layout into the vector's image in global memory (L2): [K/32 stages][plane][k-step][k half][16 row groups]
+// [8 rows][8 halves] -- rows of a warp are contiguous.  Every consumer warp then releases one arrival on the per-(vector, group)
+// counter (red.release.gpu, cumulative over the warp barrier; no block barrier on the critical path).  A consumer CTA's loader
+// thread spins on the counter (ld.acquire.gpu), executes fence.proxy.async, and streams the 256 KB image through a ring of
+// 16 KB shared-memory stages with cp.async.bulk; the two warpgroups issue six wgmma per stage and release the stage through
+// its mbarrier once their products are done.  Vectors are double-buffered by step parity; the dependency chain of the
+// recurrence itself guarantees that a buffer is rewritten only after every reader of its previous content has finished:
+// parity p of a vector is rewritten at step t+2, and its producer reaches step t+2 only through the winner of step t+1, which
+// needs every layer of step t+1 -- including each consumer of parity p, which finished its GEMM of step t first.
 //
 // What stays off the tensor cores, as in the push kernels (wavernn_push.cuh): the conditioning (per-frame tables, FIR linearity;
-// GRU-1's 64 values per row come from 4 dedicated warps in blocks of <= 8 steps through a ring in L2), the sampled-label column of
-// the I layer / GRU-1 (rank 1), the Gumbel-max race.  W_hh1.h1(t) and W_hh2.h2(t) run one step ahead in the shadow of the other
-// layers and are moved from TMEM to registers as soon as they finish.  Every wait is bounded (PollGuard, ~2 s) and raises the
-// launch's error flag instead of hanging.
-//
-// Measured (B200): 50 us per lock-step for 128 as for 256 rows -- a latency chain: four GEMM phases of ~7.7 us each (the arrival
-// of the image, ~20 bytes per clock and SM; in isolation the same ring runs at 80-124, tools/bulk_stream_bench.cu), gate math
-// 1.4-3.9 us per layer, exchanges 0.5-4.4 us.  B200TTS_TC_PROF=1 prints the cycle accounting; = 2, in a build with
-// -DB200TTS_TC_CHAIN_PROF, the chain link by link.
+// GRU-1's 64 values per row come from 3 dedicated warps in blocks of <= 8 steps through a ring in L2), the sampled-label column of
+// the I layer / GRU-1 (rank 1), the Gumbel-max race.  W_hh1.h1(t) and W_hh2.h2(t) run one step ahead, right after the
+// CTA has published its own part of step t, and wait in registers for the gate math of step t+1.  Every wait is bounded
+// (PollGuard, ~2 s) and raises the launch's error flag instead of hanging; a warpgroup that gave up keeps issuing its
+// (meaningless) MMAs to the end of the GEMM so that the warps of a wgmma never diverge, and the consumers leave together.
 #pragma once
 #include <cuda_fp16.h>
 #include "common.cuh"
@@ -45,32 +44,36 @@
 
 namespace b200tts {
 
-constexpr int kTcEW = 4;                    // epilogue threads per batch row (each takes 1/kTcEW of the CTA's columns)
-constexpr int kTcThreads = (2 + 4 * kTcEW + 4) * 32;   // warp 0 loader | 1 MMA issuer | 2-17 epilogue (row = TMEM lane 32*(warp%4) + lane) | 18-21 conditioning (GRU-1 CTAs)
+constexpr int kTcConsumerWarps = 8;         // warps 0-3 / 4-7: the warpgroups of rows 0-63 / 64-127 of a group
+constexpr int kTcLoaderWarp = 8;
+constexpr int kTcCondWarp0 = 9;             // warps 9-11: conditioning (GRU-1 CTAs)
+constexpr int kTcCondWarps = 3;
+constexpr int kTcThreads = 12 * 32;         // 3 warps per SM sub-partition: up to 168 registers per thread
 constexpr int kTcRows = 128;                // rows per group
 constexpr int kTcMaxGroups = 2;
 constexpr int kTcStageBytes = 16384;        // K = 32 of one vector: [plane 2][k-step 2][k half 2][row group 16][8 rows][8 halves]
 constexpr int kTcStagesPerVec = 16;
 constexpr int kTcVecBytes = kTcStagesPerVec * kTcStageBytes;
-constexpr int kTcCtas = 144;
+constexpr int kTcCtas = 128;
 constexpr int kTcWimgBytes = 131072;        // per-CTA weight image slot
 constexpr int kTcPrm = 128;                 // per-CTA fp32 parameters
-constexpr int kTcWinCopies = 8;              // the winner words are written 8 times: 32 GRU-1 CTAs x 512 threads read them at the same moment
+constexpr int kTcStages = 6;                // shared-memory ring (fc3: 4, its 32 KB of noise take the room of two stages)
+constexpr int kTcWinCopies = 8;             // the winner words are written 8 times: 32 GRU-1 CTAs x 256 threads read them at the same moment
 constexpr int kTcCondBlk = 8;               // GRU-1 conditioning is produced in blocks of <= 8 consecutive steps of one frame
 constexpr int kTcCondSlot = kTcRows * 64;   // floats of one (step, group) of the conditioning ring
-constexpr int kTcSmemBytes = 131072 + 6 * kTcStageBytes + kTcPrm * 4;   // the GRU-2 / fc3 CTAs' need (largest); GRU-1: 96 KB + 6 stages + FIR
-constexpr int kTcFirMaxBytes = kTcSmemBytes - (98304 + 6 * kTcStageBytes + kTcPrm * 4);
+constexpr int kTcSmemBytes = kTcWimgBytes + kTcStages * kTcStageBytes + kTcPrm * 4;   // GRU-2 / fc CTAs (largest); GRU-1: 96 KB + stages + FIR
+constexpr int kTcFirMaxBytes = kTcSmemBytes - (98304 + kTcStages * kTcStageBytes + kTcPrm * 4);
 enum { TV_H1 = 0, TV_X1, TV_H2, TV_X2, TV_F1, TV_F2, TV_COUNT };
 enum { TCN_C1 = 0, TCN_C2, TCN_F1, TCN_F2, TCN_W, TCN_COUNT = 8 };
 enum { TC_ROLE_G1 = 0, TC_ROLE_G2, TC_ROLE_F1, TC_ROLE_F2, TC_ROLE_F3 };
 
 struct TcArgs {
-  const uint8_t* wimg;           // [144][kTcWimgBytes] fp16 B-operand images (b200tts_api.cu: tc_pack)
-  const float* prm;              // [144][128]
+  const uint8_t* wimg;           // [128][kTcWimgBytes] fp16 B-operand images (b200tts_api.cu: tc_pack)
+  const float* prm;              // [128][128]
   uint8_t* vec;                  // [TV_COUNT][ng][2][kTcVecBytes]
   float* x1f;                    // [ng][2][128][512] fp32 copy of x1 (GRU-2 CTAs add their h2 to it: x2 = x1 + h2)
   unsigned long long* winners;   // [ng][2][kTcWinCopies][128][16]
-  unsigned* cnt;                 // [ng][TCN_COUNT][32] arrival counters (one 128-byte line each, one arrival per epilogue WARP), zeroed before the launch
+  unsigned* cnt;                 // [ng][TCN_COUNT][32] arrival counters (one 128-byte line each, one arrival per consumer WARP), zeroed before the launch
   float* condg;                  // [32 GRU-1 CTAs][2 block buffers][ng][kTcCondBlk][128 rows][64] conditioning ring (stays in L2)
   int* error;
   const float* tab;              // [B][T+1][128][52] conditioning tables (push_cond_table_kernel)
@@ -83,8 +86,6 @@ struct TcArgs {
   const int16_t* teacher;        // [B][S]
   float* logits_out;             // [S][B][NC]
   int16_t* labels;               // [B][S]
-  long long* prof;               // optional [144][12] cycle accounting
-  int prof_mode;                 // 1: cycles per role and activity; 2: globaltimer sums of the chain events of group 0 (launch_tc prints both)
 };
 
 // ---- small PTX wrappers ------------------------------------------------------------------------------------------------
@@ -122,7 +123,7 @@ __device__ __forceinline__ bool tc_cnt_wait(const unsigned* p, unsigned need, Po
   }
 }
 // the same for a whole (converged) warp: lane 0 polls, the warp barrier passes the acquired view on -- 32x fewer requests on
-// the counter's L2 line (tens of thousands of threads wait on the same few lines at the same moment)
+// the counter's L2 line (thousands of threads wait on the same few lines at the same moment)
 __device__ __forceinline__ bool tc_cnt_wait_warp(const unsigned* p, unsigned need, PollGuard& pg, int lane) {
   bool ok = true;
   if (lane == 0) ok = tc_cnt_wait(p, need, pg);
@@ -131,84 +132,54 @@ __device__ __forceinline__ bool tc_cnt_wait_warp(const unsigned* p, unsigned nee
   if (!ok) pg.aborted = true;
   return ok;
 }
-// K-major, no swizzle: core matrix = 8 rows x 16 bytes; LBO = stride between the two K halves of one MMA, SBO = stride
-// between 8-row groups (cute/arch/mma_sm100_desc.hpp; same form as tools/umma_split_bench.cu, verified on the GPU)
+// wgmma shared-memory matrix descriptor, K-major, no swizzle: core matrix = 8 rows x 16 bytes; LBO = stride between the two
+// K halves of one k-step, SBO = stride between 8-row groups (PTX ISA, "Matrix Descriptor Format" of wgmma)
 __device__ __forceinline__ uint64_t tc_desc(uint32_t saddr, uint32_t lbo_bytes, uint32_t sbo_bytes) {
   uint64_t d = 0;
   d |= (uint64_t)((saddr & 0x3FFFF) >> 4);
   d |= (uint64_t)(lbo_bytes >> 4) << 16;
   d |= (uint64_t)(sbo_bytes >> 4) << 32;
-  d |= (uint64_t)1 << 46;
   return d;
 }
-__device__ __forceinline__ void tc_mma(uint32_t tmem_d, uint64_t da, uint64_t db, uint32_t idesc, uint32_t accumulate) {
+// D[64 x N] (+)= A[64 x 16] . B[16 x N], f16 operands from shared memory, fp32 accumulators in registers (accumulate = 0
+// overwrites D).  Fragment of a thread: D[4i + 2h + e] = (row 16 * (warp % 4) + lane / 4 + 8h, column 8i + 2 (lane % 4) + e).
+__device__ __forceinline__ void tc_wgmma32(float (&d)[16], uint64_t da, uint64_t db, uint32_t accumulate) {
   asm volatile(
-      "{\n\t.reg .pred p;\n\tsetp.ne.b32 p, %4, 0;\n\t"
-      "tcgen05.mma.cta_group::1.kind::f16 [%0], %1, %2, %3, p;\n\t}\n" ::"r"(tmem_d), "l"(da), "l"(db), "r"(idesc), "r"(accumulate)
-      : "memory");
+      "{\n\t.reg .pred p;\n\tsetp.ne.b32 p, %18, 0;\n\t"
+      "wgmma.mma_async.sync.aligned.m64n32k16.f32.f16.f16 {%0,%1,%2,%3,%4,%5,%6,%7,%8,%9,%10,%11,%12,%13,%14,%15}, %16, %17, p, 1, 1, 0, 0;\n\t}\n"
+      : "+f"(d[0]), "+f"(d[1]), "+f"(d[2]), "+f"(d[3]), "+f"(d[4]), "+f"(d[5]), "+f"(d[6]), "+f"(d[7]), "+f"(d[8]), "+f"(d[9]), "+f"(d[10]), "+f"(d[11]), "+f"(d[12]), "+f"(d[13]), "+f"(d[14]), "+f"(d[15])
+      : "l"(da), "l"(db), "r"(accumulate));
 }
-__device__ __forceinline__ void tc_commit(unsigned long long* bar) {
-  asm volatile("tcgen05.commit.cta_group::1.mbarrier::arrive::one.shared::cluster.b64 [%0];" ::"r"(tc_smem(bar)) : "memory");
+__device__ __forceinline__ void tc_wgmma48(float (&d)[24], uint64_t da, uint64_t db, uint32_t accumulate) {
+  asm volatile(
+      "{\n\t.reg .pred p;\n\tsetp.ne.b32 p, %26, 0;\n\t"
+      "wgmma.mma_async.sync.aligned.m64n48k16.f32.f16.f16 {%0,%1,%2,%3,%4,%5,%6,%7,%8,%9,%10,%11,%12,%13,%14,%15,%16,%17,%18,%19,%20,%21,%22,%23}, %24, %25, p, 1, 1, 0, 0;\n\t}\n"
+      : "+f"(d[0]), "+f"(d[1]), "+f"(d[2]), "+f"(d[3]), "+f"(d[4]), "+f"(d[5]), "+f"(d[6]), "+f"(d[7]), "+f"(d[8]), "+f"(d[9]), "+f"(d[10]), "+f"(d[11]), "+f"(d[12]), "+f"(d[13]), "+f"(d[14]), "+f"(d[15]), "+f"(d[16]), "+f"(d[17]), "+f"(d[18]), "+f"(d[19]), "+f"(d[20]), "+f"(d[21]), "+f"(d[22]), "+f"(d[23])
+      : "l"(da), "l"(db), "r"(accumulate));
 }
-__device__ __forceinline__ void tc_ld16(uint32_t taddr, uint32_t (&v)[16]) {
-  asm volatile("tcgen05.ld.sync.aligned.32x32b.x16.b32 {%0, %1, %2, %3, %4, %5, %6, %7, %8, %9, %10, %11, %12, %13, %14, %15}, [%16];\n"
-               : "=r"(v[0]), "=r"(v[1]), "=r"(v[2]), "=r"(v[3]), "=r"(v[4]), "=r"(v[5]), "=r"(v[6]), "=r"(v[7]), "=r"(v[8]),
-                 "=r"(v[9]), "=r"(v[10]), "=r"(v[11]), "=r"(v[12]), "=r"(v[13]), "=r"(v[14]), "=r"(v[15])
-               : "r"(taddr)
-               : "memory");
+__device__ __forceinline__ void tc_wgmma64(float (&d)[32], uint64_t da, uint64_t db, uint32_t accumulate) {
+  asm volatile(
+      "{\n\t.reg .pred p;\n\tsetp.ne.b32 p, %34, 0;\n\t"
+      "wgmma.mma_async.sync.aligned.m64n64k16.f32.f16.f16 {%0,%1,%2,%3,%4,%5,%6,%7,%8,%9,%10,%11,%12,%13,%14,%15,%16,%17,%18,%19,%20,%21,%22,%23,%24,%25,%26,%27,%28,%29,%30,%31}, %32, %33, p, 1, 1, 0, 0;\n\t}\n"
+      : "+f"(d[0]), "+f"(d[1]), "+f"(d[2]), "+f"(d[3]), "+f"(d[4]), "+f"(d[5]), "+f"(d[6]), "+f"(d[7]), "+f"(d[8]), "+f"(d[9]), "+f"(d[10]), "+f"(d[11]), "+f"(d[12]), "+f"(d[13]), "+f"(d[14]), "+f"(d[15]), "+f"(d[16]), "+f"(d[17]), "+f"(d[18]), "+f"(d[19]), "+f"(d[20]), "+f"(d[21]), "+f"(d[22]), "+f"(d[23]), "+f"(d[24]), "+f"(d[25]), "+f"(d[26]), "+f"(d[27]), "+f"(d[28]), "+f"(d[29]), "+f"(d[30]), "+f"(d[31])
+      : "l"(da), "l"(db), "r"(accumulate));
 }
-// 16 consecutive output columns of one GEMM from its five accumulators: ((c0 + c1) + (c2 + c3)) + cross / 2048
+template <int R>
+__device__ __forceinline__ void tc_fence_regs(float (&d)[R]) {
+#pragma unroll
+  for (int i = 0; i < R; ++i) asm volatile("" : "+f"(d[i])::"memory");
+}
 template <int N>
-__device__ __forceinline__ void tc_read16(uint32_t tslot, int col0, float (&out)[16]) {
-  uint32_t c0[16], c1[16], c2[16], c3[16], cx[16];
-  tc_ld16(tslot + col0, c0);
-  tc_ld16(tslot + N + col0, c1);
-  tc_ld16(tslot + 2 * N + col0, c2);
-  tc_ld16(tslot + 3 * N + col0, c3);
-  tc_ld16(tslot + 4 * N + col0, cx);
-  asm volatile("tcgen05.wait::ld.sync.aligned;" ::: "memory");
-#pragma unroll
-  for (int i = 0; i < 16; ++i)
-    out[i] = __fadd_rn(__fadd_rn(__fadd_rn(__uint_as_float(c0[i]), __uint_as_float(c1[i])),
-                                 __fadd_rn(__uint_as_float(c2[i]), __uint_as_float(c3[i]))),
-                       __uint_as_float(cx[i]) * (1.0f / 2048.0f));
+__device__ __forceinline__ void tc_wgmma(float (&d)[N / 2], uint64_t da, uint64_t db, uint32_t accumulate) {
+  if constexpr (N == 32) tc_wgmma32(d, da, db, accumulate);
+  else if constexpr (N == 48) tc_wgmma48(d, da, db, accumulate);
+  else tc_wgmma64(d, da, db, accumulate);
 }
-__device__ __forceinline__ void tc_ld8(uint32_t taddr, uint32_t (&v)[8]) {
-  asm volatile("tcgen05.ld.sync.aligned.32x32b.x8.b32 {%0, %1, %2, %3, %4, %5, %6, %7}, [%8];\n"
-               : "=r"(v[0]), "=r"(v[1]), "=r"(v[2]), "=r"(v[3]), "=r"(v[4]), "=r"(v[5]), "=r"(v[6]), "=r"(v[7])
-               : "r"(taddr) : "memory");
-}
-__device__ __forceinline__ void tc_ld4(uint32_t taddr, uint32_t (&v)[4]) {
-  asm volatile("tcgen05.ld.sync.aligned.32x32b.x4.b32 {%0, %1, %2, %3}, [%4];\n"
-               : "=r"(v[0]), "=r"(v[1]), "=r"(v[2]), "=r"(v[3]) : "r"(taddr) : "memory");
-}
-__device__ __forceinline__ void tc_ld2(uint32_t taddr, uint32_t (&v)[2]) {
-  asm volatile("tcgen05.ld.sync.aligned.32x32b.x2.b32 {%0, %1}, [%2];\n" : "=r"(v[0]), "=r"(v[1]) : "r"(taddr) : "memory");
-}
-template <int W>
-__device__ __forceinline__ void tc_ldW(uint32_t taddr, uint32_t (&v)[W]) {
-  if constexpr (W == 16) tc_ld16(taddr, v);
-  else if constexpr (W == 8) tc_ld8(taddr, v);
-  else if constexpr (W == 4) tc_ld4(taddr, v);
-  else tc_ld2(taddr, v);
-}
-// W consecutive output columns of one GEMM from its five accumulators: ((c0 + c1) + (c2 + c3)) + cross / 2048
-template <int N, int W>
-__device__ __forceinline__ void tc_readW(uint32_t tslot, int col0, float (&out)[W]) {
-  static_assert(W == 2 || W == 4 || W == 8 || W == 16, "tcgen05.ld width");
-  uint32_t c0[W], c1[W], c2[W], c3[W], cx[W];
-  tc_ldW<W>(tslot + col0, c0);
-  tc_ldW<W>(tslot + N + col0, c1);
-  tc_ldW<W>(tslot + 2 * N + col0, c2);
-  tc_ldW<W>(tslot + 3 * N + col0, c3);
-  tc_ldW<W>(tslot + 4 * N + col0, cx);
-  asm volatile("tcgen05.wait::ld.sync.aligned;" ::: "memory");
-#pragma unroll
-  for (int i = 0; i < W; ++i)
-    out[i] = __fadd_rn(__fadd_rn(__fadd_rn(__uint_as_float(c0[i]), __uint_as_float(c1[i])),
-                                 __fadd_rn(__uint_as_float(c2[i]), __uint_as_float(c3[i]))),
-                       __uint_as_float(cx[i]) * (1.0f / 2048.0f));
-}
+__device__ __forceinline__ void tc_wg_fence() { asm volatile("wgmma.fence.sync.aligned;" ::: "memory"); }
+__device__ __forceinline__ void tc_wg_commit() { asm volatile("wgmma.commit_group.sync.aligned;" ::: "memory"); }
+template <int P>
+__device__ __forceinline__ void tc_wg_wait() { asm volatile("wgmma.wait_group.sync.aligned %0;" ::"n"(P) : "memory"); }
+
 // fp32 -> (hi, lo') fp16 planes, 8 values -> one 16-byte word per plane
 __device__ __forceinline__ void tc_split8(const float* v, uint4& hi, uint4& lo) {
   uint32_t h[4], l[4];
@@ -229,96 +200,118 @@ __device__ __forceinline__ uint32_t tc_img_off(int k8, int row) {
   return (uint32_t)(kstep >> 1) * kTcStageBytes + (uint32_t)(kstep & 1) * 4096u + (uint32_t)ki * 2048u + (uint32_t)(row >> 3) * 128u +
          (uint32_t)(row & 7) * 16u;
 }
-__device__ __forceinline__ void tc_store8(uint8_t* img, int k8, int row, const float* v) {
-  uint4 hi, lo;
-  tc_split8(v, hi, lo);
-  uint8_t* p = img + tc_img_off(k8, row);
-  *reinterpret_cast<uint4*>(p) = hi;
-  *reinterpret_cast<uint4*>(p + 8192) = lo;
-}
-
-// W = 2, 4 or 8 consecutive units starting at unit k0 (k0 % W == 0) of row `row`: W halves per plane
-template <int W>
-__device__ __forceinline__ void tc_storeW(uint8_t* img, int k0, int row, const float* v) {
-  static_assert(W == 2 || W == 4 || W == 8 || W == 16, "store width");
-  if constexpr (W == 16) {
-    tc_store8(img, k0 >> 3, row, v);
-    tc_store8(img, (k0 >> 3) + 1, row, v + 8);
-  } else if constexpr (W == 8) {
-    tc_store8(img, k0 >> 3, row, v);
-  } else {
-    uint32_t h[W / 2], l[W / 2];
-#pragma unroll
-    for (int i = 0; i < W / 2; ++i) {
-      const __half a = __float2half_rn(v[2 * i]), b = __float2half_rn(v[2 * i + 1]);
-      const __half al = __float2half_rn((v[2 * i] - __half2float(a)) * 2048.0f);
-      const __half bl = __float2half_rn((v[2 * i + 1] - __half2float(b)) * 2048.0f);
-      h[i] = (uint32_t)__half_as_ushort(a) | ((uint32_t)__half_as_ushort(b) << 16);
-      l[i] = (uint32_t)__half_as_ushort(al) | ((uint32_t)__half_as_ushort(bl) << 16);
-    }
-    uint8_t* p = img + tc_img_off(k0 >> 3, row) + (uint32_t)(k0 & 7) * 2u;
-    if constexpr (W == 4) {
-      *reinterpret_cast<uint2*>(p) = make_uint2(h[0], h[1]);
-      *reinterpret_cast<uint2*>(p + 8192) = make_uint2(l[0], l[1]);
-    } else {
-      *reinterpret_cast<uint32_t*>(p) = h[0];
-      *reinterpret_cast<uint32_t*>(p + 8192) = l[0];
-    }
-  }
+// units k0, k0 + 1 (k0 even) of row `row`: one 32-bit word per plane
+__device__ __forceinline__ void tc_store2(uint8_t* img, int k0, int row, float v0, float v1) {
+  const __half a = __float2half_rn(v0), b = __float2half_rn(v1);
+  const __half al = __float2half_rn((v0 - __half2float(a)) * 2048.0f);
+  const __half bl = __float2half_rn((v1 - __half2float(b)) * 2048.0f);
+  uint8_t* p = img + tc_img_off(k0 >> 3, row) + (uint32_t)(k0 & 7) * 2u;
+  *reinterpret_cast<uint32_t*>(p) = (uint32_t)__half_as_ushort(a) | ((uint32_t)__half_as_ushort(b) << 16);
+  *reinterpret_cast<uint32_t*>(p + 8192) = (uint32_t)__half_as_ushort(al) | ((uint32_t)__half_as_ushort(bl) << 16);
 }
 
 struct TcRoleInfo {
   int role, ci;            // role, index inside the role
-  int N;                   // MMA N (columns per GEMM)
   int njobs;               // GEMMs per (step, group)
   int nstage;              // shared-memory stages
   int wbytes;              // weight image bytes
 };
 __device__ __forceinline__ TcRoleInfo tc_role(int cta) {
   TcRoleInfo r;
-  if (cta < 32) { r.role = TC_ROLE_G1; r.ci = cta; r.N = 48; r.njobs = 1; r.nstage = 6; r.wbytes = 98304; }
-  else if (cta < 96) { r.role = TC_ROLE_G2; r.ci = cta - 32; r.N = 32; r.njobs = 2; r.nstage = 6; r.wbytes = 131072; }
-  else if (cta < 112) { r.role = TC_ROLE_F1; r.ci = cta - 96; r.N = 32; r.njobs = 1; r.nstage = 8; r.wbytes = 65536; }
-  else if (cta < 128) { r.role = TC_ROLE_F2; r.ci = cta - 112; r.N = 32; r.njobs = 1; r.nstage = 8; r.wbytes = 65536; }
-  else { r.role = TC_ROLE_F3; r.ci = cta - 128; r.N = 64; r.njobs = 1; r.nstage = 5; r.wbytes = 131072; }   // one stage less: room for the partial winners
+  if (cta < 32) { r.role = TC_ROLE_G1; r.ci = cta; r.njobs = 1; r.nstage = kTcStages; r.wbytes = 98304; }
+  else if (cta < 96) { r.role = TC_ROLE_G2; r.ci = cta - 32; r.njobs = 2; r.nstage = kTcStages; r.wbytes = 131072; }
+  else if (cta < 104) { r.role = TC_ROLE_F1; r.ci = cta - 96; r.njobs = 1; r.nstage = kTcStages; r.wbytes = 131072; }
+  else if (cta < 112) { r.role = TC_ROLE_F2; r.ci = cta - 104; r.njobs = 1; r.nstage = kTcStages; r.wbytes = 131072; }
+  else { r.role = TC_ROLE_F3; r.ci = cta - 112; r.njobs = 1; r.nstage = 4; r.wbytes = 131072; }
   return r;
 }
-// job j of a role: which vector it multiplies, which counter announces it, how many arrivals (4 epilogue warps per producer CTA) fill it
+// job j of a role: which vector it multiplies, which counter announces it, how many arrivals (8 consumer warps per producer CTA) fill it
 __device__ __forceinline__ void tc_job(int role, int j, int& vec, int& cnt, int& nprod) {
   switch (role) {
-    case TC_ROLE_G1: vec = TV_H1; cnt = TCN_C1; nprod = 32 * 4 * kTcEW; break;
-    case TC_ROLE_G2: if (j == 0) { vec = TV_X1; cnt = TCN_C1; nprod = 32 * 4 * kTcEW; } else { vec = TV_H2; cnt = TCN_C2; nprod = 64 * 4 * kTcEW; } break;
-    case TC_ROLE_F1: vec = TV_X2; cnt = TCN_C2; nprod = 64 * 4 * kTcEW; break;
-    case TC_ROLE_F2: vec = TV_F1; cnt = TCN_F1; nprod = 16 * 4 * kTcEW; break;
-    default: vec = TV_F2; cnt = TCN_F2; nprod = 16 * 4 * kTcEW; break;
-  }
-}
-// accumulator slot (TMEM column base) of job j of group g; q = running GEMM number of the CTA
-__device__ __forceinline__ int tc_slot(int role, int j, int g, unsigned q) {
-  switch (role) {
-    case TC_ROLE_G1: return g;                         // the shadow result waits in TMEM for the gate math of the next step
-    case TC_ROLE_G2: return j == 0 ? 2 : g;            // slot 2: W_ih2.x1 (transient); slots 0/1: W_hh2.h2 of group 0/1 (waiting)
-    case TC_ROLE_F3: return 0;
-    default: return (int)(q % 3u);
+    case TC_ROLE_G1: vec = TV_H1; cnt = TCN_C1; nprod = 32 * kTcConsumerWarps; break;
+    case TC_ROLE_G2: if (j == 0) { vec = TV_X1; cnt = TCN_C1; nprod = 32 * kTcConsumerWarps; } else { vec = TV_H2; cnt = TCN_C2; nprod = 64 * kTcConsumerWarps; } break;
+    case TC_ROLE_F1: vec = TV_X2; cnt = TCN_C2; nprod = 64 * kTcConsumerWarps; break;
+    case TC_ROLE_F2: vec = TV_F1; cnt = TCN_F1; nprod = 8 * kTcConsumerWarps; break;
+    default: vec = TV_F2; cnt = TCN_F2; nprod = 8 * kTcConsumerWarps; break;
   }
 }
 
+// OR of `flag` over the 8 consumer warps (named barrier 1): they all leave a loop at the same point
+__device__ __forceinline__ bool tc_consumers_any(bool flag) {
+  unsigned any;
+  asm volatile("{\n\t.reg .pred p, q;\n\tsetp.ne.u32 q, %1, 0;\n\tbar.red.or.pred p, 1, %2, q;\n\tselp.u32 %0, 1, 0, p;\n\t}\n"
+               : "=r"(any) : "r"(flag ? 1u : 0u), "n"(kTcConsumerWarps * 32) : "memory");
+  return any != 0;
+}
+
+// One GEMM of this warpgroup's 64 rows: out[N/2] = A (the vector image streamed through the stage ring) . W (image at w_saddr),
+// K = 512, as ((c0 + c1) + c2) + c3 + cross / 2048 with c_k the hi.hi products of k-steps 8k ... 8k+7.  `s` counts the stages
+// consumed by this CTA.  Each consumer warp releases a stage (one of kTcConsumerWarps arrivals) once its products are done.
+template <int N>
+__device__ __forceinline__ void tc_gemm(float (&out)[N / 2], uint32_t st0, uint32_t w_saddr, unsigned nstage, unsigned& s, unsigned long long* bar_full,
+                                        unsigned long long* bar_empty, int wg, int lane, PollGuard& pg) {
+  float acc[N / 2], crs[N / 2];
+#pragma unroll
+  for (int i = 0; i < N / 2; ++i) { acc[i] = 0.f; crs[i] = 0.f; }
+  const uint64_t dB = tc_desc(w_saddr, (uint32_t)(N / 8) * 128u, 128u);
+  const uint64_t dA0 = tc_desc(st0 + (uint32_t)wg * 1024u, 2048u, 128u);      // this warpgroup's 8 row groups
+  const uint32_t btile = (uint32_t)N * 32u;                                     // bytes of one k-step tile of B
+  auto release = [&](unsigned stage) {
+    __syncwarp();
+    if (lane == 0) tc_mbar_arrive(&bar_empty[stage % nstage]);
+  };
+  for (int ks = 0; ks < kTcStagesPerVec; ++ks, ++s) {
+    const unsigned sl = s % nstage, su = s / nstage;
+    tc_mbar_wait(&bar_full[sl], su & 1u, pg);         // after an abort: no wait, the MMAs below still run (on stale data)
+    const uint64_t dA = dA0 + (uint64_t)((sl * kTcStageBytes) >> 4);
+    tc_fence_regs(acc);
+    tc_fence_regs(crs);
+    tc_wg_fence();
+#pragma unroll
+    for (int h = 0; h < 2; ++h) {
+      const int K = ks * 2 + h;
+      const uint64_t a_hi = dA + (uint64_t)((h * 4096) >> 4);
+      const uint64_t a_lo = dA + (uint64_t)((8192 + h * 4096) >> 4);
+      const uint64_t b_hi = dB + (uint64_t)(((uint32_t)K * btile) >> 4);
+      const uint64_t b_lo = dB + (uint64_t)(((uint32_t)(32 + K) * btile) >> 4);
+      tc_wgmma<N>(acc, a_hi, b_hi, (K & 7) ? 1u : 0u);
+      tc_wgmma<N>(crs, a_hi, b_lo, K ? 1u : 0u);
+      tc_wgmma<N>(crs, a_lo, b_hi, 1u);
+    }
+    tc_wg_commit();
+    if ((ks & 3) == 3) {                              // end of a K = 128 chunk: fold its hi.hi sum into out
+      tc_wg_wait<0>();
+      tc_fence_regs(acc);
+      tc_fence_regs(crs);
+#pragma unroll
+      for (int i = 0; i < N / 2; ++i) out[i] = ks == 3 ? acc[i] : __fadd_rn(out[i], acc[i]);
+      release(s - 1);
+      release(s);
+    } else if ((ks & 3) != 0) {                       // the previous stage's products are done
+      tc_wg_wait<1>();
+      release(s - 1);
+    }
+  }
+#pragma unroll
+  for (int i = 0; i < N / 2; ++i) out[i] = __fadd_rn(out[i], crs[i] * (1.0f / 2048.0f));
+}
+
 __global__ void __launch_bounds__(kTcThreads, 1) wavernn_tc_kernel(TcArgs A) {
-  extern __shared__ __align__(128) uint8_t tsm[];
-  __shared__ __align__(8) unsigned long long bar_full[8], bar_empty[8], bar_accfull[3], bar_accfree[3], bar_condfull[2], bar_condempty[2], bar_w;
-  __shared__ uint32_t tmem_base_s;
-  const int tid = threadIdx.x, warp = tid >> 5, lane = tid & 31;
+  extern __shared__ __align__(1024) uint8_t tsm[];
+  __shared__ __align__(8) unsigned long long bar_full[kTcStages], bar_empty[kTcStages], bar_condfull[2], bar_condempty[2], bar_w;
+  const int tid = threadIdx.x, lane = tid & 31;
+  const int warp = __shfl_sync(0xffffffffu, tid >> 5, 0);     // provably warp-uniform: the role branches hold wgmma
   const TcRoleInfo R = tc_role(blockIdx.x);
   const int ng = A.ng;
   uint8_t* Wsm = tsm;
   uint8_t* stages = tsm + R.wbytes;
   float* prm = reinterpret_cast<float*>(stages + (size_t)R.nstage * kTcStageBytes);
   float* fir_s = prm + kTcPrm;                         // GRU-1 CTAs only: [hop][NT]
+  float* noise_s = prm + kTcPrm;                       // fc3 CTAs only: [32][256 consumer threads] log q
 
   if (tid == 0) {
-    for (int i = 0; i < 8; ++i) { mbar_init(&bar_full[i], 1); mbar_init(&bar_empty[i], 1); }
-    for (int i = 0; i < 3; ++i) { mbar_init(&bar_accfull[i], 1); mbar_init(&bar_accfree[i], 4 * kTcEW); }     // one arrival per epilogue warp
-    for (int i = 0; i < 2; ++i) { mbar_init(&bar_condfull[i], 4); mbar_init(&bar_condempty[i], 4 * kTcEW); }   // per conditioning / epilogue warp
+    for (int i = 0; i < kTcStages; ++i) { mbar_init(&bar_full[i], 1); mbar_init(&bar_empty[i], kTcConsumerWarps); }
+    for (int i = 0; i < 2; ++i) { mbar_init(&bar_condfull[i], kTcCondWarps); mbar_init(&bar_condempty[i], kTcConsumerWarps); }
     mbar_init(&bar_w, 1);
   }
   for (int i = tid; i < kTcPrm; i += kTcThreads) prm[i] = A.prm[(size_t)blockIdx.x * kTcPrm + i];
@@ -330,57 +323,13 @@ __global__ void __launch_bounds__(kTcThreads, 1) wavernn_tc_kernel(TcArgs A) {
     const uint8_t* src = A.wimg + (size_t)blockIdx.x * kTcWimgBytes;
     for (int off = 0; off < R.wbytes; off += 32768) tma_bulk_g2s(Wsm + off, src + off, 32768u, &bar_w);
   }
-  if (warp == 0) {
-    __syncwarp();
-    asm volatile("tcgen05.alloc.cta_group::1.sync.aligned.shared::cta.b32 [%0], %1;" ::"r"(tc_smem(&tmem_base_s)), "r"(512));
-    asm volatile("tcgen05.relinquish_alloc_permit.cta_group::1.sync.aligned;" ::);
-  }
   mbar_wait(&bar_w, 0);
-  asm volatile("tcgen05.fence::before_thread_sync;" ::: "memory");
   __syncthreads();
-  asm volatile("tcgen05.fence::after_thread_sync;" ::: "memory");
-  const uint32_t tmem = tmem_base_s;
   PollGuard pg{A.error, 0, 0, false};
-  // optional cycle accounting (env B200TTS_TC_PROF): 12 slots per CTA, see launch_tc for the names
-  long long pacc[12];
-#pragma unroll
-  for (int i = 0; i < 12; ++i) pacc[i] = 0;
-  long long tlast = clock64();
-// chain-event probe (B200TTS_TC_PROF=2): compiled in only with -DB200TTS_TC_CHAIN_PROF -- even when switched off at run time its
-// predicates on the critical path cost 2 % of a lock-step (52.2 -> 53.3 us, same box: profiles/r02_tc_ab_variants.txt)
-#ifdef B200TTS_TC_CHAIN_PROF
-#define TC_GT(slot, cond)                                                          \
-  do {                                                                             \
-    if (A.prof_mode == 2 && (cond)) {                                              \
-      unsigned long long gt_;                                                      \
-      asm volatile("mov.u64 %0, %%globaltimer;" : "=l"(gt_));                      \
-      pacc[slot] += (long long)gt_;                                                \
-    }                                                                              \
-  } while (0)
-#define TC_CYCLES_ON (A.prof && A.prof_mode != 2)
-#else
-#define TC_GT(slot, cond) do { } while (0)
-#define TC_CYCLES_ON (A.prof)
-#endif
-#define TC_MARK(slot)                        \
-  do {                                       \
-    if (TC_CYCLES_ON) {                      \
-      const long long now_ = clock64();      \
-      pacc[slot] += now_ - tlast;            \
-      tlast = now_;                          \
-    }                                        \
-  } while (0)
-#define TC_FLUSH(first, last)                                                                                \
-  do {                                                                                                       \
-    if (A.prof)                                                                                              \
-      for (int i_ = first; i_ <= last; ++i_) A.prof[(size_t)blockIdx.x * 12 + i_] = pacc[i_];                \
-  } while (0)
-  const int N = R.N;
-  const int acc_cols = 5 * N;
   auto vec_img = [&](int v, int g, int par) { return A.vec + (((size_t)v * ng + g) * 2 + par) * (size_t)kTcVecBytes; };
   auto counter = [&](int g, int which) { return A.cnt + ((size_t)g * TCN_COUNT + which) * 32; };
 
-  if (warp == 0) {
+  if (warp == kTcLoaderWarp) {
     // ================= loader: counter -> bulk copies into the stage ring =================
     if (lane == 0) {
       unsigned s = 0;
@@ -390,8 +339,6 @@ __global__ void __launch_bounds__(kTcThreads, 1) wavernn_tc_kernel(TcArgs A) {
             int v, cw, nprod;
             tc_job(R.role, j, v, cw, nprod);
             if (!tc_cnt_wait(counter(g, cw), (unsigned)nprod * (unsigned)(t + 1), pg)) break;
-            TC_MARK(0);
-            TC_GT(0, j == 0 && g == 0 && t >= 1);
             asm volatile("fence.proxy.async;" ::: "memory");      // generic-proxy stores of the producers -> this thread's async-proxy reads
             const uint8_t* src = vec_img(v, g, t & 1);
             for (int ks = 0; ks < kTcStagesPerVec; ++ks, ++s) {
@@ -400,371 +347,277 @@ __global__ void __launch_bounds__(kTcThreads, 1) wavernn_tc_kernel(TcArgs A) {
               mbar_expect_tx(&bar_full[slot], kTcStageBytes);
               tma_bulk_g2s(stages + (size_t)slot * kTcStageBytes, src + (size_t)ks * kTcStageBytes, kTcStageBytes, &bar_full[slot]);
             }
-            TC_MARK(1);
             if (pg.aborted) break;
           }
-      TC_FLUSH(0, 1);
     }
     __syncwarp();
-  } else if (warp == 1) {
-    // ================= MMA issuer =================
-    if (lane == 0) {
-      // instruction descriptor: D = f32, A = B = f16, both K-major, N, M = 128
-      const uint32_t idesc = (1u << 4) | ((uint32_t)(N >> 3) << 17) | ((uint32_t)(kTcRows >> 4) << 24);
-      const uint32_t w0 = tc_smem(Wsm), st0 = tc_smem(stages);
-      const uint32_t btile = (uint32_t)N * 32u;                       // bytes of one k-step tile of B
-      unsigned s = 0, q = 0, accphase = 0;
-      for (int t = 0; t < A.steps && !pg.aborted; ++t)
-        for (int g = 0; g < ng && !pg.aborted; ++g)
-          for (int j = 0; j < R.njobs; ++j, ++q) {
-            const int slot = tc_slot(R.role, j, g, q);
-            const unsigned use = (accphase >> slot) & 1u;
-            accphase ^= 1u << slot;
-            if (!tc_mbar_wait(&bar_accfree[slot], use ^ 1u, pg)) break;
-            TC_MARK(2);
-            asm volatile("tcgen05.fence::after_thread_sync;" ::: "memory");
-            const uint32_t d0 = tmem + (uint32_t)(slot * acc_cols);
-            // descriptors = base + (byte offset >> 4) in the 14-bit address field (all addresses < 256 KB: no carry out of it)
-            const uint64_t dB = tc_desc(w0 + (uint32_t)j * 65536u, (uint32_t)(N / 8) * 128u, 128u);   // GRU-2: second matrix image at + 64 KB
-            const uint64_t dA0 = tc_desc(st0, 2048u, 128u);
-            for (int ks = 0; ks < kTcStagesPerVec; ++ks, ++s) {
-              const unsigned sl = s % (unsigned)R.nstage, su = s / (unsigned)R.nstage;
-              if (!tc_mbar_wait(&bar_full[sl], su & 1u, pg)) break;
-              TC_MARK(3);
-              TC_GT(2, ks == 0 && j == 0 && g == 0 && t >= 1);
-              TC_GT(3, ks == kTcStagesPerVec - 1 && j == 0 && g == 0 && t >= 1);
-              asm volatile("tcgen05.fence::after_thread_sync;" ::: "memory");
-              const uint64_t dA = dA0 + (uint64_t)((sl * kTcStageBytes) >> 4);
-#pragma unroll
-              for (int h = 0; h < 2; ++h) {
-                const int K = ks * 2 + h;
-                const uint64_t a_hi = dA + (uint64_t)((h * 4096) >> 4);
-                const uint64_t a_lo = dA + (uint64_t)((8192 + h * 4096) >> 4);
-                const uint64_t b_hi = dB + (uint64_t)(((uint32_t)K * btile) >> 4);
-                const uint64_t b_lo = dB + (uint64_t)(((uint32_t)(32 + K) * btile) >> 4);
-                tc_mma(d0 + (uint32_t)((K >> 3) * N), a_hi, b_hi, idesc, (K & 7) ? 1u : 0u);
-                tc_mma(d0 + (uint32_t)(4 * N), a_hi, b_lo, idesc, K ? 1u : 0u);
-                tc_mma(d0 + (uint32_t)(4 * N), a_lo, b_hi, idesc, 1u);
-              }
-              tc_commit(&bar_empty[sl]);
-              TC_MARK(4);
-            }
-            if (pg.aborted) break;
-            tc_commit(&bar_accfull[slot]);
-            TC_GT(4, j == 0 && g == 0 && t >= 1);
-          }
-      TC_FLUSH(2, 4);
-    }
-    __syncwarp();
-  } else if (warp < 2 + 4 * kTcEW) {
-    // ================= epilogue: kTcEW threads per batch row (TMEM lane 32*(warp%4) + lane), each a slice of the CTA's columns ======
-    const int row = 32 * (warp & 3) + lane;
-    const int sub = (warp - 2) >> 2;                       // which slice of the columns
-    const uint32_t tlane = tmem + ((uint32_t)(32 * (warp & 3)) << 16);
+  } else if (warp < kTcConsumerWarps) {
+    // ================= consumers: MMA + gate math; rows ra, rb = ra + 8 of the group, column pairs 8i + 2c ================
+    const int wg = warp >> 2, c = lane & 3;
+    const int ra = 64 * wg + 16 * (warp & 3) + (lane >> 2);
+    const int rows[2] = {ra, ra + 8};
     const float ncls_m1 = (float)(A.NC - 1);
-    unsigned accphase = 0, q = 0;
-    // One arrival per WARP: its 32 rows are stored -> lane 0 releases (red.release.gpu is cumulative over what the warp barrier
-    // ordered before it).  No block barrier on the critical path; the warp also agrees on giving up (a lane that timed out must
-    // not leave the others of its warp behind in a .sync.aligned instruction).
-    auto publish = [&](int g, int which, bool mark = true) {
-      if (mark) TC_MARK(8);
+    const uint32_t w0 = tc_smem(Wsm), st0 = tc_smem(stages);
+    const unsigned ns = (unsigned)R.nstage;
+    unsigned s = 0;
+    // One arrival per WARP: its rows are stored -> lane 0 releases (red.release.gpu is cumulative over what the warp barrier
+    // ordered before it).  No block barrier on the critical path; the warp also agrees on giving up.
+    auto publish = [&](int g, int which) {
       // (the generic -> async proxy fence of this exchange is executed by the CONSUMER's loader thread, after its acquire)
       if (__any_sync(0xffffffffu, pg.aborted)) { pg.aborted = true; return; }
       if (lane == 0) tc_red_release(counter(g, which), 1u);
-      TC_MARK(9);
-    };
-    auto acc_wait = [&](int slot) {
-      const unsigned use = (accphase >> slot) & 1u;
-      accphase ^= 1u << slot;
-      tc_mbar_wait(&bar_accfull[slot], use, pg);
-      asm volatile("tcgen05.fence::after_thread_sync;" ::: "memory");
-    };
-    auto acc_release = [&](int slot) {                     // one arrival per warp
-      asm volatile("tcgen05.fence::before_thread_sync;" ::: "memory");
-      __syncwarp();
-      if (lane == 0) tc_mbar_arrive(&bar_accfree[slot]);
     };
 
     if (R.role == TC_ROLE_G1) {
-      constexpr int U = 16 / kTcEW;                        // units per thread
-      const int u0 = U * sub;
-      float h1own[kTcMaxGroups][U], ghs[kTcMaxGroups][3][U];   // ghs: W_hh1 . h1(t-1) of this thread's units (0 at t = 0)
+      // units of this thread: q = 0..3 -> 2c, 2c+1, 2c+8, 2c+9; gate `gate` of unit q sits at fragment 4 (2 gate + q/2) + 2 h + q%2
+      int uq[4] = {2 * c, 2 * c + 1, 2 * c + 8, 2 * c + 9};
+      float h1own[kTcMaxGroups][8], ghs[kTcMaxGroups][24];     // ghs: W_hh1 . h1(t-1) in fragment order (0 at t = 0)
 #pragma unroll
-      for (int g = 0; g < kTcMaxGroups; ++g)
+      for (int g = 0; g < kTcMaxGroups; ++g) {
 #pragma unroll
-        for (int i = 0; i < U; ++i) { h1own[g][i] = 0.f; ghs[g][0][i] = 0.f; ghs[g][1][i] = 0.f; ghs[g][2][i] = 0.f; }
+        for (int i = 0; i < 8; ++i) h1own[g][i] = 0.f;
+#pragma unroll
+        for (int i = 0; i < 24; ++i) ghs[g][i] = 0.f;
+      }
       const float* Ax = prm;                               // [4 kinds][16]
       const float* bhh = prm + 64;                         // [3 gates][16]
       int blk_t0 = 0, blk_t1 = 0, blk_i = -1;               // current conditioning block: steps [blk_t0, blk_t1) of all groups
       const float* cring = A.condg + (size_t)R.ci * 2 * ng * kTcCondBlk * kTcCondSlot;
-      for (int t = 0; t <= A.steps && !pg.aborted; ++t) {
+      for (int t = 0; t <= A.steps; ++t) {
         if (t < A.steps && t == blk_t1) {
           blk_t0 = t;
           blk_t1 = min(min(t + kTcCondBlk, (t / A.hop + 1) * A.hop), A.steps);
           ++blk_i;
           tc_mbar_wait(&bar_condfull[blk_i & 1], (unsigned)(blk_i >> 1) & 1u, pg);
-          TC_MARK(6);
         }
 #pragma unroll
         for (int g = 0; g < kTcMaxGroups; ++g) {
           if (g >= ng) continue;
-          const int grow = g * kTcRows + row;
-          // this thread's conditioned values of (t, g) (4 kinds x U units): issued before the winner wait, they arrive in its shadow
-          float cd[4][U];
+          // this thread's conditioned values of (t, g) (4 kinds x 4 units x 2 rows): issued before the winner wait
+          float cd[2][4][4];
           if (t < A.steps) {
-            const float* cp = cring + ((size_t)((blk_i & 1) * ng + g) * kTcCondBlk + (t - blk_t0)) * kTcCondSlot + (size_t)row * 64 + u0;
 #pragma unroll
-            for (int kind = 0; kind < 4; ++kind)
+            for (int h = 0; h < 2; ++h) {
+              const float* cp = cring + ((size_t)((blk_i & 1) * ng + g) * kTcCondBlk + (t - blk_t0)) * kTcCondSlot + (size_t)rows[h] * 64 + 2 * c;
 #pragma unroll
-              for (int i = 0; i < U; i += 4) {
-                const float4 v = __ldcg(reinterpret_cast<const float4*>(cp + kind * 16 + i));
-                cd[kind][i] = v.x; cd[kind][i + 1] = v.y; cd[kind][i + 2] = v.z; cd[kind][i + 3] = v.w;
+              for (int kind = 0; kind < 4; ++kind) {
+                const float2 v0 = __ldcg(reinterpret_cast<const float2*>(cp + kind * 16));
+                const float2 v1 = __ldcg(reinterpret_cast<const float2*>(cp + kind * 16 + 8));
+                cd[h][kind][0] = v0.x; cd[h][kind][1] = v0.y; cd[h][kind][2] = v1.x; cd[h][kind][3] = v1.y;
               }
-          }
-          float x = 0.f;
-          if (t > 0) {
-            tc_cnt_wait_warp(counter(g, TCN_W), 64u * (unsigned)t, pg, lane);
-            TC_MARK(5);
-            TC_GT(5, g == 0 && t < A.steps);
-            TC_GT(7, g == 0 && t >= 2);
-            const unsigned long long* wp = A.winners + ((((size_t)g * 2 + ((t - 1) & 1)) * kTcWinCopies + (R.ci & (kTcWinCopies - 1))) * kTcRows + row) * 16;
-            unsigned long long best = 0ull;
-#pragma unroll
-            for (int i = 0; i < 16; i += 2) {
-              const ulonglong2 w2 = __ldcg(reinterpret_cast<const ulonglong2*>(wp + i));
-              best = w2.x > best ? w2.x : best;
-              best = w2.y > best ? w2.y : best;
             }
-            const int label = (int)push_cls(best);
-            if (grow < A.B) {
-              if (R.ci == 0 && sub == 0) A.labels[(size_t)grow * A.S + (t - 1)] = (int16_t)label;
-              const int fb = A.teacher ? (int)A.teacher[(size_t)grow * A.S + (t - 1)] : label;
-              x = label_to_float(fb, ncls_m1);
+          }
+          float x[2] = {0.f, 0.f};
+          if (t > 0) {
+            tc_cnt_wait_warp(counter(g, TCN_W), (unsigned)(16 * kTcConsumerWarps) * (unsigned)t, pg, lane);
+#pragma unroll
+            for (int h = 0; h < 2; ++h) {
+              const int row = rows[h], grow = g * kTcRows + row;
+              const unsigned long long* wp = A.winners + ((((size_t)g * 2 + ((t - 1) & 1)) * kTcWinCopies + (R.ci & (kTcWinCopies - 1))) * kTcRows + row) * 16;
+              unsigned long long best = 0ull;
+#pragma unroll
+              for (int i = 0; i < 16; i += 2) {
+                const ulonglong2 w2 = __ldcg(reinterpret_cast<const ulonglong2*>(wp + i));
+                best = w2.x > best ? w2.x : best;
+                best = w2.y > best ? w2.y : best;
+              }
+              const int label = (int)push_cls(best);
+              if (grow < A.B) {
+                if (R.ci == 0 && c == 0) A.labels[(size_t)grow * A.S + (t - 1)] = (int16_t)label;
+                const int fb = A.teacher ? (int)A.teacher[(size_t)grow * A.S + (t - 1)] : label;
+                x[h] = label_to_float(fb, ncls_m1);
+              }
             }
           }
           if (t == A.steps) continue;                      // the extra trip only collects the last winner
-          TC_MARK(6);
-          float hnew[U], x1[U];
 #pragma unroll
-          for (int i = 0; i < U; ++i) {
-            const float iout = fmaf(Ax[u0 + i], x, cd[0][i]);
-            const float gir = fmaf(Ax[16 + u0 + i], x, cd[1][i]);
-            const float giz = fmaf(Ax[32 + u0 + i], x, cd[2][i]);
-            const float gin = fmaf(Ax[48 + u0 + i], x, cd[3][i]);
-            const float h = gru_update(gir, giz, gin, ghs[g][0][i] + bhh[u0 + i], ghs[g][1][i] + bhh[16 + u0 + i],
-                                       ghs[g][2][i] + bhh[32 + u0 + i], h1own[g][i]);
-            h1own[g][i] = h;
-            hnew[i] = h;
-            x1[i] = iout + h;
+          for (int h = 0; h < 2; ++h) {
+            float hnew[4], x1[4];
+#pragma unroll
+            for (int qi = 0; qi < 4; ++qi) {
+              const int u = uq[qi], f = 4 * (qi >> 1) + 2 * h + (qi & 1);
+              const float iout = fmaf(Ax[u], x[h], cd[h][0][qi]);
+              const float gir = fmaf(Ax[16 + u], x[h], cd[h][1][qi]);
+              const float giz = fmaf(Ax[32 + u], x[h], cd[h][2][qi]);
+              const float gin = fmaf(Ax[48 + u], x[h], cd[h][3][qi]);
+              const float hv = gru_update(gir, giz, gin, ghs[g][f] + bhh[u], ghs[g][8 + f] + bhh[16 + u], ghs[g][16 + f] + bhh[32 + u],
+                                          h1own[g][4 * h + qi]);
+              h1own[g][4 * h + qi] = hv;
+              hnew[qi] = hv;
+              x1[qi] = iout + hv;
+            }
+            const int row = rows[h];
+            tc_store2(vec_img(TV_H1, g, t & 1), 16 * R.ci + 2 * c, row, hnew[0], hnew[1]);
+            tc_store2(vec_img(TV_H1, g, t & 1), 16 * R.ci + 2 * c + 8, row, hnew[2], hnew[3]);
+            tc_store2(vec_img(TV_X1, g, t & 1), 16 * R.ci + 2 * c, row, x1[0], x1[1]);
+            tc_store2(vec_img(TV_X1, g, t & 1), 16 * R.ci + 2 * c + 8, row, x1[2], x1[3]);
+            float* xf = A.x1f + (((size_t)g * 2 + (t & 1)) * kTcRows + row) * 512 + 16 * R.ci + 2 * c;
+            *reinterpret_cast<float2*>(xf) = make_float2(x1[0], x1[1]);
+            *reinterpret_cast<float2*>(xf + 8) = make_float2(x1[2], x1[3]);
           }
-          TC_MARK(8);
-          tc_storeW<U>(vec_img(TV_H1, g, t & 1), 16 * R.ci + u0, row, hnew);
-          tc_storeW<U>(vec_img(TV_X1, g, t & 1), 16 * R.ci + u0, row, x1);
-          float* xf = A.x1f + (((size_t)g * 2 + (t & 1)) * kTcRows + row) * 512 + 16 * R.ci + u0;
-#pragma unroll
-          for (int i = 0; i < U; i += 4) *reinterpret_cast<float4*>(xf + i) = make_float4(x1[i], x1[i + 1], x1[i + 2], x1[i + 3]);
-          publish(g, TCN_C1, false);
-          TC_GT(6, g == 0 && t >= 1);
-          // off the critical path: W_hh1 . h1(t) (the GEMM all GRU-1 CTAs start once h1(t) is complete) is moved from TMEM to
-          // registers as soon as it is done, so that the gate math of step t+1 finds it there
-          acc_wait(g);
-          {
-            const uint32_t ts = tlane + (uint32_t)(g * 240);
-#pragma unroll
-            for (int gate = 0; gate < 3; ++gate) tc_readW<48, U>(ts, gate * 16 + u0, ghs[g][gate]);
-          }
-          acc_release(g);
-          TC_MARK(7);
+          publish(g, TCN_C1);
+          // W_hh1 . h1(t) (the GEMM all GRU-1 CTAs start once h1(t) is complete) waits in registers for the gate math of step t+1
+          tc_gemm<48>(ghs[g], st0, w0, ns, s, bar_full, bar_empty, wg, lane, pg);
         }
+        if (tc_consumers_any(pg.aborted)) break;
         if (t < A.steps && t == blk_t1 - 1) {                // the block's values are all in registers / used: one arrival per warp
           __syncwarp();
           if (lane == 0) tc_mbar_arrive(&bar_condempty[blk_i & 1]);
         }
       }
     } else if (R.role == TC_ROLE_G2) {
-      constexpr int U = 8 / kTcEW;                         // 2 units per thread
-      static_assert(U == 2, "GRU-2 epilogue is written for 2 units per thread");
-      const int u0 = U * sub;
-      float h2own[kTcMaxGroups][U], ghs[kTcMaxGroups][3][U];
+      // units of this thread: 2c, 2c+1; gate `gate` at fragment 4 gate + 2 h + e
+      float h2own[kTcMaxGroups][4], ghs[kTcMaxGroups][16];
 #pragma unroll
-      for (int g = 0; g < kTcMaxGroups; ++g)
+      for (int g = 0; g < kTcMaxGroups; ++g) {
 #pragma unroll
-        for (int i = 0; i < U; ++i) { h2own[g][i] = 0.f; ghs[g][0][i] = 0.f; ghs[g][1][i] = 0.f; ghs[g][2][i] = 0.f; }
+        for (int i = 0; i < 4; ++i) h2own[g][i] = 0.f;
+#pragma unroll
+        for (int i = 0; i < 16; ++i) ghs[g][i] = 0.f;
+      }
       const float* bhh = prm;                              // [3 gates][8]
-      for (int t = 0; t < A.steps && !pg.aborted; ++t) {
+      for (int t = 0; t < A.steps; ++t) {
         const int fr = t / A.hop;
 #pragma unroll
         for (int g = 0; g < kTcMaxGroups; ++g) {
           if (g >= ng) continue;
-          const int grow = g * kTcRows + row, src = min(grow, A.B - 1);
           // conditioning (aux projection + bias of the three gates, constant within a frame): table rows 32 + gate*4 + unit%4
-          float cd[3][U];
-          {
-            const float* tb = A.tab + (((size_t)src * (A.T + 1) + fr) * 128 + 2 * R.ci + (u0 >> 2)) * kPushCondRows + 32 + (u0 & 3);
+          float cd[2][3][2];
+#pragma unroll
+          for (int h = 0; h < 2; ++h) {
+            const int src = min(g * kTcRows + rows[h], A.B - 1);
+            const float* tb = A.tab + (((size_t)src * (A.T + 1) + fr) * 128 + 2 * R.ci + (c >> 1)) * kPushCondRows + 32 + 2 * (c & 1);
 #pragma unroll
             for (int gate = 0; gate < 3; ++gate) {
               const float2 v = __ldg(reinterpret_cast<const float2*>(tb + gate * 4));
-              cd[gate][0] = v.x; cd[gate][1] = v.y;
+              cd[h][gate][0] = v.x; cd[h][gate][1] = v.y;
             }
           }
-          float gi[3][U];
-          TC_MARK(8);
-          acc_wait(2);
-          TC_MARK(5);
-          TC_GT(5, g == 0 && t >= 1);
+          float gi[16];
+          tc_gemm<32>(gi, st0, w0, ns, s, bar_full, bar_empty, wg, lane, pg);      // W_ih2 . x1(t)
+          // own units of x1 (fp32).  Its counter was complete before this CTA's GEMM could even start (the loader waited for
+          // it), so the check passes at its first poll; it gives this warp's loads their acquire
+          tc_cnt_wait_warp(counter(g, TCN_C1), (unsigned)(32 * kTcConsumerWarps) * (unsigned)(t + 1), pg, lane);
 #pragma unroll
-          for (int gate = 0; gate < 3; ++gate) tc_readW<32, U>(tlane + 320u, gate * 8 + u0, gi[gate]);
-          acc_release(2);
-          TC_MARK(7);
-          // own units of x1 (fp32).  Its counter was complete before this CTA's GEMM could even start (the loader waited for it), so the
-          // check passes at its first poll.  It stays AFTER the accumulator read: polled before the accumulator wait (in the shadow of
-          // the GEMM) the 64 x 16 warps' acquire loads compete with the bulk-copy stream and the step gets 0.8 us longer (same box A/B)
-          tc_cnt_wait_warp(counter(g, TCN_C1), (unsigned)(32 * 4 * kTcEW) * (unsigned)(t + 1), pg, lane);
-          const float2 xa = __ldcg(reinterpret_cast<const float2*>(A.x1f + (((size_t)g * 2 + (t & 1)) * kTcRows + row) * 512 + 8 * R.ci + u0));
-          const float x1[U] = {xa.x, xa.y};
-          float hnew[U], x2[U];
+          for (int h = 0; h < 2; ++h) {
+            const int row = rows[h];
+            const float2 xa = __ldcg(reinterpret_cast<const float2*>(A.x1f + (((size_t)g * 2 + (t & 1)) * kTcRows + row) * 512 + 8 * R.ci + 2 * c));
+            const float x1[2] = {xa.x, xa.y};
+            float hnew[2], x2[2];
 #pragma unroll
-          for (int i = 0; i < U; ++i) {
-            const float h = gru_update(gi[0][i] + cd[0][i], gi[1][i] + cd[1][i], gi[2][i] + cd[2][i], ghs[g][0][i] + bhh[u0 + i],
-                                       ghs[g][1][i] + bhh[8 + u0 + i], ghs[g][2][i] + bhh[16 + u0 + i], h2own[g][i]);
-            h2own[g][i] = h;
-            hnew[i] = h;
-            x2[i] = x1[i] + h;
+            for (int e = 0; e < 2; ++e) {
+              const int u = 2 * c + e, f = 2 * h + e;
+              const float hv = gru_update(gi[f] + cd[h][0][e], gi[4 + f] + cd[h][1][e], gi[8 + f] + cd[h][2][e], ghs[g][f] + bhh[u],
+                                          ghs[g][4 + f] + bhh[8 + u], ghs[g][8 + f] + bhh[16 + u], h2own[g][2 * h + e]);
+              h2own[g][2 * h + e] = hv;
+              hnew[e] = hv;
+              x2[e] = x1[e] + hv;
+            }
+            tc_store2(vec_img(TV_H2, g, t & 1), 8 * R.ci + 2 * c, row, hnew[0], hnew[1]);
+            tc_store2(vec_img(TV_X2, g, t & 1), 8 * R.ci + 2 * c, row, x2[0], x2[1]);
           }
-          tc_storeW<U>(vec_img(TV_H2, g, t & 1), 8 * R.ci + u0, row, hnew);
-          tc_storeW<U>(vec_img(TV_X2, g, t & 1), 8 * R.ci + u0, row, x2);
           publish(g, TCN_C2);
-          TC_GT(6, g == 0 && t >= 1);
-          // off the critical path: W_hh2 . h2(t) from TMEM to registers for step t+1
-          acc_wait(g);
-          TC_MARK(6);
-#pragma unroll
-          for (int gate = 0; gate < 3; ++gate) tc_readW<32, U>(tlane + (uint32_t)(g * 160), gate * 8 + u0, ghs[g][gate]);
-          acc_release(g);
-          TC_MARK(7);
+          // W_hh2 . h2(t) for step t+1
+          tc_gemm<32>(ghs[g], st0, w0 + 65536u, ns, s, bar_full, bar_empty, wg, lane, pg);
         }
+        if (tc_consumers_any(pg.aborted)) break;
       }
     } else if (R.role == TC_ROLE_F1 || R.role == TC_ROLE_F2) {
-      constexpr int U = 32 / kTcEW;                        // 8 units per thread
-      static_assert(U == 8, "fc1 / fc2 epilogue is written for 8 units per thread");
-      const int u0 = U * sub;
+      // units of this thread: 8i + 2c + e, i = 0..7
       const int trow = R.role == TC_ROLE_F1 ? 44 : 48;     // table rows of the aux projection + bias: fc1 44-47, fc2 48-51
       const int vout = R.role == TC_ROLE_F1 ? TV_F1 : TV_F2, cout = R.role == TC_ROLE_F1 ? TCN_F1 : TCN_F2;
-      for (int t = 0; t < A.steps && !pg.aborted; ++t) {
+      for (int t = 0; t < A.steps; ++t) {
         const int fr = t / A.hop;
-        for (int g = 0; g < ng && !pg.aborted; ++g, ++q) {
-          const int grow = g * kTcRows + row, src = min(grow, A.B - 1);
-          float cd[U];
-          {
-            const float* tb = A.tab + (((size_t)src * (A.T + 1) + fr) * 128 + 8 * R.ci + (u0 >> 2)) * kPushCondRows + trow;
+        for (int g = 0; g < ng; ++g) {
+          float a[32];
+          tc_gemm<64>(a, st0, w0, ns, s, bar_full, bar_empty, wg, lane, pg);
 #pragma unroll
-            for (int c4 = 0; c4 < U / 4; ++c4) {
-              const float4 v = __ldg(reinterpret_cast<const float4*>(tb + c4 * kPushCondRows));
-              cd[c4 * 4] = v.x; cd[c4 * 4 + 1] = v.y; cd[c4 * 4 + 2] = v.z; cd[c4 * 4 + 3] = v.w;
-            }
-          }
-          const int slot = (int)(q % 3u);
-          TC_MARK(8);
-          acc_wait(slot);
-          TC_MARK(5);
-          TC_GT(5, g == 0 && t >= 1);
-          float a[U];
-          tc_readW<32, U>(tlane + (uint32_t)(slot * 160), u0, a);
-          acc_release(slot);
-          TC_MARK(7);
-#pragma unroll
-          for (int i = 0; i < U; ++i) a[i] = fmaxf(a[i] + cd[i], 0.f);
-          tc_storeW<U>(vec_img(vout, g, t & 1), 32 * R.ci + u0, row, a);
-          publish(g, cout);
-          TC_GT(6, g == 0 && t >= 1);
-        }
-      }
-    } else {
-      // ---- fc3 + Gumbel-max: 16 of this CTA's 64 classes per thread, the 4 partial winners of a row meet in shared memory ----
-      constexpr int U = 64 / kTcEW;
-      static_assert(U == 16, "fc3 epilogue is written for 16 classes per thread");
-      const float* b3 = prm;
-      unsigned long long* swin = reinterpret_cast<unsigned long long*>(prm + kTcPrm);      // [kTcEW][128]
-      for (int t = 0; t < A.steps && !pg.aborted; ++t) {
-        for (int g = 0; g < ng && !pg.aborted; ++g) {
-          const int grow = g * kTcRows + row;
-          const bool live = grow < A.B;
-          const int cls0 = 64 * R.ci + U * sub;
-          // noise first: it does not depend on the accumulators
-          float nl[U];
-          if (live && A.rng_mode == 0) {
-            const unsigned long long uid = A.utt_ids ? A.utt_ids[grow] : A.utt_offset + (unsigned long long)grow;
-#pragma unroll
-            for (int i = 0; i < U / 4; ++i) {
-              float q4[4];
-              philox_exp4(A.seed, uid, (uint32_t)t, (uint32_t)((cls0 >> 2) + i), q4);
-#pragma unroll
-              for (int k = 0; k < 4; ++k) nl[4 * i + k] = logf(q4[k]);
-            }
-          } else if (live) {
-            const float4* qp = reinterpret_cast<const float4*>(A.q + ((size_t)t * A.B + grow) * A.NC + cls0);
-#pragma unroll
-            for (int i = 0; i < U / 4; ++i) {
-              const float4 v = __ldg(qp + i);
-              nl[4 * i] = logf(v.x); nl[4 * i + 1] = logf(v.y); nl[4 * i + 2] = logf(v.z); nl[4 * i + 3] = logf(v.w);
-            }
-          } else {
-#pragma unroll
-            for (int i = 0; i < U; ++i) nl[i] = 0.f;
-          }
-          TC_MARK(8);
-          acc_wait(0);
-          TC_MARK(5);
-          TC_GT(5, g == 0 && t >= 1);
-          unsigned long long best = 0ull;
-#pragma unroll
-          for (int hb = 0; hb < 2; ++hb) {
-            float l[8];
-            tc_readW<64, 8>(tlane, U * sub + 8 * hb, l);
+          for (int h = 0; h < 2; ++h) {
+            const int row = rows[h], src = min(g * kTcRows + row, A.B - 1);
+            const float* tb = A.tab + (((size_t)src * (A.T + 1) + fr) * 128 + 16 * R.ci + (c >> 1)) * kPushCondRows + trow + 2 * (c & 1);
 #pragma unroll
             for (int i = 0; i < 8; ++i) {
-              const int cls = cls0 + 8 * hb + i;
-              const float lv = l[i] + b3[U * sub + 8 * hb + i];
-              if (live && A.logits_out) A.logits_out[((size_t)t * A.B + grow) * A.NC + cls] = lv;
-              const unsigned long long p = push_pack(lv - nl[8 * hb + i], (uint32_t)cls, (uint32_t)(t + 1));
-              best = p > best ? p : best;
+              const float2 cd = __ldg(reinterpret_cast<const float2*>(tb + (size_t)(2 * i) * kPushCondRows));
+              tc_store2(vec_img(vout, g, t & 1), 64 * R.ci + 8 * i + 2 * c, row, fmaxf(a[4 * i + 2 * h] + cd.x, 0.f),
+                        fmaxf(a[4 * i + 2 * h + 1] + cd.y, 0.f));
             }
           }
-          acc_release(0);
-          TC_MARK(7);
-          swin[sub * kTcRows + row] = best;
-          // block barrier of the 4*kTcEW epilogue warps; it also ORs the abort flags so that everybody leaves at the same point
-          unsigned any;
-          asm volatile("{\n\t.reg .pred p, q;\n\tsetp.ne.u32 q, %1, 0;\n\tbar.red.or.pred p, 1, %2, q;\n\tselp.u32 %0, 1, 0, p;\n\t}\n"
-                       : "=r"(any) : "r"(pg.aborted ? 1u : 0u), "n"(128 * kTcEW) : "memory");
-          if (any) { pg.aborted = true; break; }
-          if (sub == 0) {
-#pragma unroll
-            for (int k = 1; k < kTcEW; ++k) {
-              const unsigned long long o = swin[k * kTcRows + row];
-              best = o > best ? o : best;
-            }
-#pragma unroll
-            for (int cp = 0; cp < kTcWinCopies; ++cp)
-              A.winners[((((size_t)g * 2 + (t & 1)) * kTcWinCopies + cp) * kTcRows + row) * 16 + R.ci] = best;
-            publish(g, TCN_W);
-            TC_GT(6, g == 0 && t >= 1);
-          }
-          // (swin is rewritten only after the next accumulator wait, which follows this barrier in every thread's program order;
-          //  the readers above finish before they arrive at the NEXT barrier, and writers of the next round pass THIS one first --
-          //  a second barrier is needed for strict safety)
-          asm volatile("bar.sync 2, %0;" ::"n"(128 * kTcEW) : "memory");
+          publish(g, cout);
+          if (tc_consumers_any(pg.aborted)) { pg.aborted = true; break; }
         }
+        if (pg.aborted) break;
+      }
+    } else {
+      // ---- fc3 + Gumbel-max: 16 of this CTA's 64 classes per row and thread, the 4 threads of a row meet by shuffles ----
+      const float* b3 = prm;
+      for (int t = 0; t < A.steps; ++t) {
+        for (int g = 0; g < ng; ++g) {
+          // noise first: it does not depend on the accumulators (log q of class 64 ci + 8i + 2c + e, fragment order); it waits
+          // for the GEMM in this thread's own shared-memory slot, the registers go to the accumulators
+          float* nl = noise_s + tid;
+#pragma unroll
+          for (int h = 0; h < 2; ++h) {
+            const int grow = g * kTcRows + rows[h];
+            const bool live = grow < A.B;
+#pragma unroll
+            for (int i = 0; i < 8; ++i) {
+              const int cls = 64 * R.ci + 8 * i + 2 * c;
+              float n0 = 0.f, n1 = 0.f;
+              if (live && A.rng_mode == 0) {
+                const unsigned long long uid = A.utt_ids ? A.utt_ids[grow] : A.utt_offset + (unsigned long long)grow;
+                float q4[4];
+                philox_exp4(A.seed, uid, (uint32_t)t, (uint32_t)(cls >> 2), q4);
+                n0 = logf((c & 1) ? q4[2] : q4[0]);          // this thread's two of the four classes
+                n1 = logf((c & 1) ? q4[3] : q4[1]);
+              } else if (live) {
+                const float2 v = __ldg(reinterpret_cast<const float2*>(A.q + ((size_t)t * A.B + grow) * A.NC + cls));
+                n0 = logf(v.x); n1 = logf(v.y);
+              }
+              nl[(4 * i + 2 * h) * 256] = n0;
+              nl[(4 * i + 2 * h + 1) * 256] = n1;
+            }
+          }
+          float l[32];
+          tc_gemm<64>(l, st0, w0, ns, s, bar_full, bar_empty, wg, lane, pg);
+#pragma unroll
+          for (int h = 0; h < 2; ++h) {
+            const int row = rows[h], grow = g * kTcRows + row;
+            const bool live = grow < A.B;
+            unsigned long long best = 0ull;
+#pragma unroll
+            for (int i = 0; i < 8; ++i) {
+              const int cls = 64 * R.ci + 8 * i + 2 * c;
+              const float l0 = l[4 * i + 2 * h] + b3[8 * i + 2 * c], l1 = l[4 * i + 2 * h + 1] + b3[8 * i + 2 * c + 1];
+              if (live && A.logits_out) *reinterpret_cast<float2*>(A.logits_out + ((size_t)t * A.B + grow) * A.NC + cls) = make_float2(l0, l1);
+              const unsigned long long p0 = push_pack(l0 - nl[(4 * i + 2 * h) * 256], (uint32_t)cls, (uint32_t)(t + 1));
+              const unsigned long long p1 = push_pack(l1 - nl[(4 * i + 2 * h + 1) * 256], (uint32_t)(cls + 1), (uint32_t)(t + 1));
+              best = p0 > best ? p0 : best;
+              best = p1 > best ? p1 : best;
+            }
+#pragma unroll
+            for (int o = 1; o <= 2; o <<= 1) {
+              const unsigned long long other = __shfl_xor_sync(0xffffffffu, best, o);
+              best = other > best ? other : best;
+            }
+            if (c == 0) {
+#pragma unroll
+              for (int cp = 0; cp < kTcWinCopies; ++cp)
+                A.winners[((((size_t)g * 2 + (t & 1)) * kTcWinCopies + cp) * kTcRows + row) * 16 + R.ci] = best;
+            }
+          }
+          publish(g, TCN_W);
+          if (tc_consumers_any(pg.aborted)) { pg.aborted = true; break; }
+        }
+        if (pg.aborted) break;
       }
     }
-    if (tid == 64) TC_FLUSH(5, 9);
-  } else if (R.role == TC_ROLE_G1) {
+  } else if (warp >= kTcCondWarp0 && R.role == TC_ROLE_G1) {
     // ================= conditioning warps (GRU-1 CTAs): the 64 conditioned values of every row, a BLOCK of <= 8 steps at a time ========
     // Within a frame the <= 7 table rows an output combines do not change, only the FIR phase does: they are loaded once per block
     // and combined for every step of it (8x fewer table loads than step by step).  The results go to a small ring in global
     // memory (two block buffers per CTA, L2 resident) that the gate threads read back one step at a time.
     // lane = value: lanes 0-15 / 16-31 take the 16 table entries (kind*4 + unit%4) of two adjacent 4-unit table blocks.
-    const int cwarp = warp - (2 + 4 * kTcEW);
+    const int cwarp = warp - kTcCondWarp0;
     const int half = lane >> 4, i16 = lane & 15;
     const size_t fstride = (size_t)128 * kPushCondRows;
     float* cring = A.condg + (size_t)R.ci * 2 * ng * kTcCondBlk * kTcCondSlot;
@@ -773,12 +626,10 @@ __global__ void __launch_bounds__(kTcThreads, 1) wavernn_tc_kernel(TcArgs A) {
       const int fr = t0 / A.hop, ph0 = t0 - fr * A.hop;
       const int t1 = min(min(t0 + kTcCondBlk, (fr + 1) * A.hop), A.steps), n = t1 - t0;
       if (!tc_mbar_wait(&bar_condempty[b & 1], ((unsigned)(b >> 1) & 1u) ^ 1u, pg)) break;
-      TC_MARK(10);
       for (int g = 0; g < ng; ++g) {
         float* dst = cring + (size_t)((b & 1) * ng + g) * kTcCondBlk * kTcCondSlot;
 #pragma unroll 2
-        for (int rr = 0; rr < 32; ++rr) {                      // 2 rows x 2 blocks x 7 table loads in flight per lane
-          const int row = cwarp * 32 + rr;
+        for (int row = cwarp; row < kTcRows; row += kTcCondWarps) {   // 2 rows x 2 blocks x 7 table loads in flight per lane
           const int src = min(g * kTcRows + row, A.B - 1);
 #pragma unroll
           for (int p = 0; p < 2; ++p) {
@@ -805,15 +656,10 @@ __global__ void __launch_bounds__(kTcThreads, 1) wavernn_tc_kernel(TcArgs A) {
       }
       __syncwarp();
       if (lane == 0) tc_mbar_arrive(&bar_condfull[b & 1]);
-      TC_MARK(11);
       t0 = t1;
     }
-    if (tid == (2 + 4 * kTcEW) * 32) TC_FLUSH(10, 11);
   }
-  // ---- teardown ----
-  asm volatile("tcgen05.fence::before_thread_sync;" ::: "memory");
   __syncthreads();
-  if (warp == 0) asm volatile("tcgen05.dealloc.cta_group::1.sync.aligned.b32 %0, %1;" ::"r"(tmem), "r"(512));
 }
 
 }  // namespace b200tts

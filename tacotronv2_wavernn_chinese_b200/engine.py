@@ -38,7 +38,7 @@ class WaveRNNEngine:
 
     def __init__(self, state_dict: dict, dims: dict, device: int | None = None):
         if not torch.cuda.is_available():
-            raise RuntimeError('no CUDA device: the B200 WaveRNN path has no CPU fallback')
+            raise RuntimeError('no CUDA device: the WaveRNN path has no CPU fallback')
         self.lib = _lib.load()
         self.device = torch.cuda.current_device() if device is None else int(device)
         self.dims = dict(dims)
@@ -228,7 +228,7 @@ class WaveRNNEngine:
         _lib.check(self.lib.b200tts_wavernn_check(self._h))
 
     def fp32_peak_tflops(self) -> float:
-        """Measured fp32 CUDA-core ceiling of this device (register-only FFMA2 loop), TFLOP/s."""
+        """Measured fp32 CUDA-core ceiling of this device (register-only FFMA loop), TFLOP/s."""
         v = C.c_double()
         _lib.check(self.lib.b200tts_debug_fp32_peak(self.device, C.byref(v)))
         return float(v.value)

@@ -17,7 +17,7 @@ and below ~32 rows it barely depends on the row count at all, so
   * the sampling noise and the prenet dropout are keyed by the GLOBAL sentence index (`rng.d_utterance_ids`), so a
     sentence's audio depends neither on the chunking nor on the number of ranks.
 Tacotron itself is replicated on every rank: one thread block decodes one sentence, all sentences of a set decode
-concurrently (<= 148 per GPU), so sharding it would not shorten anything -- and it removes the mel exchange.
+concurrently (<= 132 per GPU), so sharding it would not shorten anything -- and it removes the mel exchange.
 """
 from __future__ import annotations
 
@@ -47,8 +47,9 @@ def padded_lockstep_rows(frames, chunks, hop=275):
     return done, need
 
 
-# us per lock-step of the push kernel by row count (B200, profiles/r02_push_v5_phase_cycles.txt): the scheduler's cost model
-STEP_US = {8: 9.0, 16: 14.5, 32: 20.6}
+# us per lock-step of the push kernel by row count (one H100 80GB HBM3 at 700 W, tools/quick_time.py grid 1,8,16,32 3000): the
+# scheduler's cost model
+STEP_US = {8: 18.0, 16: 34.3, 32: 31.0}
 
 
 def pack_schedule(frames, rows, hop=275):

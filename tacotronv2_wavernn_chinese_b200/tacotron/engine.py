@@ -20,7 +20,7 @@ def _ptr(t):
 class TacoDecoderEngine:
     def __init__(self, weights: dict, cfg: dict | None = None, device: int | None = None):
         if not torch.cuda.is_available():
-            raise RuntimeError('no CUDA device: the B200 Tacotron decoder has no CPU fallback')
+            raise RuntimeError('no CUDA device: the Tacotron decoder has no CPU fallback')
         self.lib = _lib.load()
         self.device = torch.cuda.current_device() if device is None else int(device)
         self.cfg = dict(DEFAULT_CFG)

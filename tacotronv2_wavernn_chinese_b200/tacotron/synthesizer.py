@@ -1,4 +1,4 @@
-"""`Synthesizer` with the reference's surface (tacotron_synthesize.py:38-127), computed on the B200.
+"""`Synthesizer` with the reference's surface (tacotron_synthesize.py:38-127), computed on the GPU.
 
     synth = Synthesizer(); synth.load('logs-Tacotron-2/taco_pretrained', symbols=...)
     mel_path = synth.synthesize('m ao2 h a2 ...', out_dir, idx, step)      # writes step-{step}-{idx}-mel-pred.npy

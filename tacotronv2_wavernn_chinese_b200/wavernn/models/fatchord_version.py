@@ -1,4 +1,4 @@
-"""`WaveRNN` / `UpsampleNetwork` with the reference's Python surface, computed on the B200.
+"""`WaveRNN` / `UpsampleNetwork` with the reference's Python surface, computed on the GPU.
 
 Mirrors lturing/tacotronv2_wavernn_chinese `wavernn/models/fatchord_version.py`:
 constructor arguments (:93-95), `load` (:414), `save` (:419), `get_step` (:407),
@@ -125,12 +125,12 @@ class WaveRNN(nn.Module):
     def _engine_for_current_weights(self, device=None) -> WaveRNNEngine:
         """(Re)packs the weights into a libb200tts context when they changed since the last call."""
         if self.mode != 'RAW':
-            raise NotImplementedError("only voc_mode='RAW' is on the B200 path (the shipped model, wavernn_hparams.py:35)")
+            raise NotImplementedError("only voc_mode='RAW' is on the GPU path (the shipped model, wavernn_hparams.py:35)")
         p = next(self.parameters())
         dev = device if device is not None else (p.device.index if p.is_cuda else torch.cuda.current_device()
                                                  if torch.cuda.is_available() else None)
         if dev is None:
-            raise RuntimeError('no CUDA device: the B200 WaveRNN path has no CPU fallback')
+            raise RuntimeError('no CUDA device: the WaveRNN path has no CPU fallback')
         key = (dev, self._weights_key())
         if self._engine is None or self._engine_key != key:
             if self._engine is not None:
@@ -141,7 +141,7 @@ class WaveRNN(nn.Module):
 
     def forward(self, x, mels):
         raise NotImplementedError('WaveRNN.forward is the teacher-forced TRAINING path (fatchord_version.py:131-167), '
-                                  'out of scope for the B200 generation build; use generate()')
+                                  'out of scope for the CUDA generation build; use generate()')
 
     def generate(self, mels, save_path: Union[str, Path, None], batched, target, overlap, mu_law,
                  seed=None, kernel='auto', return_all=False):

@@ -9,8 +9,8 @@ if ROOT not in sys.path:
 
 
 def pytest_configure(config):
-    config.addinivalue_line('markers', 'gpu: needs a real B200 (run with -m gpu on the GPU box)')
-    config.addinivalue_line('markers', 'reference: needs /root/reference (build container only)')
+    config.addinivalue_line('markers', 'gpu: needs a real H100 (run with -m gpu)')
+    config.addinivalue_line('markers', 'reference: needs the reference checkout')
 
 
 @pytest.fixture(scope='session', autouse=True)

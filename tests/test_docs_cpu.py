@@ -1,4 +1,4 @@
-"""Every file the documents cite as evidence exists in the tree (profiles/ summaries, tools, fixtures, generators)."""
+"""Every file the documents cite as evidence exists in the tree (tools, fixtures, generators, sources)."""
 import os
 import re
 
@@ -6,21 +6,18 @@ import pytest
 
 from conftest import ROOT
 
-DOCS = ['DESIGN.md', 'README.md', 'INTEGRATION.md', 'profiles/README.md', 'tools/README.md']
+DOCS = ['DESIGN.md', 'README.md', 'INTEGRATION.md', 'tools/README.md']
 PATH = re.compile(r'`((?:profiles|tools|tests|oracle|include|tacotronv2_wavernn_chinese_b200)/[A-Za-z0-9_./\-]+'
                   r'\.(?:txt|json|csv|py|cu|cuh|h|npz|md|sh))`')
-BARE = re.compile(r'`(r0[0-9]_[A-Za-z0-9_.\-]+\.(?:txt|json|csv))`')
 
 
 @pytest.mark.parametrize('doc', DOCS)
 def test_cited_files_exist(doc):
     text = open(os.path.join(ROOT, doc), encoding='utf-8').read()
     cited = set(PATH.findall(text))
-    if doc.startswith('profiles/'):
-        cited |= {'profiles/' + m for m in BARE.findall(text)}
     missing = sorted(p for p in cited if not os.path.exists(os.path.join(ROOT, p)))
     assert not missing, missing
-    if doc in ('DESIGN.md', 'profiles/README.md'):
+    if doc == 'DESIGN.md':
         assert len(cited) >= 20          # the pattern still finds the citations
 
 

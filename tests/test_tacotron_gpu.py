@@ -1,4 +1,4 @@
-"""sm_100a Tacotron-2 decoder loop (taco_decoder_kernel, through the C ABI) against the oracle with shared dropout masks.
+"""sm_90a Tacotron-2 decoder loop (taco_decoder_kernel, through the C ABI) against the oracle with shared dropout masks.
 The oracle's decoder step AND its whole 405-step run of config 4 are pinned against the reference's serialized graph
 (tests/test_tacotron_step_pins.py, tests/test_tacotron_run_pins.py; see oracle/tacotron_oracle.py).  Tolerance from the north star: mel within 1e-4 abs, identical stop step."""
 import numpy as np
@@ -70,7 +70,7 @@ def test_single_sentence_grid_decoder_vs_oracle_synthetic_weights(window):
 
 HORIZON = 60     # steps over which fp32 evaluations of the shipped checkpoint still agree to 1e-4 (CPU test
                  # test_real_checkpoint_decoder_is_chaotic: fp32-vs-fp64 ORACLE error 2e-5 @80, 3.5e-4 @120, O(1) by 300;
-                 # measured on B200, tools/taco_err_profile.py: kernel-vs-fp64 <= 3.4e-5 to step 60, 5e-4 @79, 3.8e-4 @150)
+                 # measured on an earlier GPU with tools/taco_err_profile.py: kernel-vs-fp64 <= 3.4e-5 to step 60, 5e-4 @79, 3.8e-4 @150)
 HORIZON2 = 150   # ... and to 1e-2 (frame magnitudes ~7)
 
 

@@ -1,4 +1,4 @@
-"""Parity of the sm_100a WaveRNN path against the oracle and the reference-generated goldens.
+"""Parity of the sm_90a WaveRNN path against the oracle and the reference-generated goldens.
 Everything here calls the CUDA kernels through the C ABI (engine.WaveRNNEngine -> libb200tts.so)."""
 import os
 
@@ -334,7 +334,7 @@ TC_BATCHES = [256, 200, 128, 100, 40]
 
 @pytest.mark.parametrize('B', TC_BATCHES)
 def test_tc_teacher_forced_logits_vs_oracle(torch_cuda, B):
-    """The split-fp16 tcgen05 kernel to the SAME bar as the fp32 CUDA-core mappings: all rows, 300 steps, shipped checkpoint."""
+    """The split-fp16 wgmma kernel to the SAME bar as the fp32 CUDA-core mappings: all rows, 300 steps, shipped checkpoint."""
     test_mapping_teacher_forced_logits_vs_oracle(torch_cuda, B, kernel='tc')
 
 
@@ -451,7 +451,7 @@ def test_large_request_is_cut_into_row_ranges(torch_cuda):
 
 
 def test_auto_dispatch_and_slicing_through_the_tensor_core_kernel(torch_cuda):
-    """kernel='auto': 161-256 rows run wavernn_tc_kernel; more than 256 rows are cut into launches of 256 rows (tensor-core pipeline)
+    """kernel='auto': 129-256 rows run wavernn_tc_kernel; more than 256 rows are cut into launches of 256 rows (tensor-core pipeline)
     plus a tail on the CUDA-core kernels.  The noise is keyed by the global row, so every range equals the same rows generated by
     hand; a row's arithmetic in the tensor-core kernel does not depend on its batch (bit-equal against a 200-row launch)."""
     eng, _ = engine_for('ckpt')

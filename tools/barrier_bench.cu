@@ -1,6 +1,6 @@
-// Microbenchmark: cost of one grid-wide barrier on B200 for several protocols, with and without a payload
+// Microbenchmark: cost of one grid-wide barrier for several protocols, with and without a payload
 // (each CTA writes P floats before the barrier and reads 128*P floats after it, like one layer of the grid kernel).
-// Development aid, not product code.   nvcc -gencode arch=compute_100a,code=sm_100a -O3 -o tools/barrier_bench.bin tools/barrier_bench.cu
+// Development aid, not product code.   nvcc -gencode arch=compute_90a,code=sm_90a -O3 -o tools/barrier_bench.bin tools/barrier_bench.cu
 #include <cooperative_groups.h>
 #include <cstdio>
 #include <cstdlib>
@@ -75,7 +75,7 @@ __global__ void chase(const unsigned* next, int iters, unsigned* out, long long*
 
 template <int FLAVOR>
 float run(int ncta, int iters, int payload, unsigned* ctr, unsigned* flags, float* buf, float* sink) {
-  cudaMemset(ctr, 0, 256); cudaMemset(flags, 0, 148 * 128);
+  cudaMemset(ctr, 0, 256); cudaMemset(flags, 0, 132 * 128);
   void* args[] = {&ctr, &flags, &buf, &iters, &payload, &sink};
   cudaEvent_t e0, e1; cudaEventCreate(&e0); cudaEventCreate(&e1);
   cudaEventRecord(e0);
@@ -90,8 +90,8 @@ float run(int ncta, int iters, int payload, unsigned* ctr, unsigned* flags, floa
 int main(int argc, char** argv) {
   int iters = argc > 1 ? atoi(argv[1]) : 20000;
   unsigned *ctr, *flags; float *buf, *sink;
-  cudaMalloc(&ctr, 256); cudaMalloc(&flags, 148 * 128); cudaMalloc(&buf, 2 * 148 * 4096 * sizeof(float)); cudaMalloc(&sink, 4);
-  cudaMemset(buf, 0, 2 * 148 * 4096 * sizeof(float));
+  cudaMalloc(&ctr, 256); cudaMalloc(&flags, 132 * 128); cudaMalloc(&buf, 2 * 132 * 4096 * sizeof(float)); cudaMalloc(&sink, 4);
+  cudaMemset(buf, 0, 2 * 132 * 4096 * sizeof(float));
   // L2 latency (pointer chase over 8 MB, stride 4 KB+)
   {
     const int n = 1 << 21; unsigned* h = (unsigned*)malloc(n * 4);
@@ -104,7 +104,7 @@ int main(int argc, char** argv) {
   }
   const char* names[] = {"red.release+ld.acquire", "fence+atomicAdd+volatile+fence", "fence+red.relaxed+ld.relaxed+fence",
                          "cg::grid.sync", "flag/CTA 128B apart", "flag/CTA packed"};
-  for (int ncta : {128, 148})
+  for (int ncta : {128, 132})
     for (int payload : {0, 4, 1024}) {
       printf("ncta=%d payload=%d floats/CTA:", ncta, payload);
       float r[6];

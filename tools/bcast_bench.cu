@@ -1,6 +1,6 @@
 // Microbenchmark: every CTA of a 128-CTA grid reads the SAME 512 KB matrix ([512 k][256 u] fp32, one layer's activations)
 // from L2, the access pattern of the grid kernel.  Variants: loads in flight, traversal order, TMA bulk copies.
-// Development aid.  nvcc -gencode arch=compute_100a,code=sm_100a -O3 -o tools/bcast_bench.bin tools/bcast_bench.cu
+// Development aid.  nvcc -gencode arch=compute_90a,code=sm_90a -O3 -o tools/bcast_bench.bin tools/bcast_bench.cu
 #include <cstdio>
 #include <cstdlib>
 #include <cstdint>
@@ -96,7 +96,7 @@ int main(int argc, char** argv) {
   char* buf; float* sink;
   cudaMalloc(&buf, 4 * 512 * 1024); cudaMemset(buf, 0, 4 * 512 * 1024); cudaMalloc(&sink, 4);
   const float4* b4 = (const float4*)buf;
-  for (int ncta : {1, 16, 128, 148}) {
+  for (int ncta : {1, 16, 128, 132}) {
     printf("ncta=%d: us per 512 KB read by every CTA  (GB/s per SM)\n", ncta);
 #define RUN_LDG(U, S) { float us = time_it([&] { read_ldg<U, S><<<ncta, 256>>>(b4, reps, sink); }, reps); printf("   ldg unroll=%-2d stagger=%d : %7.2f us  (%6.1f GB/s)\n", U, (int)S, us, 0.524288 / us * 1e3); }
     RUN_LDG(4, false) RUN_LDG(4, true) RUN_LDG(8, false) RUN_LDG(8, true) RUN_LDG(16, false) RUN_LDG(16, true) RUN_LDG(32, true)

@@ -1,9 +1,8 @@
 // Development aid (tools/README.md): how fast can ONE SM pull a 256 KB image out of L2 into shared memory?
-// The tensor-core step kernel (csrc/wavernn_tc.cuh) measured ~20 bytes per clock and SM for its activation images whatever
-// moved them; this isolates the data path: a writer kernel leaves the buffer dirty in L2 (written by other SMs), then G
+// The tensor-core step kernel (csrc/wavernn_tc.cuh) streams its activation images this way; this isolates the data path: a writer kernel leaves the buffer dirty in L2 (written by other SMs), then G
 // reader CTAs stream it (a) with cp.async.bulk through a ring of 16 KB stages and mbarriers, no MMA, (b) with ld.global.cg by
-// 512 threads.  Prints cycles per 256 KB and bytes per clock for G = 1, 16, 64 readers.
-//   nvcc -gencode arch=compute_100a,code=sm_100a -O3 -o tools/bulk_stream_bench.bin tools/bulk_stream_bench.cu
+// 512 threads.  Prints cycles per 256 KB and bytes per clock for G = 1, 16, 64, 128 readers.
+//   nvcc -gencode arch=compute_90a,code=sm_90a -O3 -o tools/bulk_stream_bench.bin tools/bulk_stream_bench.cu
 #include <cstdio>
 #include <cstdint>
 #include <cuda_runtime.h>
@@ -71,7 +70,7 @@ int main() {
   cudaFuncSetAttribute(reader_bulk<8>, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)smem);
   cudaFuncSetAttribute(reader_bulk<4>, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)smem);
   cudaFuncSetAttribute(reader_ldg, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)smem);
-  for (int G : {1, 16, 64, 144}) {
+  for (int G : {1, 16, 64, 128}) {
     for (int mode = 0; mode < 3; ++mode) {
       writer<<<64, 256>>>((uint4*)buf, kBytes / 16);
       if (mode == 0) reader_bulk<8><<<G, 128, smem>>>(buf, reps, cyc);

@@ -1,5 +1,5 @@
 // Microbenchmark of the all-to-all activation exchange of the push kernel (wavernn_push.cuh), in isolation.
-//   nvcc -gencode arch=compute_100a,code=sm_100a -O3 -std=c++17 -o tools/exchange_bench.bin tools/exchange_bench.cu
+//   nvcc -gencode arch=compute_90a,code=sm_90a -O3 -std=c++17 -o tools/exchange_bench.bin tools/exchange_bench.cu
 // 128 co-resident CTAs x 512 threads.  One "exchange": every CTA publishes 4*G floats (G rows x 4 units), then every
 // thread of every CTA must obtain the float4s it owns in the 128 x G x 4 vector (G/4 per thread), then a block barrier.
 // Reports SM cycles per exchange for several protocols:

@@ -1,13 +1,19 @@
 // Cost model of the grid kernel's inner loop on one SM (development aid, see tools/README.md).
-//   nvcc -gencode arch=compute_100a,code=sm_100a -O3 -o build_ab/fma_tile_bench tools/fma_tile_bench.cu
+//   nvcc -gencode arch=compute_90a,code=sm_90a -O3 -o build_ab/fma_tile_bench tools/fma_tile_bench.cu
 // A thread owns a U x RT register tile and runs `iters` blocks of 4 k-steps (4*U*RT FMAs), 16 warps per CTA, one CTA
 // per SM.  MODE 0: operands stay in registers (pure FMA-pipe rate).  MODE 1: weights re-read from shared memory every
 // block (LDS.128, warp-broadcast), activations in registers.  MODE 2: weights from shared memory AND activations from a
 // 512 KB L2-resident matrix (ld.global.cg 128-bit), i.e. the real loop without the barriers.  PACK 0: scalar FFMA,
-// PACK 1: FFMA2 (two utterances per instruction, weight broadcast).  Prints FMA per clock per SM.
+// PACK 1: pairs of utterances against one weight register (fma2_rn below: two
+// scalar FFMAs on Hopper, which has no packed fp32 FMA).  Prints FMA per clock per SM.
 #include <cstdio>
 #include <cstdlib>
 #include <cuda_runtime.h>
+
+// same helper as csrc/common.cuh (this tool is compiled on its own)
+__device__ __forceinline__ float2 fma2_rn(float2 a, float2 b, float2 c) {
+  return make_float2(__fmaf_rn(a.x, b.x, c.x), __fmaf_rn(a.y, b.y, c.y));
+}
 
 template <int U, int RT, int PACK>
 __device__ __forceinline__ void fma_block(float (&acc)[RT][U], const float4 (&w)[RT], const float (&a)[4][U]) {
@@ -17,10 +23,10 @@ __device__ __forceinline__ void fma_block(float (&acc)[RT][U], const float4 (&w)
 #pragma unroll
       for (int u = 0; u < U; u += 2) {
         float2 s = make_float2(acc[r][u], acc[r][u + 1]);
-        s = __ffma2_rn(make_float2(a[0][u], a[0][u + 1]), make_float2(w[r].x, w[r].x), s);
-        s = __ffma2_rn(make_float2(a[1][u], a[1][u + 1]), make_float2(w[r].y, w[r].y), s);
-        s = __ffma2_rn(make_float2(a[2][u], a[2][u + 1]), make_float2(w[r].z, w[r].z), s);
-        s = __ffma2_rn(make_float2(a[3][u], a[3][u + 1]), make_float2(w[r].w, w[r].w), s);
+        s = fma2_rn(make_float2(a[0][u], a[0][u + 1]), make_float2(w[r].x, w[r].x), s);
+        s = fma2_rn(make_float2(a[1][u], a[1][u + 1]), make_float2(w[r].y, w[r].y), s);
+        s = fma2_rn(make_float2(a[2][u], a[2][u + 1]), make_float2(w[r].z, w[r].z), s);
+        s = fma2_rn(make_float2(a[3][u], a[3][u + 1]), make_float2(w[r].w, w[r].w), s);
         acc[r][u] = s.x; acc[r][u + 1] = s.y;
       }
     } else {

@@ -6,7 +6,7 @@ from tacotronv2_wavernn_chinese_b200 import synth
 from tacotronv2_wavernn_chinese_b200.engine import WaveRNNEngine
 
 kernels = sys.argv[1].split(',') if len(sys.argv) > 1 else ['utterance']
-batches = [int(x) for x in sys.argv[2].split(',')] if len(sys.argv) > 2 else [1, 148, 256]
+batches = [int(x) for x in sys.argv[2].split(',')] if len(sys.argv) > 2 else [1, 132, 256]
 steps = int(sys.argv[3]) if len(sys.argv) > 3 else 2000
 eng = WaveRNNEngine(synth.synth_state_dict(0), synth.DEFAULT_DIMS, device=0)
 for k in kernels:

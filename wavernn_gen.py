@@ -1,5 +1,5 @@
 #!/usr/bin/env python
-"""Vocode a mel `.npy` with WaveRNN on a B200 -- drop-in for the reference's `wavernn_gen.py`.
+"""Vocode a mel `.npy` with WaveRNN on an H100 -- drop-in for the reference's `wavernn_gen.py`.
 
 Same command line (reference wavernn_gen.py:49-61), same input contract (float32 `(T, 80)` mel in [0, 1], :22-28), same
 output name `./wavernn_inference_output/{stem}_gen_NOT_BATCHED_step={k}k.wav` (:35-39, :124).  Deliberate differences:
@@ -79,7 +79,7 @@ def build_model():
 
 
 def main(argv=None):
-    parser = argparse.ArgumentParser(description='WaveRNN vocoder on B200')
+    parser = argparse.ArgumentParser(description='WaveRNN vocoder on H100')
     for flags, kw in CLI:
         parser.add_argument(*flags, **kw)
     parser.set_defaults(batched=None)
@@ -90,9 +90,9 @@ def main(argv=None):
     overlap = args.overlap if args.overlap is not None else hp.voc_overlap
     batched = hp.voc_gen_batched if args.batched is None else args.batched
     if args.force_cpu:
-        raise SystemExit('--force_cpu: this build runs the generation loop on sm_100a only; there is no CPU fallback')
+        raise SystemExit('--force_cpu: this build runs the generation loop on sm_90a only; there is no CPU fallback')
     if not torch.cuda.is_available():
-        raise SystemExit('no CUDA device visible; the B200 WaveRNN path has no CPU fallback')
+        raise SystemExit('no CUDA device visible; the WaveRNN path has no CPU fallback')
     print('Using device:', torch.device('cuda'))
     print('\nInitialising Model...\n')
     model = build_model()

@@ -22,7 +22,7 @@ mu_law = True                     # labels are mu-law companded
 peak_norm = True
 
 # --- vocoder architecture ---------------------------------------------------------------------------
-voc_mode = 'RAW'                  # 'RAW' = softmax over 2**bits labels (the only mode on the B200 path); 'MOL' unsupported
+voc_mode = 'RAW'                  # 'RAW' = softmax over 2**bits labels (the only mode on the GPU path); 'MOL' unsupported
 voc_upsample_factors = (5, 5, 11) # product must equal hop_length
 voc_rnn_dims = 512
 voc_fc_dims = 512
