@@ -13,6 +13,7 @@
  *                                 incl. decode_mu_law                   wavernn/utils/dsp.py:98-103
  *   b200tts_wavernn_generate_host  same, HOST buffers in/out (what wavernn_gen.py:41 sees end to end)
  *   gen_opts.fold_target/_overlap  <- fold_with_overlap + xfade_and_unfold  fatchord_version.py:293-405 (--batched)
+ *   b200tts_griffin_lim        <- audio.inv_mel_spectrogram (Griffin-Lim) tacotron/datasets/audio.py:122-137, :176-210
  *
  * Conventions
  *   - plain C types only; no torch / CUDA types in any signature (`stream` is a cudaStream_t passed as void*).
@@ -234,6 +235,59 @@ int b200tts_taco_postnet(b200tts_taco* ctx, const float* d_frames, const int32_t
 /* The keep flags the PHILOX dropout mode draws: d_masks [B][steps][2][prenet_units]. */
 int b200tts_taco_philox_masks(int device, uint64_t seed, uint64_t utterance_offset, int B, int steps, int prenet_units,
                               uint8_t* d_masks, void* stream);
+
+/* ------------------------------------------------------------------------------------------------------------------
+ * Griffin-Lim mel inversion (the preview wav of tacotron_synthesize.py:110-112).
+ *   b200tts_griffin_lim  <- audio.inv_mel_spectrogram(mel.T, hparams)  tacotron/datasets/audio.py:122-137
+ *                           = _denormalize :297-309, _db_to_amp :277-278, _mel_to_linear :256-260, _griffin_lim :176-186,
+ *                           _stft / _istft (librosa 0.7.2 stft / istft) :203-210, inv_preemphasis :52-55
+ * Symmetric mels clipped to +-max_abs_value (signal_normalization, allow_clipping_in_normalization) and librosa's stft with
+ * center=True and constant padding are assumed.  T frames give exactly hop * (T - 1) samples.
+ * ------------------------------------------------------------------------------------------------------------------ */
+typedef struct {
+  int32_t n_fft;            /* 2048 (the only size implemented)  */
+  int32_t hop_size;         /* 275                               */
+  int32_t win_size;         /* 1100 (<= n_fft), periodic Hann    */
+  int32_t num_mels;         /* 80 (<= 128)                       */
+  float max_abs_value;      /* 4                                 */
+  float min_level_db;       /* -100                              */
+  float ref_level_db;       /* 20                                */
+  float magnitude_power;    /* 2                                 */
+  float power;              /* 1.5                               */
+  float preemphasis;        /* 0.97; 0 when preemphasize is off  */
+} b200tts_gl_cfg;
+
+enum { B200TTS_GL_PHASE_PHILOX = 0, B200TTS_GL_PHASE_EXT = 1 };
+/* Initial phase e^{2 pi i u} of _griffin_lim (:181, np.random.rand): u from Philox4x32-10 keyed by (seed, utterance_offset + row,
+ * frame, bin), or read from d_u[B][T_max][n_fft/2 + 1] (EXT; tests share the phase with the oracle). */
+typedef struct {
+  int32_t mode;
+  uint64_t seed;
+  uint64_t utterance_offset;
+  const float* d_u;
+} b200tts_gl_phase;
+
+typedef struct b200tts_gl b200tts_gl;
+
+/* h_inv_mel_basis [n_fft/2 + 1][num_mels]: pinv of the mel filterbank (librosa.filters.mel(sample_rate, n_fft, num_mels, fmin,
+ * fmax), _build_mel_basis :268-271), computed by the caller (in float64) and rounded to fp32. */
+int b200tts_gl_create(b200tts_gl** out, int device, const b200tts_gl_cfg* cfg, const float* h_inv_mel_basis);
+void b200tts_gl_destroy(b200tts_gl* ctx);
+
+/* d_mel [B][T_max][num_mels] (frames x mels, the decoder's layout) -> d_wave [B][hop * (T_max - 1)] float32 after n_iters
+ * iterations.  d_frames [B] (may be NULL = T_max for every row): true frame count of each row of a zero-padded ragged batch;
+ * row b is then computed exactly as a stand-alone run of d_frames[b] frames and is zero from hop * (d_frames[b] - 1) on (values
+ * above T_max count as T_max; rows with fewer than 2 frames come back all zero).  d_u_out [B][T_max][n_fft/2 + 1] (may be NULL):
+ * the phase, as angle / 2 pi mod 1, of the last stft (of `init` when n_iters = 0) -- with init = EXT and n_iters = 1 this
+ * teacher-forces a single iteration.  Rows beyond a row's frame count are left untouched in d_u_out. */
+int b200tts_griffin_lim(b200tts_gl* ctx, const float* d_mel, const int32_t* d_frames, int B, int T_max, const b200tts_gl_phase* init,
+                        int n_iters, float* d_wave, float* d_u_out, void* stream);
+
+/* The uniforms the PHILOX phase mode draws: d_u[B][T][n_bins]. */
+int b200tts_gl_philox_uniform(int device, uint64_t seed, uint64_t utterance_offset, int B, int T, int n_bins, float* d_u, void* stream);
+
+/* Number of kernel launches issued on this context since creation. */
+int64_t b200tts_gl_launch_count(const b200tts_gl* ctx);
 
 /* Debug aid: mean SM cycles per CTA spent in {compute, barrier} of each of the 6 phases of the last grid-kernel
  * launch; only recorded when the environment variable B200TTS_GRID_PROF is set while generating. */

@@ -30,6 +30,9 @@ hparams = HParams(
     # audio / mel scaling
     num_mels=80, sample_rate=22050, hop_size=275, win_size=1100,
     max_abs_value=4.0, symmetric_mels=True, clip_outputs=True, lower_bound_decay=0.1,
+    # Griffin-Lim mel inversion (tacotron/datasets/audio.py:122-137, :176-186 there; tacotron_synthesize.py --griffin_lim)
+    n_fft=2048, fmin=95, fmax=7600, min_level_db=-100, ref_level_db=20, magnitude_power=2., power=1.5, griffin_lim_iters=60,
+    preemphasize=True, preemphasis=0.97, signal_normalization=True, allow_clipping_in_normalization=True,
     # model
     outputs_per_step=1, stop_at_any=True, batch_norm_position='after',
     embedding_dim=128,

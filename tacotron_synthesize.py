@@ -11,9 +11,12 @@ clip((mel + 4) / 8, 0, 1) (reference :114-116, :187-191), which `wavernn_gen.py 
     public dictionaries, checked string-for-string against the reference on 300 train.txt lines).  Space separated pinyin
     tokens pass through it unchanged, so the round-1 form `--text 'm ao2 h a2 ...'` keeps working.
   * no PNG plots (the alignment is saved as `...-align.npy` instead).  The preview wav `step-{step}-{idx}-wav-from-mel.wav`
-    (:110-112) is written only when `--voc_weights` names a WaveRNN checkpoint: it is vocoded by WaveRNN on the GPU in the same
-    process (Griffin-Lim feature inversion is out of scope) and saved through the reference's own writer chain -- DC notch,
-    peak normalisation, int16 (`tacotron/datasets/audio.py:17-34`, restated in tacotronv2_wavernn_chinese_b200/tacotron/audio.py).
+    (:110-112) is written on request, by one of two vocoders on the GPU in the same process:
+      --griffin_lim         the reference's own: Griffin-Lim mel inversion (`audio.inv_mel_spectrogram`, hparams.griffin_lim_iters
+                            iterations; the random initial phase is Philox(--seed)), needs only the Tacotron checkpoint;
+      --voc_weights PATH    WaveRNN from that checkpoint.
+    Either way it is saved through the reference's own writer chain -- DC notch, peak normalisation, int16
+    (`tacotron/datasets/audio.py:17-34`, restated in tacotronv2_wavernn_chinese_b200/tacotron/audio.py).
 """
 from __future__ import annotations
 
@@ -46,6 +49,18 @@ def preview_wav(mel_path, voc_weights, voc_hp_file, sample_rate, seed=0):
     return wav_path
 
 
+def preview_wav_griffin_lim(mel_path, hp, seed=0):
+    """mel `.npy` -> `...-wav-from-mel.wav` next to it by Griffin-Lim (reference :110-112).  The saved array is
+    clip((mel + 4) / 8, 0, 1), so the mel is taken back as npy * 8 - 4."""
+    import numpy as np
+    from tacotronv2_wavernn_chinese_b200.tacotron import audio
+    mel = np.load(mel_path).astype(np.float32) * (2 * hp.max_abs_value) - hp.max_abs_value     # (T, 80)
+    wav = audio.inv_mel_spectrogram(mel.T, hp, seed=seed)
+    wav_path = mel_path[:-len('mel-pred.npy')] + 'wav-from-mel.wav'
+    audio.save_wav(wav, wav_path, sr=hp.sample_rate)
+    return wav_path
+
+
 def main(argv=None):
     ap = argparse.ArgumentParser()
     ap.add_argument('--text', required=True, help='Hanzi sentence (or space separated pinyin tokens)')
@@ -57,7 +72,10 @@ def main(argv=None):
     ap.add_argument('--seed', type=int, default=0, help='Philox seed of the (always on) prenet dropout')
     ap.add_argument('--voc_weights', default=None, help='WaveRNN checkpoint: also write the preview wav step-..-wav-from-mel.wav')
     ap.add_argument('--voc_hp_file', default='wavernn_hparams.py', help='WaveRNN hyper-parameter file (with --voc_weights)')
+    ap.add_argument('--griffin_lim', action='store_true', help='also write the preview wav step-..-wav-from-mel.wav by Griffin-Lim')
     args = ap.parse_args(argv)
+    if args.griffin_lim and args.voc_weights:
+        ap.error('--griffin_lim and --voc_weights both choose the preview vocoder; give one')
     hp = hparams.parse(args.hparams)
     from tacotronv2_wavernn_chinese_b200.tacotron.pinyin import get_pyin
     pyin, text = get_pyin(args.text)                    # reference :187: pinyin feeds the model, the normalised text names the files
@@ -72,6 +90,8 @@ def main(argv=None):
     print(f'pred_mel_path: {mel_path}')
     if args.voc_weights:
         print(f'wav_path: {preview_wav(mel_path, args.voc_weights, args.voc_hp_file, hp.sample_rate, args.seed)}')
+    elif args.griffin_lim:
+        print(f'wav_path: {preview_wav_griffin_lim(mel_path, hp, args.seed)}')
     print(f'last: {time.time() - t0} seconds')
     return mel_path
 

@@ -57,6 +57,18 @@ class TacoDropout(C.Structure):
     _fields_ = [('mode', C.c_int32), ('seed', C.c_uint64), ('utterance_offset', C.c_uint64), ('d_masks', C.c_void_p)]
 
 
+class GlCfg(C.Structure):
+    _fields_ = [('n_fft', C.c_int32), ('hop_size', C.c_int32), ('win_size', C.c_int32), ('num_mels', C.c_int32),
+                ('max_abs_value', C.c_float), ('min_level_db', C.c_float), ('ref_level_db', C.c_float),
+                ('magnitude_power', C.c_float), ('power', C.c_float), ('preemphasis', C.c_float)]
+
+
+class GlPhase(C.Structure):
+    _fields_ = [('mode', C.c_int32), ('seed', C.c_uint64), ('utterance_offset', C.c_uint64), ('d_u', C.c_void_p)]
+
+
+GL_PHASE_PHILOX, GL_PHASE_EXT = 0, 1
+
 # every symbol include/b200tts.h declares: (restype, argtypes)
 SIGNATURES = {
     'b200tts_abi_version': (C.c_int, []),
@@ -89,6 +101,12 @@ SIGNATURES = {
     'b200tts_taco_encode': (C.c_int, [C.c_void_p, C.c_void_p, C.c_void_p, C.c_int, C.c_int, C.c_void_p, C.c_void_p]),
     'b200tts_taco_postnet': (C.c_int, [C.c_void_p, C.c_void_p, C.c_void_p, C.c_int, C.c_int, C.c_void_p, C.c_void_p]),
     'b200tts_taco_philox_masks': (C.c_int, [C.c_int, C.c_uint64, C.c_uint64, C.c_int, C.c_int, C.c_int, C.c_void_p, C.c_void_p]),
+    'b200tts_gl_create': (C.c_int, [C.POINTER(C.c_void_p), C.c_int, C.POINTER(GlCfg), C.c_void_p]),
+    'b200tts_gl_destroy': (None, [C.c_void_p]),
+    'b200tts_griffin_lim': (C.c_int, [C.c_void_p, C.c_void_p, C.c_void_p, C.c_int, C.c_int, C.POINTER(GlPhase), C.c_int, C.c_void_p,
+                                      C.c_void_p, C.c_void_p]),
+    'b200tts_gl_philox_uniform': (C.c_int, [C.c_int, C.c_uint64, C.c_uint64, C.c_int, C.c_int, C.c_int, C.c_void_p, C.c_void_p]),
+    'b200tts_gl_launch_count': (C.c_int64, [C.c_void_p]),
 }
 
 _lib = None

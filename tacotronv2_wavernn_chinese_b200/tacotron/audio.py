@@ -8,9 +8,19 @@ What the chain does to a float waveform, in order:
   3. soften the dynamics: sign(x) |x|^0.95 (the `f1` gain of :29 cancels in step 4);
   4. scale the peak to 32767 (never by more than 32767 / 0.01) and truncate towards zero to int16.
 
-Here the preview wav is vocoded by WaveRNN instead of Griffin-Lim (feature inversion is out of scope); the writer is the same.
+The preview wav comes either from WaveRNN or, like the reference's, from Griffin-Lim mel inversion (`inv_mel_spectrogram`,
+audio.py:122-137, on the GPU through libb200tts); the writer is the same.
+
+Griffin-Lim (what `inv_mel_spectrogram` computes, T frames -> 275 (T - 1) samples):
+  1. denormalise the symmetric mel: D = (clip(mel, -4, 4) + 4) * 100 / 8 - 100                       (_denormalize :297-309)
+  2. S = max(1e-10, pinv(M) . (10 ** ((D + 20) / 20)) ** (1/2)) ** 1.5, M the Slaney mel filterbank      (_mel_to_linear :256-260)
+  3. 60 Griffin-Lim iterations from a uniform random phase, librosa 0.7.2 stft / istft                  (_griffin_lim :176-186)
+  4. lfilter([1], [1, -0.97])                                                                           (inv_preemphasis :52-55)
+The random phase is Philox(seed) keyed by (utterance, frame, bin) instead of numpy's global generator.
 """
 from __future__ import annotations
+
+import functools
 
 import numpy as np
 
@@ -49,3 +59,81 @@ def save_wav(wav, path, sr):
     """Write `wav` (float, any scale) as a 16-bit PCM file at `sr` Hz the way the reference's `audio.save_wav` does."""
     from scipy.io import wavfile
     wavfile.write(str(path), int(sr), to_int16(wav))
+
+
+# ---- Griffin-Lim mel inversion ----------------------------------------------------------------------------------------
+def _hz_to_mel(f):
+    """librosa 0.7.2 hz_to_mel (htk=False): linear below 1 kHz, logarithmic above (Slaney's Auditory Toolbox)."""
+    f = np.asanyarray(f, dtype=np.float64)
+    f_sp, min_log_hz = 200.0 / 3, 1000.0
+    logstep = np.log(6.4) / 27.0
+    return np.where(f >= min_log_hz, min_log_hz / f_sp + np.log(np.maximum(f, min_log_hz) / min_log_hz) / logstep, f / f_sp)
+
+
+def _mel_to_hz(m):
+    m = np.asanyarray(m, dtype=np.float64)
+    f_sp, min_log_hz = 200.0 / 3, 1000.0
+    min_log_mel, logstep = min_log_hz / f_sp, np.log(6.4) / 27.0
+    return np.where(m >= min_log_mel, min_log_hz * np.exp(logstep * (m - min_log_mel)), f_sp * m)
+
+
+def mel_filterbank(sr, n_fft, n_mels, fmin, fmax):
+    """[n_mels][1 + n_fft/2] float64: librosa 0.7.2 filters.mel(sr, n_fft, n_mels, fmin, fmax) (Slaney scale, each triangle
+    normalised to unit area, norm=1), the `_build_mel_basis` of audio.py:268-271."""
+    fftfreqs = np.linspace(0, float(sr) / 2, int(1 + n_fft // 2), endpoint=True)
+    mel_f = _mel_to_hz(np.linspace(_hz_to_mel(fmin), _hz_to_mel(fmax), n_mels + 2))
+    fdiff = np.diff(mel_f)
+    ramps = np.subtract.outer(mel_f, fftfreqs)
+    w = np.maximum(0, np.minimum(-ramps[:n_mels] / fdiff[:n_mels, None], ramps[2:] / fdiff[1:, None]))
+    return w * (2.0 / (mel_f[2:n_mels + 2] - mel_f[:n_mels]))[:, None]
+
+
+@functools.lru_cache(maxsize=4)
+def _inv_mel_basis(sr, n_fft, n_mels, fmin, fmax):
+    b = np.linalg.pinv(mel_filterbank(sr, n_fft, n_mels, fmin, fmax))
+    b.flags.writeable = False
+    return b
+
+
+def inv_mel_basis(hparams):
+    """np.linalg.pinv of the filterbank in float64, [1 + n_fft/2][num_mels] (`_inv_mel_basis` of audio.py:256-260)."""
+    assert hparams.fmax <= hparams.sample_rate // 2                     # audio.py:269
+    return _inv_mel_basis(hparams.sample_rate, hparams.n_fft, hparams.num_mels, float(hparams.fmin), float(hparams.fmax))
+
+
+_engines = {}
+
+
+def _engine(hparams, device=None):
+    import torch
+    from .griffin_lim import GriffinLimEngine
+    dev = torch.cuda.current_device() if device is None and torch.cuda.is_available() else device
+    key = (dev, tuple(sorted((k, repr(v)) for k, v in hparams.values().items())))
+    if key not in _engines:
+        _engines[key] = GriffinLimEngine(hparams, device=dev)
+    return _engines[key]
+
+
+def griffin_lim_batch(mels, hparams, seed=0, device=None):
+    """Ragged list of mels [num_mels][T_i] (the layout inv_mel_spectrogram takes) -> list of float32 waves of
+    hop * (T_i - 1) samples, in one GPU launch sequence.  Utterance i draws its initial phase as utterance i of Philox(seed)."""
+    import torch
+    mels = [np.asarray(m, dtype=np.float32) for m in mels]
+    if not mels:
+        return []
+    frames = np.array([m.shape[1] for m in mels], dtype=np.int32)
+    T = int(frames.max())
+    batch = np.zeros((len(mels), T, hparams.num_mels), dtype=np.float32)
+    for i, m in enumerate(mels):
+        batch[i, :m.shape[1]] = m.T
+    eng = _engine(hparams, device)
+    wave = eng.run(batch, frames if (frames != T).any() else None, seed=seed)['wave']
+    with torch.cuda.device(eng.device):
+        wave = wave.cpu().numpy()
+    return [wave[i, :hparams.hop_size * (int(n) - 1)].copy() for i, n in enumerate(frames)]
+
+
+def inv_mel_spectrogram(mel_spectrogram, hparams, seed=0):
+    """The reference's `audio.inv_mel_spectrogram(mel.T, hparams)` (audio.py:122-137): mel [num_mels][T], T >= 2 -> float32 wave
+    of hop * (T - 1) samples, Griffin-Lim with hparams.griffin_lim_iters iterations on the GPU."""
+    return griffin_lim_batch([mel_spectrogram], hparams, seed=seed)[0]

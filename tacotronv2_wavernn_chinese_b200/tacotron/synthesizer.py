@@ -4,8 +4,9 @@
     mel_path = synth.synthesize('m ao2 h a2 ...', out_dir, idx, step)      # writes step-{step}-{idx}-mel-pred.npy
 
 Encoder, decoder loop and postnet all run through libb200tts (b200tts_taco_encode / _decode / _postnet); the checkpoint is
-the reference's TF bundle read without TensorFlow (tacotron/ckpt.py).  Not reproduced: the Griffin-Lim preview wav and the
-matplotlib PNGs the reference also writes (:110-111, :118-125) -- feature extraction / plotting are out of scope.
+the reference's TF bundle read without TensorFlow (tacotron/ckpt.py).  The Griffin-Lim preview wav (:110-112) is written by
+tacotron_synthesize.py --griffin_lim from the saved mel (tacotron/audio.py inv_mel_spectrogram, on the GPU).  Not reproduced:
+the matplotlib PNGs the reference also writes (:111, :118-125) -- plotting is out of scope.
 """
 from __future__ import annotations
 

@@ -1,6 +1,7 @@
 """Signal helpers the generation path touches, with the reference's public names
 (`wavernn/utils/dsp.py`: label_2_float :8, float_2_label :12, save_wav :22, encode_mu_law :92, decode_mu_law :98).
-Feature extraction (STFT / mel / Griffin-Lim) is preprocessing and not part of this package.
+Feature extraction (STFT / mel analysis) is preprocessing and not part of this package; Griffin-Lim mel inversion, the
+Tacotron side's preview vocoder, lives in tacotronv2_wavernn_chinese_b200/tacotron/audio.py.
 
 Conventions (same as the reference): a `bits`-bit label l in [0, 2**bits - 1] maps to the float 2*l/(2**bits - 1) - 1 in
 [-1, 1]; mu-law companding uses mu = n_classes - 1.
