@@ -289,6 +289,55 @@ int b200tts_gl_philox_uniform(int device, uint64_t seed, uint64_t utterance_offs
 /* Number of kernel launches issued on this context since creation. */
 int64_t b200tts_gl_launch_count(const b200tts_gl* ctx);
 
+/* ------------------------------------------------------------------------------------------------------------------
+ * Mel analysis (the reference's feature extraction, tacotron/datasets/preprocessor.py:52-121 _process_utterance_v1).
+ *   flags = 0                               <- audio.melspectrogram(wav, hparams)       tacotron/datasets/audio.py:95-102
+ *   flags = TRIM | PREEMPHASIS | RESCALE    <- _process_utterance_v1 without the file I/O: trim_silence :71-77 (librosa 0.7.2
+ *                                              effects.trim), preemphasis :47-50, rescale preprocessor.py:70-72,
+ *                                              melspectrogram of the pre-emphasised signal, and the padded audio :100-111
+ * librosa's stft with center=True and constant padding, symmetric clipped normalisation.  A signal of n samples gives
+ * T = 1 + n / hop frames.  The float parameters preemphasis and rescaling_max enter the fp64 steps as the shortest decimal
+ * that rounds to them (0.97f -> 0.97), which is what a Python caller passed.
+ * ------------------------------------------------------------------------------------------------------------------ */
+typedef struct {
+  int32_t n_fft;            /* 2048 (the only size implemented)       */
+  int32_t hop_size;         /* 275                                    */
+  int32_t win_size;         /* 1100 (<= n_fft), periodic Hann         */
+  int32_t num_mels;         /* 80 (<= 128)                            */
+  float max_abs_value;      /* 4                                      */
+  float min_level_db;       /* -100                                   */
+  float ref_level_db;       /* 20                                     */
+  float magnitude_power;    /* 2                                      */
+  float preemphasis;        /* 0.97                                   */
+  float rescaling_max;      /* 0.999                                  */
+  int32_t trim_fft_size;    /* 2048: trim frame length                */
+  int32_t trim_hop_size;    /* 512                                    */
+  float trim_top_db;        /* 25                                     */
+} b200tts_mel_cfg;
+
+enum { B200TTS_MEL_TRIM = 1, B200TTS_MEL_PREEMPHASIS = 2, B200TTS_MEL_RESCALE = 4 };
+
+typedef struct b200tts_mel b200tts_mel;
+
+/* h_mel_basis [num_mels][n_fft/2 + 1]: the fp32 Slaney filterbank (librosa.filters.mel(sample_rate, n_fft, num_mels, fmin,
+ * fmax), _build_mel_basis :268-271), computed by the caller. */
+int b200tts_mel_create(b200tts_mel** out, int device, const b200tts_mel_cfg* cfg, const float* h_mel_basis);
+void b200tts_mel_destroy(b200tts_mel* ctx);
+
+/* d_wav [B][L_max] float32 signals, d_len [B] their lengths (clamped to [0, L_max]).  Outputs, with T_max = 1 + L_max / hop:
+ *   d_mel    [B][T_max][num_mels]  frames x mels, zero beyond each row's frame count
+ *   d_frames [B]                   frame count T of each row (0 for a row that TRIM empties, a row shorter than
+ *                                  trim_fft_size when trimming, and an empty row)
+ *   d_bounds [B][2] (may be NULL)  [start, end) of the kept samples (the whole row without TRIM)
+ *   d_audio  [B][T_max * hop] (may be NULL)  the (rescaled) kept samples, zero-padded from end - start on
+ * Each row is computed exactly as a stand-alone run of that row.  TRIM: a frame is non-silent when its mean square is within
+ * trim_top_db of the loudest frame's; a row whose frames are all exactly zero has none. */
+int b200tts_mel_analyze(b200tts_mel* ctx, const float* d_wav, const int32_t* d_len, int B, int L_max, int flags, float* d_mel,
+                        int32_t* d_frames, int32_t* d_bounds, float* d_audio, void* stream);
+
+/* Number of kernel launches issued on this context since creation. */
+int64_t b200tts_mel_launch_count(const b200tts_mel* ctx);
+
 /* Debug aid: mean SM cycles per CTA spent in {compute, barrier} of each of the 6 phases of the last grid-kernel
  * launch; only recorded when the environment variable B200TTS_GRID_PROF is set while generating. */
 int b200tts_wavernn_debug_phase_cycles(b200tts_wavernn* ctx, double* out12);

@@ -33,6 +33,9 @@ hparams = HParams(
     # Griffin-Lim mel inversion (tacotron/datasets/audio.py:122-137, :176-186 there; tacotron_synthesize.py --griffin_lim)
     n_fft=2048, fmin=95, fmax=7600, min_level_db=-100, ref_level_db=20, magnitude_power=2., power=1.5, griffin_lim_iters=60,
     preemphasize=True, preemphasis=0.97, signal_normalization=True, allow_clipping_in_normalization=True,
+    # mel analysis of recorded audio (tacotron/datasets/preprocessor.py:52-121 there; tacotron_hparams.py:68-69, 90-93)
+    rescale=True, rescaling_max=0.999,
+    trim_silence=True, trim_fft_size=2048, trim_hop_size=512, trim_top_db=25,
     # model
     outputs_per_step=1, stop_at_any=True, batch_norm_position='after',
     embedding_dim=128,

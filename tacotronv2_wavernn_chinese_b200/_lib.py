@@ -69,6 +69,16 @@ class GlPhase(C.Structure):
 
 GL_PHASE_PHILOX, GL_PHASE_EXT = 0, 1
 
+
+class MelCfg(C.Structure):
+    _fields_ = [('n_fft', C.c_int32), ('hop_size', C.c_int32), ('win_size', C.c_int32), ('num_mels', C.c_int32),
+                ('max_abs_value', C.c_float), ('min_level_db', C.c_float), ('ref_level_db', C.c_float),
+                ('magnitude_power', C.c_float), ('preemphasis', C.c_float), ('rescaling_max', C.c_float),
+                ('trim_fft_size', C.c_int32), ('trim_hop_size', C.c_int32), ('trim_top_db', C.c_float)]
+
+
+MEL_TRIM, MEL_PREEMPHASIS, MEL_RESCALE = 1, 2, 4
+
 # every symbol include/b200tts.h declares: (restype, argtypes)
 SIGNATURES = {
     'b200tts_abi_version': (C.c_int, []),
@@ -107,6 +117,11 @@ SIGNATURES = {
                                       C.c_void_p, C.c_void_p]),
     'b200tts_gl_philox_uniform': (C.c_int, [C.c_int, C.c_uint64, C.c_uint64, C.c_int, C.c_int, C.c_int, C.c_void_p, C.c_void_p]),
     'b200tts_gl_launch_count': (C.c_int64, [C.c_void_p]),
+    'b200tts_mel_create': (C.c_int, [C.POINTER(C.c_void_p), C.c_int, C.POINTER(MelCfg), C.c_void_p]),
+    'b200tts_mel_destroy': (None, [C.c_void_p]),
+    'b200tts_mel_analyze': (C.c_int, [C.c_void_p, C.c_void_p, C.c_void_p, C.c_int, C.c_int, C.c_int, C.c_void_p, C.c_void_p,
+                                      C.c_void_p, C.c_void_p, C.c_void_p]),
+    'b200tts_mel_launch_count': (C.c_int64, [C.c_void_p]),
 }
 
 _lib = None

@@ -87,6 +87,16 @@ __device__ __forceinline__ void gl_fft1024(float2* a, float2* b, const float2* _
   }
 }
 
+// Real split step of the forward 2048-point rfft: Z = FFT1024 of the even/odd-packed signal, za = Z[k], zb = Z[(1024-k) mod
+// 1024], w = e^{-2 pi i k / 2048}  ->  rfft bins *X0 = X[k] and *X1 = X[1024-k], 0 <= k <= 512.
+__device__ __forceinline__ void gl_forward_split(float2 za, float2 zb, float2 w, float2* X0, float2* X1) {
+  const float2 fe = make_float2(0.5f * (za.x + zb.x), 0.5f * (za.y - zb.y));   // (Z[k] + conj Z[N-k]) / 2
+  const float2 fo = make_float2(0.5f * (za.y + zb.y), -0.5f * (za.x - zb.x));  // (Z[k] - conj Z[N-k]) / 2i
+  const float2 wf = cmul(w, fo);
+  *X0 = make_float2(fe.x + wf.x, fe.y + wf.y);          // X[k]
+  *X1 = make_float2(fe.x - wf.x, -(fe.y - wf.y));       // X[N-k] = conj(fe - w fo)
+}
+
 // Spectrum pair (k, 1024-k) -> inverse-split inputs Z'[k], Z'[1024-k] (irfft of Y = (Y[0..1024]) as a 1024-point complex IFFT).
 // Y0/Y1 are Y[k], Y[1024-k]; for k = 0 they are Y[0], Y[1024] (imaginary parts already dropped, as irfft does).
 __device__ __forceinline__ void gl_inverse_split(int k, float2 Y0, float2 Y1, float2 w, float2* out) {
@@ -161,13 +171,9 @@ __global__ void __launch_bounds__(kGlThreads) gl_frame_kernel(GlArgs A) {
     // real split -> X[k], X[N-k]; unit phasor times S; inverse split into buf[1]
     for (int k = threadIdx.x; k <= kGlHalf / 2; k += kGlThreads) {
       const int k2 = kGlHalf - k;
-      const float2 za = buf[0][k], zb = buf[0][k2 & (kGlHalf - 1)];
-      const float2 fe = make_float2(0.5f * (za.x + zb.x), 0.5f * (za.y - zb.y));   // (Z[k] + conj Z[N-k]) / 2
-      const float2 fo = make_float2(0.5f * (za.y + zb.y), -0.5f * (za.x - zb.x));  // (Z[k] - conj Z[N-k]) / 2i
       const float2 w = __ldg(A.tws + k);
-      const float2 wf = cmul(w, fo);
-      const float2 X0 = make_float2(fe.x + wf.x, fe.y + wf.y);          // X[k]
-      const float2 X1 = make_float2(fe.x - wf.x, -(fe.y - wf.y));       // X[N-k] = conj(fe - w fo)
+      float2 X0, X1;
+      gl_forward_split(buf[0][k], buf[0][k2 & (kGlHalf - 1)], w, &X0, &X1);
       float2 Y[2];
       const float2 X[2] = {X0, X1};
       const int kk[2] = {k, k2};

@@ -17,6 +17,15 @@ Griffin-Lim (what `inv_mel_spectrogram` computes, T frames -> 275 (T - 1) sample
   3. 60 Griffin-Lim iterations from a uniform random phase, librosa 0.7.2 stft / istft                  (_griffin_lim :176-186)
   4. lfilter([1], [1, -0.97])                                                                           (inv_preemphasis :52-55)
 The random phase is Philox(seed) keyed by (utterance, frame, bin) instead of numpy's global generator.
+
+Mel analysis (the reference's feature extraction, on the GPU through libb200tts; `preprocess_wav` is `_process_utterance_v1`,
+tacotron/datasets/preprocessor.py:52-121, without the file I/O):
+  1. load_wav: 16-bit / 32-bit / 8-bit PCM or float32, averaged to mono, at hparams.sample_rate only      (audio.py:14-15)
+  2. trim silence: frames of 2048 samples every 512 more than 25 dB below the loudest are cut at both ends  (:71-77)
+  3. pre-emphasis lfilter([1, -0.97], [1]) in float64, then each signal / its peak * 0.999               (:47-50, preprocessor :70-72)
+  4. melspectrogram: |stft|^2, Slaney filterbank, 20 log10(max(1e-5, .)) - 20, symmetric +-4 with clipping  (:95-102)
+  5. the training audio: the rescaled trimmed wav zero-padded to T * 275 samples                          (preprocessor :100-111)
+`melspectrogram(wav, hparams)` is step 4 alone, as in the reference.
 """
 from __future__ import annotations
 
@@ -95,6 +104,13 @@ def _inv_mel_basis(sr, n_fft, n_mels, fmin, fmax):
     return b
 
 
+def mel_basis(hparams):
+    """The filterbank rounded to float32, [num_mels][1 + n_fft/2]: what `_linear_to_mel` (audio.py:250-254) multiplies by."""
+    assert hparams.fmax <= hparams.sample_rate // 2                     # audio.py:269
+    return mel_filterbank(hparams.sample_rate, hparams.n_fft, hparams.num_mels, float(hparams.fmin),
+                          float(hparams.fmax)).astype(np.float32)
+
+
 def inv_mel_basis(hparams):
     """np.linalg.pinv of the filterbank in float64, [1 + n_fft/2][num_mels] (`_inv_mel_basis` of audio.py:256-260)."""
     assert hparams.fmax <= hparams.sample_rate // 2                     # audio.py:269
@@ -104,13 +120,19 @@ def inv_mel_basis(hparams):
 _engines = {}
 
 
-def _engine(hparams, device=None):
+def _engine(hparams, device=None, kind='griffin_lim'):
+    """The cached GPU engine of `kind` ('griffin_lim' or 'mel_analysis') for these hparams on `device`."""
     import torch
-    from .griffin_lim import GriffinLimEngine
+    if kind == 'griffin_lim':
+        from .griffin_lim import GriffinLimEngine as cls
+    elif kind == 'mel_analysis':
+        from .mel_analysis import MelAnalysisEngine as cls
+    else:
+        raise ValueError(f'unknown engine kind {kind!r}')
     dev = torch.cuda.current_device() if device is None and torch.cuda.is_available() else device
-    key = (dev, tuple(sorted((k, repr(v)) for k, v in hparams.values().items())))
+    key = (kind, dev, tuple(sorted((k, repr(v)) for k, v in hparams.values().items())))
     if key not in _engines:
-        _engines[key] = GriffinLimEngine(hparams, device=dev)
+        _engines[key] = cls(hparams, device=dev)
     return _engines[key]
 
 
@@ -137,3 +159,87 @@ def inv_mel_spectrogram(mel_spectrogram, hparams, seed=0):
     """The reference's `audio.inv_mel_spectrogram(mel.T, hparams)` (audio.py:122-137): mel [num_mels][T], T >= 2 -> float32 wave
     of hop * (T - 1) samples, Griffin-Lim with hparams.griffin_lim_iters iterations on the GPU."""
     return griffin_lim_batch([mel_spectrogram], hparams, seed=seed)[0]
+
+
+# ---- mel analysis (feature extraction) ---------------------------------------------------------------------------------
+def load_wav(path, sr):
+    """`audio.load_wav` (audio.py:14-15, librosa.core.load(path, sr=sr)[0]) without resampling: float32 mono samples.
+    PCM is scaled as soundfile does (int16 / 32768, int32 / 2^31, (uint8 - 128) / 128), float32 is read as is, channels are
+    averaged.  A file at another rate, a missing or an unreadable file raise ValueError."""
+    from scipy.io import wavfile
+    try:
+        rate, x = wavfile.read(str(path))
+    except (OSError, ValueError, EOFError) as e:
+        raise ValueError(f'cannot read {path}: {e}') from e
+    if rate != int(sr):
+        raise ValueError(f'{path} is sampled at {rate} Hz, expected {int(sr)} Hz (resampling is not implemented)')
+    if x.dtype == np.int16:
+        y = x.astype(np.float32) / np.float32(32768)
+    elif x.dtype == np.int32:
+        y = x.astype(np.float32) / np.float32(2 ** 31)
+    elif x.dtype == np.uint8:
+        y = (x.astype(np.float32) - np.float32(128)) / np.float32(128)
+    elif x.dtype == np.float32:
+        y = x
+    else:
+        raise ValueError(f'{path}: unsupported sample format {x.dtype}')
+    if y.ndim == 2:
+        y = y.mean(axis=1, dtype=np.float32)              # librosa.to_mono
+    return np.ascontiguousarray(y, dtype=np.float32)
+
+
+def _analyze(wavs, hparams, flags, device=None, want_audio=False):
+    import torch
+    wavs = [np.ascontiguousarray(w, dtype=np.float32).reshape(-1) for w in wavs]
+    if any(w.size == 0 for w in wavs):
+        raise ValueError('empty signal')
+    lengths = np.array([w.size for w in wavs], dtype=np.int64)
+    batch = np.zeros((len(wavs), int(lengths.max())), dtype=np.float32)
+    for i, w in enumerate(wavs):
+        batch[i, :w.size] = w
+    eng = _engine(hparams, device, kind='mel_analysis')
+    out = eng.run(batch, lengths, flags=flags, want_audio=want_audio)
+    with torch.cuda.device(eng.device):
+        return {k: (v.cpu().numpy() if v is not None else None) for k, v in out.items()}
+
+
+def melspectrogram_batch(wavs, hparams, device=None):
+    """Ragged list of signals -> list of float32 mels [num_mels][1 + len // hop], one GPU launch sequence."""
+    if len(wavs) == 0:
+        return []
+    r = _analyze(wavs, hparams, 0, device)
+    return [np.ascontiguousarray(r['mel'][i, :int(n)].T) for i, n in enumerate(r['frames'])]
+
+
+def melspectrogram(wav, hparams):
+    """The reference's `audio.melspectrogram(wav, hparams)` (audio.py:95-102): [num_mels][T] float32, T = 1 + len // hop."""
+    return melspectrogram_batch([wav], hparams)[0]
+
+
+def preprocess_batch(wavs, hparams, device=None):
+    """`_process_utterance_v1` (preprocessor.py:52-121) without the file I/O, for a ragged list of signals as load_wav returns
+    them: trim silence, pre-emphasis, rescale, melspectrogram of the pre-emphasised signal.  Returns a list of
+    (mel [T][num_mels] float32, out [T * hop] float32 training audio, (start, end) of the kept samples).  A signal the trim
+    empties raises ValueError (the reference cannot process it either)."""
+    from .mel_analysis import preprocess_flags, TRIM
+    if len(wavs) == 0:
+        return []
+    flags = preprocess_flags(hparams)
+    if flags & TRIM:
+        short = [i for i, w in enumerate(wavs) if np.size(w) < hparams.trim_fft_size]
+        if short:
+            raise ValueError(f'signal {short[0]} has fewer than trim_fft_size = {hparams.trim_fft_size} samples')
+    r = _analyze(wavs, hparams, flags, device, want_audio=True)
+    res = []
+    for i, n in enumerate(r['frames']):
+        n = int(n)
+        if n == 0:
+            raise ValueError(f'signal {i} is silent: trimming leaves no samples')
+        s, e = (int(v) for v in r['bounds'][i])
+        res.append((np.ascontiguousarray(r['mel'][i, :n]), r['audio'][i, :n * hparams.hop_size].copy(), (s, e)))
+    return res
+
+
+def preprocess_wav(wav, hparams):
+    """One signal through `preprocess_batch`: (mel [T][num_mels], out [T * hop], (start, end))."""
+    return preprocess_batch([wav], hparams)[0]

@@ -1,7 +1,8 @@
 """Signal helpers the generation path touches, with the reference's public names
 (`wavernn/utils/dsp.py`: label_2_float :8, float_2_label :12, save_wav :22, encode_mu_law :92, decode_mu_law :98).
-Feature extraction (STFT / mel analysis) is preprocessing and not part of this package; Griffin-Lim mel inversion, the
-Tacotron side's preview vocoder, lives in tacotronv2_wavernn_chinese_b200/tacotron/audio.py.
+The reference's `melspectrogram` here (:72) is not restated: the shipped checkpoint was trained on the Tacotron
+preprocessor's features, whose GPU mel analysis lives in tacotronv2_wavernn_chinese_b200/tacotron/audio.py next to Griffin-Lim
+mel inversion, the Tacotron side's preview vocoder.
 
 Conventions (same as the reference): a `bits`-bit label l in [0, 2**bits - 1] maps to the float 2*l/(2**bits - 1) - 1 in
 [-1, 1]; mu-law companding uses mu = n_classes - 1.

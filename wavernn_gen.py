@@ -5,7 +5,12 @@ Same command line (reference wavernn_gen.py:49-61), same input contract (float32
 output name `./wavernn_inference_output/{stem}_gen_NOT_BATCHED_step={k}k.wav` (:35-39, :124).  Deliberate differences:
   * the model runs on the GPU through libb200tts.so (the reference pins `device = cpu`, :93); `--force_cpu` is refused
     because this build has no CPU path.
-  * `.wav` input is refused: that branch of the reference uses undefined names (:19, :30) and cannot run.
+  * `.wav` input is copy-synthesis: the file is loaded, written back as `__{stem}__{k}k_steps_target.wav` (:19, whose
+    undefined `file_name` is read as the stem), analysed on the GPU and vocoded.  The reference's branch would call
+    `wavernn/utils/dsp.py: melspectrogram` (fmax = sr/2, no ref_level_db, [0, 1] normalisation, reflect padding) and crashes
+    before it gets there; we compute instead the features the shipped checkpoint was trained on: the Tacotron preprocessor's
+    `_process_utterance_v1` (trim silence, pre-emphasis, rescale, melspectrogram with the Tacotron hparams) mapped to [0, 1]
+    as wavernn_preprocess.py:155-157 does.  The file must already be at the model's sample rate (no resampling).
   * `--batched` really selects fold-with-overlap generation (the reference parses the flag, then forces it off, :77).
   * extra flags: `--seed` (Philox stream of the sampler), `--kernel {auto,utterance,grid}`.
 """
@@ -20,6 +25,7 @@ import torch
 
 from tacotronv2_wavernn_chinese_b200.wavernn.models.fatchord_version import WaveRNN
 from tacotronv2_wavernn_chinese_b200.wavernn.utils import hparams as hp
+from tacotronv2_wavernn_chinese_b200.wavernn.utils.dsp import save_wav
 from tacotronv2_wavernn_chinese_b200.wavernn.utils.display import simple_table
 from tacotronv2_wavernn_chinese_b200.wavernn.utils.paths import Paths
 
@@ -32,7 +38,7 @@ CLI = [
     (('--samples', '-s'), dict(type=int, help='utterances to take from the test set (unused: --file only)')),
     (('--target', '-t'), dict(type=int, help='samples per fold in --batched mode (default hp.voc_target)')),
     (('--overlap', '-o'), dict(type=int, help='cross-fade samples between folds (default hp.voc_overlap)')),
-    (('--file', '-f'), dict(type=str, help='mel spectrogram .npy, float32 (T, num_mels) in [0, 1]')),
+    (('--file', '-f'), dict(type=str, help='mel spectrogram .npy, float32 (T, num_mels) in [0, 1], or a .wav to re-synthesise')),
     (('--voc_weights', '-w'), dict(type=str, help='checkpoint to load instead of logs_wavernn/checkpoints/latest_weights.pyt')),
     (('--gta', '-g'), dict(dest='gta', action='store_true', help='accepted for compatibility, ignored')),
     (('--force_cpu', '-c'), dict(action='store_true', help='refused: there is no CPU path')),
@@ -42,12 +48,40 @@ CLI = [
 ]
 
 
-def load_mel(path):
-    """`.npy` -> float32 tensor [1, num_mels, T]; shape / range checks as in the reference (:22-28)."""
+def tacotron_hparams():
+    """The Tacotron hparams the WaveRNN features are computed with; they must agree with the WaveRNN hparams on the sample
+    rate, the hop and the number of mels."""
+    from tacotron_hparams import hparams as taco
+    for a, b in (('sample_rate', 'sample_rate'), ('hop_size', 'hop_length'), ('num_mels', 'num_mels')):
+        if getattr(taco, a) != getattr(hp, b):
+            raise ValueError(f'Tacotron {a} = {getattr(taco, a)} differs from WaveRNN {b} = {getattr(hp, b)}')
+    return taco
+
+
+def wav_to_mel(wav):
+    """Float32 samples -> the [0, 1] mel [num_mels, T] WaveRNN was trained on: `_process_utterance_v1`'s features
+    (tacotron/datasets/preprocessor.py:52-121) through clip((mel + 4) / 8, 0, 1) (wavernn_preprocess.py:155-157)."""
+    from tacotronv2_wavernn_chinese_b200.tacotron import audio
+    taco = tacotron_hparams()
+    mel = audio.preprocess_wav(wav, taco)[0]                      # [T][num_mels], symmetric scale
+    m = taco.max_abs_value
+    return np.clip((mel + m) / (2 * m), 0, 1).T
+
+
+def load_mel(path, target_path=None):
+    """`.npy` or `.wav` -> float32 tensor [1, num_mels, T]; shape / range checks as in the reference (:22-28).  A `.wav` is
+    loaded at hp.sample_rate, written to `target_path` (if given) and analysed (see the module docstring)."""
     path = str(path)
-    if not path.endswith('.npy'):
-        raise ValueError(f'Expected a .npy mel spectrogram, but got {os.path.splitext(path)[1] or path}!')
-    mel = np.load(path).T
+    if path.endswith('.wav'):
+        from tacotronv2_wavernn_chinese_b200.tacotron import audio
+        wav = audio.load_wav(path, hp.sample_rate)
+        if target_path is not None:
+            save_wav(wav, target_path)
+        mel = wav_to_mel(wav)
+    elif path.endswith('.npy'):
+        mel = np.load(path).T
+    else:
+        raise ValueError(f'Expected an extension of .wav or .npy, but got {os.path.splitext(path)[1] or path}!')
     if mel.ndim != 2 or mel.shape[0] != hp.num_mels:
         raise ValueError(f'Expected a numpy array shaped (n_hops, n_mels={hp.num_mels}), but got {mel.T.shape}!')
     lo, hi = float(mel.min()), float(mel.max())
@@ -58,8 +92,8 @@ def load_mel(path):
 
 def gen_from_file(model, load_path, save_path, batched, target, overlap, seed=None, kernel='auto'):
     k = model.get_step() // 1000
-    mel = load_mel(load_path)
     stem = str(load_path).split('/')[-1].strip().split('.')[0]
+    mel = load_mel(load_path, target_path=os.path.join(str(save_path), f'__{stem}__{k}k_steps_target.wav'))
     mode = f'gen_batched_target{target}_overlap{overlap}' if batched else 'gen_NOT_BATCHED'
     save_str = os.path.join(str(save_path), f'{stem}_{mode}_step={k}k.wav')
     t0 = time.time()
