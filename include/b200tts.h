@@ -157,8 +157,8 @@ int64_t b200tts_wavernn_launch_count(const b200tts_wavernn* ctx);
 /* Milliseconds (CUDA events on the launch stream) spent in the per-sample generation kernel by the most recent
  * generate call; blocks until that kernel has finished.  Negative on error. */
 double b200tts_wavernn_last_kernel_ms(b200tts_wavernn* ctx);
-/* Which step kernel the last generate call ran: 1 utterance, 2 wide grid, 3 push, 4 multi-group push, 5 tensor-core pipeline
- * (0: none yet).  Instrumentation for bench.py's roofline; no reference counterpart. */
+/* Which step kernel the last generate call ran: 1 utterance, 2 wide grid, 3 push, 5 tensor-core pipeline (0: none yet; 4 is
+ * no longer returned).  Instrumentation for bench.py's roofline; no reference counterpart. */
 int b200tts_wavernn_last_kernel(const b200tts_wavernn* ctx);
 
 /* Synchronises the device and reports whether the most recent generate call on this context completed: the persistent

@@ -17,7 +17,6 @@
 #include "wavernn_utt.cuh"
 #include "wavernn_grid.cuh"
 #include "wavernn_push.cuh"
-#include "wavernn_pushmg.cuh"
 #include "wavernn_tc.cuh"
 #include "taco_decoder.cuh"
 #include "taco_encpost.cuh"
@@ -166,7 +165,7 @@ struct b200tts_wavernn {
   DeviceBuf push_blob, push_condw, push_tab, push_vec, push_best, push_prof;
   DeviceBuf tc_wimg, tc_prm, tc_vec, tc_x1f, tc_win, tc_cnt, tc_cond;     // tensor-core pipeline (wavernn_tc.cuh)
   bool tc_ok = false;
-  int last_kernel = 0;            // 1 utterance, 2 wide grid, 3 push, 4 multi-group push, 5 tensor-core pipeline
+  int last_kernel = 0;            // 1 utterance, 2 wide grid, 3 push, 5 tensor-core pipeline
   int last_push_ncta = 0;
   int* d_grid_error = nullptr;    // set by the grid kernel when a barrier wait timed out (a peer CTA vanished)
   int last_grid_ncta = 0;
@@ -385,11 +384,9 @@ extern "C" int b200tts_wavernn_create(b200tts_wavernn** out, int device, const b
     g.obhh1 = take(3 * kUPC); g.obih2 = take(3 * kUPC); g.obhh2 = take(3 * kUPC);
     g.obfc1 = take(kUPC); g.obfc2 = take(kUPC); g.obfc3 = take(kCPC);
     g.blob = off;
-    constexpr int kMaxScratch = std::max({MapTraits<0, 4, 1>::kScratchFloats, MapTraits<0, 8, 1>::kScratchFloats,
-                                          MapTraits<1, 1, 1>::kScratchFloats, MapTraits<2, 1, 1>::kScratchFloats,
-                                          MapTraits<4, 1, 1>::kScratchFloats, MapTraits<1, 1, 2>::kScratchFloats,
-                                          MapTraits<2, 1, 2>::kScratchFloats, MapTraits<4, 1, 2>::kScratchFloats,
-                                          MapTraits<2, 2, 2>::kScratchFloats});   // every variant launch_grid can dispatch
+    constexpr int kMaxScratch = std::max({MapTraits<0, 4, 1>::kScratchFloats, MapTraits<1, 1, 1>::kScratchFloats,
+                                          MapTraits<2, 1, 1>::kScratchFloats, MapTraits<4, 1, 1>::kScratchFloats,
+                                          MapTraits<4, 1, 2>::kScratchFloats});   // every variant launch_grid can dispatch
     size_t smem_need = ((size_t)g.blob + (size_t)kMaxScratch) * sizeof(float) + 2048;
     if (smem_need > 227 * 1024) g.ok = 0;
     B200_CUDA(cudaDeviceGetAttribute(&ctx->coop, cudaDevAttrCooperativeLaunch, device));
@@ -717,17 +714,14 @@ static void launch_grid_t(b200tts_wavernn* ctx, GridArgs& a, cudaStream_t st) {
 }
 
 // Mapping for B utterances: returns the padded batch; variant = index into the dispatch table below.
-enum { GV_N4, GV_N8, GV_W1, GV_W1x2, GV_W2x2, GV_W4x2, GV_W2, GV_W4, GV_W2_2x2 };
+enum { GV_N4, GV_W1, GV_W2, GV_W4, GV_W4x2 };
 static int grid_variant(int B, int* variant) {
   if (B <= 4) { *variant = GV_N4; return 4; }
-  static const bool narrow8 = getenv("B200TTS_GRID_NARROW8") != nullptr;       // A/B switch: measured 30.7 us/step against 29.4 us
-  if (B <= 8 && narrow8) { *variant = GV_N8; return 8; }                       // for the 32-wide mapping, so 5..8 utterances go wide
-  if (B <= 32) { *variant = GV_W1; return 32; }
-  static const bool mid_dual = getenv("B200TTS_GRID_MID_DUAL") != nullptr;       // A/B switch: old mid-batch mapping
-  if (B <= 64) { *variant = mid_dual ? GV_W1x2 : GV_W2; return 64; }
-  if (B <= 128) { *variant = mid_dual ? GV_W2x2 : GV_W4; return 128; }
-  static const bool big22 = getenv("B200TTS_GRID_BIG_2X2") != nullptr;         // A/B switch: 2 utt x 12 rows per thread, no row slices
-  *variant = big22 ? GV_W2_2x2 : GV_W4x2;
+  if (B <= 32) { *variant = GV_W1; return 32; }     // 5..8 utterances too: on the previous GPU the 8-row narrow mapping
+                                                    // measured 30.7 us/step against 29.4 us for this one
+  if (B <= 64) { *variant = GV_W2; return 64; }
+  if (B <= 128) { *variant = GV_W4; return 128; }
+  *variant = GV_W4x2;
   return (B + 255) / 256 * 256;
 }
 
@@ -810,14 +804,10 @@ static void launch_grid(b200tts_wavernn* ctx, const float* d_mel, GenArgs& ua, c
   B200_CUDA(cudaEventRecord(ctx->ev0, st));
   switch (variant) {
     case GV_N4: launch_grid_t<0, 4, 1>(ctx, a, st); break;
-    case GV_N8: launch_grid_t<0, 8, 1>(ctx, a, st); break;
     case GV_W1: launch_grid_t<1, 1, 1>(ctx, a, st); break;
-    case GV_W1x2: launch_grid_t<1, 1, 2>(ctx, a, st); break;
-    case GV_W2x2: launch_grid_t<2, 1, 2>(ctx, a, st); break;
-    case GV_W4x2: launch_grid_t<4, 1, 2>(ctx, a, st); break;
     case GV_W2: launch_grid_t<2, 1, 1>(ctx, a, st); break;
     case GV_W4: launch_grid_t<4, 1, 1>(ctx, a, st); break;
-    case GV_W2_2x2: launch_grid_t<2, 2, 2>(ctx, a, st); break;
+    case GV_W4x2: launch_grid_t<4, 1, 2>(ctx, a, st); break;
     default: REQUIRE(false, B200TTS_EINVAL, "internal: unknown grid variant");
   }
   B200_CUDA(cudaEventRecord(ctx->ev1, st));
@@ -840,21 +830,13 @@ static void launch_push_t(b200tts_wavernn* ctx, PushArgs& a, cudaStream_t st) {
   ctx->launches++;
 }
 
-// rows per group of the push kernels: up to 8 rows run the 8-row variant (on the previous GPU the 4-row variant was slower, its
-// 64 hot L2 lines being polled by 65 536 threads; not re-measured on the H100); env B200TTS_PUSH_MIN_G is an A/B switch.
-static inline int push_rows(int B) {
-  static const int min_g = getenv("B200TTS_PUSH_MIN_G") ? atoi(getenv("B200TTS_PUSH_MIN_G")) : 8;
-  const int g = B <= 4 ? 4 : (B <= 8 ? 8 : (B <= 16 ? 16 : 32));
-  return g < min_g ? (min_g <= 8 ? 8 : (min_g <= 16 ? 16 : 32)) : g;
-}
+// rows of the push kernel variant: up to 8 rows run the 8-row variant (on the previous GPU a 4-row variant was slower, its
+// 64 hot L2 lines being polled by 65 536 threads)
+static inline int push_rows(int B) { return B <= 8 ? 8 : (B <= 16 ? 16 : kPushMaxRows); }
 
-// Can this call take the push kernel?  (env B200TTS_PUSH=0 keeps the round-1 mappings for A/B timing.)
+// Can this call take the push kernel?
 static bool push_eligible(const b200tts_wavernn* ctx, int rows) {
-  static const bool off = getenv("B200TTS_PUSH") != nullptr && getenv("B200TTS_PUSH")[0] == '0';
-  // Default 32: the multi-group form (wavernn_pushmg.cuh, 33 ... 256 rows) is parity-green but MEASURED SLOWER than the round-1 wide
-  // mapping (twice as slow at 256 rows on the previous GPU), so it only runs when asked for.
-  static const int max_rows = getenv("B200TTS_PUSH_MAX_ROWS") ? atoi(getenv("B200TTS_PUSH_MAX_ROWS")) : kMgG;
-  return ctx->pm.ok && ctx->gm.ok && rows <= max_rows && rows <= kMgG * kMgMaxGroups && !off;
+  return ctx->pm.ok && ctx->gm.ok && rows <= kPushMaxRows;
 }
 
 // `fold` != null: rows are the folds of ONE source utterance of T0 frames (conditioning tables of utterance 0, row u
@@ -869,10 +851,9 @@ static void launch_push(b200tts_wavernn* ctx, const float* d_mel, GenArgs& ua, c
   const b200tts_wavernn_cfg& c = ctx->cfg;
   const PushModel& pm = ctx->pm;
   const int rows = pack ? pack->rows : ua.B;
-  const int ng = rows > kMgG ? (rows + kMgG - 1) / kMgG : 1;          // > 32 rows: multi-group kernel, groups of 32
-  const int G = ng > 1 ? kMgG : push_rows(rows);
+  const int G = push_rows(rows);
   const int T = fold ? T0 : ua.T, hop = c.hop_length;
-  const int tab_rows = fold ? 1 : (pack ? pack->n_utt : ng * G), src_rows = fold ? 1 : (pack ? pack->n_utt : rows);
+  const int tab_rows = fold ? 1 : (pack ? pack->n_utt : G), src_rows = fold ? 1 : (pack ? pack->n_utt : rows);
   // conditioning tables [tab_rows][T+1][ncta][52]
   ctx->push_tab.ensure((size_t)tab_rows * (T + 1) * pm.ncta * kPushCondRows * sizeof(float));
   {
@@ -883,7 +864,7 @@ static void launch_push(b200tts_wavernn* ctx, const float* d_mel, GenArgs& ua, c
     B200_CUDA(cudaGetLastError());
     ctx->launches++;
   }
-  const size_t nvec = (size_t)ng * kPushVecs * 2 * pm.ncta * G * 4, nbest = (size_t)ng * pm.ncta * G;
+  const size_t nvec = (size_t)kPushVecs * 2 * pm.ncta * G * 4, nbest = (size_t)pm.ncta * G;
   ctx->push_vec.ensure(nvec * sizeof(float));
   ctx->push_best.ensure(nbest * sizeof(unsigned long long) + 64);
   int* d_err = reinterpret_cast<int*>(ctx->push_best.as<unsigned long long>() + nbest);
@@ -900,7 +881,6 @@ static void launch_push(b200tts_wavernn* ctx, const float* d_mel, GenArgs& ua, c
   a.fir = ctx->d_fir;
   a.NT = ctx->NT;
   a.B = pack ? pack->n_utt : rows; a.S = ua.S; a.T = T; a.hop = hop; a.steps = pack ? pack->steps : ua.steps;
-  a.ng = ng;
   if (pack) { a.pack_utt = pack->utt; a.pack_start = pack->start; a.pack_segs = pack->segs; a.pack_rows = pack->rows; }
   a.row_stride = fold ? fold->stride : 0;
   a.S_src = T * hop;
@@ -915,20 +895,7 @@ static void launch_push(b200tts_wavernn* ctx, const float* d_mel, GenArgs& ua, c
     ctx->last_grid_ncta = 0;
   }
   B200_CUDA(cudaEventRecord(ctx->ev0, st));
-  if (ng > 1) {
-    const MgLayout L(ng);
-    size_t smem = ((size_t)pm.blob + (size_t)L.total) * sizeof(float);
-    REQUIRE(smem + 2048 <= 227 * 1024, B200TTS_EINVAL, "multi-group push kernel: shared memory budget exceeded");
-    B200_CUDA(cudaFuncSetAttribute(wavernn_pushmg_kernel, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)smem));
-    int per_sm = 0;
-    B200_CUDA(cudaOccupancyMaxActiveBlocksPerMultiprocessor(&per_sm, wavernn_pushmg_kernel, kPushThreads, smem));
-    REQUIRE(per_sm * ctx->sm_count >= pm.ncta, B200TTS_EINVAL, "multi-group push kernel cannot be made co-resident on this device");
-    PushModel m = pm;
-    void* args[] = {(void*)&m, (void*)&a};
-    B200_CUDA(cudaLaunchCooperativeKernel((const void*)wavernn_pushmg_kernel, dim3(pm.ncta), dim3(kPushThreads), args, smem, st));
-    ctx->launches++;
-  } else switch (G) {
-    case 4: launch_push_t<4>(ctx, a, st); break;
+  switch (G) {
     case 8: launch_push_t<8>(ctx, a, st); break;
     case 16: launch_push_t<16>(ctx, a, st); break;
     default: launch_push_t<32>(ctx, a, st); break;
@@ -937,6 +904,10 @@ static void launch_push(b200tts_wavernn* ctx, const float* d_mel, GenArgs& ua, c
 }
 
 // ---- tensor-core pipeline (wavernn_tc.cuh): 33 ... 256 rows, plain batches ----------------------------------------------
+// Smallest batch kernel=auto gives the tensor cores.  On an H100 (80GB HBM3, 700 W) the tensor-core pipeline costs 62-66 us per
+// lock-step whatever the row count (1 or 2 groups of 128 rows in flight), the wide CUDA-core mapping 37.5 us at 64 rows, 60.9 at
+// 96-128 and 90-91 from 129 rows on (a second tile of 128).
+constexpr int kTcMinRows = 129;
 static bool tc_eligible(const b200tts_wavernn* ctx, int rows, bool folding, bool packing) {
   return ctx->tc_ok && ctx->pm.ok && !folding && !packing && rows >= 1 && rows <= kTcRows * kTcMaxGroups;
 }
@@ -1017,8 +988,7 @@ static void run_generate(b200tts_wavernn* ctx, const float* d_mel, int B, int T,
   const bool packing = opts && opts->d_pack_utt;
   // kernel=auto and more than 256 rows: launches of 256 rows through the tensor-core pipeline (66 us per lock-step each on an H100)
   // beat the wide mapping on the whole batch (91 us per 256 rows); the noise is keyed by the global row, so the result does not change
-  const bool tc_off = getenv("B200TTS_TC") != nullptr && getenv("B200TTS_TC")[0] == '0';
-  const bool tc_slices = B > kTcRows * kTcMaxGroups && !tc_off && (!opts || opts->kernel == B200TTS_KERNEL_AUTO) && !debug_bufs && d_labels &&
+  const bool tc_slices = B > kTcRows * kTcMaxGroups && (!opts || opts->kernel == B200TTS_KERNEL_AUTO) && !debug_bufs && d_labels &&
                          tc_eligible(ctx, kTcRows * kTcMaxGroups, folding, packing);
   const bool sliceable = tc_slices || B > 256 || per_row * 256 > budget;
   if (!sliceable || debug_bufs || folding || packing || (!tc_slices && per_row * ((B + 255) / 256 * 256) <= budget) || !d_labels) {
@@ -1087,7 +1057,7 @@ static void run_generate_rows(b200tts_wavernn* ctx, const float* d_mel, int B, i
   }
   const bool packing = o.d_pack_utt != nullptr;
   if (packing) {
-    REQUIRE(!folding && o.d_pack_start && o.pack_rows >= 1 && o.pack_rows <= 32 && o.pack_segs >= 1 && o.pack_steps >= 1, B200TTS_EINVAL,
+    REQUIRE(!folding && o.d_pack_start && o.pack_rows >= 1 && o.pack_rows <= kPushMaxRows && o.pack_segs >= 1 && o.pack_steps >= 1, B200TTS_EINVAL,
             "bad packed-row schedule (pack_rows 1..32, pack_segs >= 1, pack_steps >= 1, not together with folding)");
     REQUIRE(o.max_steps == 0 && !o.d_logits && !o.d_teacher && r.mode == B200TTS_RNG_PHILOX && d_labels, B200TTS_EINVAL,
             "packed generation takes PHILOX noise, all steps, caller-owned labels and no debug buffers");
@@ -1101,13 +1071,8 @@ static void run_generate_rows(b200tts_wavernn* ctx, const float* d_mel, int B, i
     labels = ctx->labels.as<int16_t>();
   }
   bool use_tc = false;
-  // kernel=auto: on an H100 (80GB HBM3, 700 W) the tensor-core pipeline costs 62-66 us per lock-step whatever the row count
-  // (1 or 2 groups of 128 rows in flight), the wide CUDA-core mapping 37.5 us at 64 rows, 60.9 at 96-128 and 90-91 from 129
-  // rows on (a second tile of 128) -> the tensor cores take 129 rows and more (env B200TTS_TC_MIN_ROWS; B200TTS_TC=0 keeps the
-  // CUDA-core mappings).  Fold mode and packed rows stay on the other kernels.
-  static const int tc_min_rows = getenv("B200TTS_TC_MIN_ROWS") ? atoi(getenv("B200TTS_TC_MIN_ROWS")) : 129;
-  static const bool tc_off = getenv("B200TTS_TC") != nullptr && getenv("B200TTS_TC")[0] == '0';
-  if (o.kernel == B200TTS_KERNEL_AUTO && kernel == B200TTS_KERNEL_GRID && !tc_off && GB >= tc_min_rows && tc_eligible(ctx, GB, folding, packing))
+  // kernel=auto: the tensor cores take kTcMinRows rows and more.  Fold mode and packed rows stay on the other kernels.
+  if (o.kernel == B200TTS_KERNEL_AUTO && kernel == B200TTS_KERNEL_GRID && GB >= kTcMinRows && tc_eligible(ctx, GB, folding, packing))
     kernel = B200TTS_KERNEL_TC;
   if (kernel == B200TTS_KERNEL_TC) {
     REQUIRE(tc_eligible(ctx, GB, folding, packing), B200TTS_EINVAL,
@@ -1136,7 +1101,7 @@ static void run_generate_rows(b200tts_wavernn* ctx, const float* d_mel, int B, i
   REQUIRE(!(folding && r.d_utterance_ids), B200TTS_EINVAL, "d_utterance_ids cannot be combined with fold-with-overlap generation");
   a.teacher = o.d_teacher; a.logits_out = o.d_logits; a.labels = labels;
 
-  ctx->last_kernel = kernel == B200TTS_KERNEL_UTTERANCE ? 1 : (use_tc ? 5 : (use_push ? (GB > kMgG && !packing ? 4 : 3) : 2));
+  ctx->last_kernel = kernel == B200TTS_KERNEL_UTTERANCE ? 1 : (use_tc ? 5 : (use_push ? 3 : 2));
   if (kernel == B200TTS_KERNEL_UTTERANCE) {
     if (folding) {   // per-fold conditioning in the row-major layout this kernel reads, aux per sample (hop = 1)
       ctx->fold_mels.ensure((size_t)GB * GS * c.feat_dims * sizeof(float));
@@ -1610,8 +1575,7 @@ static int taco_decode_impl(b200tts_taco* ctx, const float* d_memory, const int3
   a.rng_mode = d.mode; a.seed = d.seed; a.utt_offset = d.utterance_offset; a.masks = d.d_masks;
   a.frames = d_frames; a.stop = d_stop; a.align = d_align; a.nsteps = d_nsteps;
   a.forced = d_forced;
-  static const bool tg_off = getenv("B200TTS_TACO_GRID") != nullptr && getenv("B200TTS_TACO_GRID")[0] == '0';
-  if (B == 1 && ctx->tg_ok && !tg_off) {
+  if (B == 1 && ctx->tg_ok) {
     // ONE sentence: the weight-stationary 128-block decoder (taco_grid.cuh).  The sentence length is needed on the host to size
     // the exchange buffers; d_lengths is a device pointer, so Tx_max (the caller's padded length) bounds it and the kernel
     // reads the true length itself.

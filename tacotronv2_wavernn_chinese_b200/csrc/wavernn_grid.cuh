@@ -18,27 +18,18 @@
 //   P5  fc3      (:223) + sampling (:232-235): every CTA owns 8 logits per utterance and joins a distributed
 //       argmax of (logit - log q), q ~ Exp(1), through one 64-bit atomicMax per (CTA, utterance)  [Gumbel-max ==
 //       Categorical(softmax(logits)).sample()]; the winner is read back by everybody at the next P0 (:235-237).
-// Two thread mappings: "wide" for B >= 9 -- lanes = utterances, register tile 4 utterances x 6 rows, 16 warps factored as
+// Two thread mappings: "wide" for B >= 5 -- lanes = utterances, register tile 4 utterances x 6 rows, 16 warps factored as
 // (GEMM x utterance warp x row slice x k slice), k-slice partial sums through shared memory, two independent utterance
-// groups per CTA (own named barrier + grid-barrier counter each) so one group computes while the other sits in a
-// barrier -- and "narrow" for B <= 8 (activation vector staged into shared memory in one L2 round trip, lanes = k,
-// warp-shuffle reductions) where the step is pure latency.
+// groups per CTA above 128 utterances (own named barrier + grid-barrier counter each) so one group computes while the
+// other sits in a barrier -- and "narrow" for B <= 4 (activation vector staged into shared memory in one L2 round trip,
+// lanes = k, warp-shuffle reductions) where the step is pure latency.
 #pragma once
 #include "common.cuh"
 
 namespace b200tts {
 
-#ifndef B200_GRID_NW_WIDE
-#define B200_GRID_NW_WIDE 16           // wide mapping: warps per CTA.  Measured at B=256: 8 warps (255 regs, 4x12 tiles) 80.5 us,
+constexpr int kGridWarpsWide = 16;     // wide mapping: warps per CTA.  Measured at B=256: 8 warps (255 regs, 4x12 tiles) 80.5 us,
                                        // 12 warps (168 regs) spill, 16 warps (128 regs, 4x6 tiles via row slices) 73.5 us
-#endif
-#ifndef B200_GRID_PD16_SMALL
-#define B200_GRID_PD16_SMALL 1        // ... for the 4/8-row tiles (fc phases), which have registers to spare
-#endif
-#ifndef B200_GRID_PD16
-#define B200_GRID_PD16 1              // columns of look-ahead in the 16-warp build (register budget 128)
-#endif
-constexpr int kGridWarpsWide = B200_GRID_NW_WIDE;
 constexpr int kGridWarpsNarrow = 8;
 constexpr int kUPC = 4;   // hidden units (and fc1/fc2 rows) per CTA
 constexpr int kCPC = 8;   // classes (fc3 rows) per CTA
@@ -102,9 +93,6 @@ __device__ __forceinline__ void group_sync(int grp) {
 // `grid_arrive`: all threads of the group call, after their last global write of the phase.
 // `grid_wait`:   all threads of the group call; `target` = (number of barriers arrived at so far) * gridDim.x.  False on
 //                timeout (a co-resident CTA is gone): the caller returns instead of hanging the GPU.
-#ifndef B200_GRID_SPLIT_BARRIER
-#define B200_GRID_SPLIT_BARRIER 2   // single-group kernels only.  0: plain barriers; 1: P01's GEMMs run before the wait on
-#endif                              // P5's barrier; 2: also GRU-2's W_hh pass starts before the wait on P01's barrier
 template <int GROUPS, int NTG>
 __device__ __forceinline__ void grid_arrive(unsigned int* ctr, int grp, int gtid) {
   group_sync<GROUPS, NTG>(grp);
@@ -140,37 +128,23 @@ __device__ __forceinline__ void grid_wait_sub(unsigned int* ctr, unsigned int ta
 }
 
 // ---- activation loads (L2 only: these buffers are rewritten by other SMs every step) ----------------------------------
-#ifndef B200_GRID_ACT_L1
-#define B200_GRID_ACT_L1 0
-#endif
-#if B200_GRID_ACT_L1
-#define B200_ACT_LD __ldca     // through L1: legal because every grid barrier's ld.acquire.gpu invalidates L1 (CCTL.IVALL)
-#else
-#define B200_ACT_LD __ldcg
-#endif
 template <int U> struct ActLoad;
 template <> struct ActLoad<1> {
-  static __device__ __forceinline__ void ld(const float* p, float (&a)[1]) { a[0] = B200_ACT_LD(p); }
+  static __device__ __forceinline__ void ld(const float* p, float (&a)[1]) { a[0] = __ldcg(p); }
   static __device__ __forceinline__ void st(float* p, const float (&a)[1]) { p[0] = a[0]; }
 };
 template <> struct ActLoad<2> {
   static __device__ __forceinline__ void ld(const float* p, float (&a)[2]) {
-    float2 v = B200_ACT_LD(reinterpret_cast<const float2*>(p)); a[0] = v.x; a[1] = v.y;
+    float2 v = __ldcg(reinterpret_cast<const float2*>(p)); a[0] = v.x; a[1] = v.y;
   }
   static __device__ __forceinline__ void st(float* p, const float (&a)[2]) { *reinterpret_cast<float2*>(p) = make_float2(a[0], a[1]); }
 };
 template <> struct ActLoad<4> {
   static __device__ __forceinline__ void ld(const float* p, float (&a)[4]) {
-    float4 v = B200_ACT_LD(reinterpret_cast<const float4*>(p)); a[0] = v.x; a[1] = v.y; a[2] = v.z; a[3] = v.w;
+    float4 v = __ldcg(reinterpret_cast<const float4*>(p)); a[0] = v.x; a[1] = v.y; a[2] = v.z; a[3] = v.w;
   }
   static __device__ __forceinline__ void st(float* p, const float (&a)[4]) {
     *reinterpret_cast<float4*>(p) = make_float4(a[0], a[1], a[2], a[3]);
-  }
-};
-template <> struct ActLoad<8> {
-  static __device__ __forceinline__ void ld(const float* p, float (&a)[8]) {
-    float4 v = B200_ACT_LD(reinterpret_cast<const float4*>(p)), w = B200_ACT_LD(reinterpret_cast<const float4*>(p) + 1);
-    a[0] = v.x; a[1] = v.y; a[2] = v.z; a[3] = v.w; a[4] = w.x; a[5] = w.y; a[6] = w.z; a[7] = w.w;
   }
 };
 
@@ -186,22 +160,13 @@ struct Gemm {           // rows x (sum of segs) weight block in shared memory
 };
 
 // acc[r][u] += sum_{c4 in [lo,hi)} W[r][4*(col4+c4) .. +3] . act[4*c4 .. +3][u0 .. u0+U)
-// The activation loads come from L2 (about a microsecond under load) and only 3 warps share a scheduler, so they are software
-// pipelined two iterations (8 k rows) ahead in registers: three rotating buffers, loads of c4+2 issued before the
-// FMAs of c4.
-#ifndef B200_GRID_RS2_FULL
-#define B200_GRID_RS2_FULL 0
-#endif
-#ifndef B200_GRID_FFMA2
-#define B200_GRID_FFMA2 1
-#endif
 template <int U, int RT>
 __device__ __forceinline__ void wide_fma4(float (&acc)[RT][U], const float4* __restrict__ W4, int ldw4, int c4,
                                           const float (&a)[4][U]) {
 #pragma unroll
   for (int r = 0; r < RT; ++r) {
     float4 w = W4[r * ldw4 + c4];
-    if constexpr (B200_GRID_FFMA2 && U % 2 == 0) {
+    if constexpr (U % 2 == 0) {
       // two utterances against ONE weight register per step (fma2_rn: two scalar FFMAs on Hopper, which has no packed
       // fp32 FMA) -- bit-identical to the scalar loop below (same rounding, same summation order per lane).
 #pragma unroll
@@ -230,8 +195,9 @@ __device__ __forceinline__ void wide_ld4(float (&a)[4][U], const float* __restri
   for (int kk = 0; kk < 4; ++kk) ActLoad<U>::ld(p + kk * Bp, a[kk]);
 }
 // n float4 weight columns starting at W4 (row stride ldw4), activation rows starting at `ap` (row stride Bp floats).
-// Steady state: the loads of the NEXT PD columns are issued before the PD x 4*RT*U FMAs of the current ones (ping-pong
-// register buffers, 4*PD LDG.128 in flight per thread), addresses advance by pointer bumps.
+// The activation loads come from L2 (about a microsecond under load), so they are software pipelined: the loads of the
+// NEXT PD columns are issued before the PD x 4*RT*U FMAs of the current ones (ping-pong register buffers, 4*PD LDG.128 in
+// flight per thread), addresses advance by pointer bumps.
 template <int U, int RT, int PD>
 __device__ __forceinline__ void wide_accumulate_pd(float (&acc)[RT][U], const float* __restrict__ W, int ldw, int col4,
                                                    const float* __restrict__ act, int Bp_, int u0, int lo, int hi) {
@@ -274,9 +240,9 @@ __device__ __forceinline__ void wide_accumulate_pd(float (&acc)[RT][U], const fl
 template <int U, int RT>
 __device__ __forceinline__ void wide_accumulate(float (&acc)[RT][U], const float* __restrict__ W, int ldw, int col4,
                                                 const float* __restrict__ act, int Bp, int u0, int lo, int hi) {
-  // measured on the previous GPU: 3-4 columns ahead on the 4/8-row tiles is slower
-  constexpr int PD = (B200_GRID_NW_WIDE >= 16) ? ((RT * U <= 32) ? B200_GRID_PD16_SMALL : B200_GRID_PD16) : 2;
-  wide_accumulate_pd<U, RT, PD>(acc, W, ldw, col4, act, Bp, u0, lo, hi);
+  // one column of look-ahead: the 16-warp build leaves 128 registers per thread, and on the previous GPU 3-4 columns ahead
+  // was slower also on the 4/8-row tiles, which have registers to spare
+  wide_accumulate_pd<U, RT, 1>(acc, W, ldw, col4, act, Bp, u0, lo, hi);
 }
 
 // Wide mapping: NG GEMMs of RT rows each; 8 warps = NG x UW (utterance warps) x KS (k slices).
@@ -325,17 +291,14 @@ __device__ __forceinline__ void wide_partials(float* part, const Gemm& g0, const
   for (int r = 0; r < RTT; ++r) ActLoad<U>::st(dst + r * BT, acc[r]);
 }
 
-// Narrow mapping (Bp == G <= 8): the whole activation vector of the phase is first staged into shared memory by all
+// Narrow mapping (Bp == G == 4): the whole activation vector of the phase is first staged into shared memory by all
 // threads (ONE L2 round trip), then lanes stride over float4 columns, RT rows per warp pass, shuffle reduction.
 // Warps [wbeg, wbeg+wcnt) take part.  Result in out[(gslot*nrows + r)*G + u].
 template <int G>
 __device__ __forceinline__ void smem_ld(const float* p, float (&a)[G]) {
+  static_assert(G == 4, "one float4 per activation row");
   const float4 v = *reinterpret_cast<const float4*>(p);
   a[0] = v.x; a[1] = v.y; a[2] = v.z; a[3] = v.w;
-  if constexpr (G == 8) {
-    const float4 w = *(reinterpret_cast<const float4*>(p) + 1);
-    a[4] = w.x; a[5] = w.y; a[6] = w.z; a[7] = w.w;
-  }
 }
 template <int NT>
 __device__ __forceinline__ void stage_rows(float* dst, const float* __restrict__ src, int nfloats, int tid) {
@@ -389,11 +352,11 @@ template <int U, int UW, int GROUPS> struct MapTraits {
   static constexpr int NW = kGridWarpsWide;                                // warps per CTA
   static constexpr int NWG = NW / GROUPS;                                  // warps per group
   static constexpr int BT = 32 * U * UW;                                   // utterances per group tile
-  static constexpr int RS12 = (NW >= 16 && UW == 1) ? 2 : 1;               // row slices of the 12-row GRU tiles (16-warp build:
+  static constexpr int RS12 = (UW == 1) ? 2 : 1;                           // row slices of the 12-row GRU tiles (16-warp build:
                                                                            // 128 registers/thread -> 4 utterances x 6 rows)
   static constexpr int KS1 = NWG / UW;                                     // k slices of the 4/8-row 1-GEMM phases (fc1/fc2/fc3)
   static constexpr int KSB = NWG / (UW * RS12);                            // ... of the 12-row 1-GEMM pass of P01 (W_hh1)
-  static constexpr int RS2 = (B200_GRID_RS2_FULL && U == 4 && GROUPS == 2) ? 1 : RS12;   // row slices in the 2-GEMM phase (GRU 2)
+  static constexpr int RS2 = RS12;                                         // row slices in the 2-GEMM phase (GRU 2)
   static constexpr int KS2 = NWG / (2 * UW * RS2);                         // ... of the 2-GEMM phase (GRU 2)
   static constexpr int kPartRows = KSB * 12 > KS1 * 8 ? KSB * 12 : KS1 * 8;
   static constexpr int kPartFloats = (kPartRows > 2 * KS2 * 12 ? kPartRows : 2 * KS2 * 12) * BT;   // largest partial-sum footprint
@@ -474,9 +437,10 @@ __global__ void __launch_bounds__(MapTraits<U, UW, GROUPS>::NW * 32, 1) wavernn_
   unsigned int nbar = 0;
   const unsigned int ncta = gridDim.x;
   __shared__ int s_ok[2];                             // outcome of the group's last barrier wait
-  // Split barriers paid off on the previous GPU when ONE group owns the SM (B <= 128); with two groups the other group
-  // already fills the barrier bubble and the split was slower, so it is off there.  Not re-measured on the H100.
-  constexpr int kSplit = (GROUPS == 1) ? B200_GRID_SPLIT_BARRIER : 0;
+  // Split barriers.  0: plain barriers; 1: P01's GEMMs run before the wait on P5's barrier; 2: also GRU-2's W_hh pass starts
+  // before the wait on P01's barrier.  They paid off on the previous GPU when ONE group owns the SM (B <= 128); with two groups
+  // the other group already fills the barrier bubble and the split was slower, so it is off there.  Not re-measured on the H100.
+  constexpr int kSplit = (GROUPS == 1) ? 2 : 0;
   bool pending = false;                               // arrived at the sampling barrier of the previous step, not yet waited
   unsigned int pend_target = 0;
   const size_t RB = (size_t)R * Bp;
@@ -752,6 +716,12 @@ __global__ void __launch_bounds__(MapTraits<U, UW, GROUPS>::NW * 32, 1) wavernn_
     }
   }
 }
+
+// Instantiated here, ahead of wavernn_tc.cuh, so that this kernel is the module's first user of `smem`.  ptxas aligns an
+// extern shared array to the largest alignment among those the module declares before it; declaring `smem` ahead of
+// wavernn_tc_kernel's 1024-byte aligned `tsm` lets the grid and push kernels' weight blobs start right behind their static
+// shared variables.
+template __global__ void wavernn_grid_kernel<0, 4, 1>(GridModel, GridArgs);
 
 // conditioning in the K-major layout the grid kernel streams: mels_T[t][c][u], aux_T[fr][o][u]
 __global__ void mel_fir_T_kernel(const float* __restrict__ mel /*[B][feat][T]*/, const float* __restrict__ fir, int B, int Bp,

@@ -42,6 +42,7 @@ namespace b200tts {
 
 constexpr int kPushThreads = 512;
 constexpr int kPushWarps = kPushThreads / 32;
+constexpr int kPushMaxRows = 32;    // rows of the widest variant, wavernn_push_kernel<32>; larger batches run other kernels
 constexpr uint32_t kPushSentinel = 0xFFFFFFFFu;
 constexpr int kPushCondRows = 52;   // per CTA and frame: 16 mel projections | 16 + 12 + 4 + 4 aux projections (+ bias)
 constexpr int kPushVecs = 6;        // h1, x1, h2, x2, f1, f2
@@ -66,7 +67,8 @@ struct PushArgs {
   const float* fir;              // [hop][NT] composite polyphase FIR of the upsampling network
   int NT;
   int B, S, T, hop, steps;
-  int ng;                        // multi-group kernel (wavernn_pushmg.cuh): groups of 32 rows; vec is [ng][6][2][ncta][32][4], best [ng][ncta][32]
+  int reserved;                  // unused; it keeps the offsets of the fields below, and ptxas's register allocation of the
+                                 // push kernels follows those offsets
   int row_stride;                // 0: row u is utterance u.  > 0 (fold-with-overlap): row u = samples [u*row_stride, ...) of utterance 0
   int S_src;                     // samples of the source utterance (conditioning is ZERO beyond, fatchord_version.py:315-317)
   int rng_mode;
@@ -87,9 +89,10 @@ struct PushArgs {
 };
 
 struct PushRowState {            // per-row bookkeeping in shared memory (normal mode: row u == utterance u from step 0, forever)
-  int utt[32], t0[32], end[32], k[32];     // current segment: utterance (-1 idle), first step, first step of the NEXT segment, index
-  int putt[32], pn[32];                    // (utterance, local step) the row was at in the PREVIOUS step (whose winner P01 collects)
-  int rst[32];                             // the current step is the first of a segment: x = 0, h1 = h2 = 0
+  // current segment: utterance (-1 idle), first step, first step of the NEXT segment, index
+  int utt[kPushMaxRows], t0[kPushMaxRows], end[kPushMaxRows], k[kPushMaxRows];
+  int putt[kPushMaxRows], pn[kPushMaxRows];   // (utterance, local step) the row was at in the PREVIOUS step (whose winner P01 collects)
+  int rst[kPushMaxRows];                      // the current step is the first of a segment: x = 0, h1 = h2 = 0
 };
 // (utterance, local step) of row u at step t+1, seen from step t
 __device__ __forceinline__ void push_row_next(const PushArgs& A, const PushRowState& R, int u, int t1, int& utt, int& n) {
@@ -180,7 +183,8 @@ template <int G> struct PushTraits {
   static constexpr int NKB = 128 / NKQ;                    // producer blocks (float4 columns) per thread and row
   static constexpr int NL = NKB * UT;                      // float4 loads per thread and vector = G/4
   static constexpr int kPartFloats = kPushWarps * 16 * G;        // up to 16 rows per pass (W_ih2 12 + fc1 4 on x1)
-  static_assert(NU >= 4 && NU <= 32 && NKQ * NKB == 128 && NL * 4 == G && (32 / NU) * NKB == 8 && (NKB == 1 || NKB == 2 || NKB == 4), "mapping");
+  static_assert(G <= kPushMaxRows && NU >= 8 && NU <= 32 && NKQ * NKB == 128 && NL * 4 == G && (32 / NU) * NKB == 8 && (NKB == 2 || NKB == 4),
+                "mapping");
   // shared memory after the weight blob (floats)
   static constexpr int oPartX = 0;
   static constexpr int oPartY = oPartX + kPartFloats;
@@ -197,7 +201,7 @@ template <int G> struct PushTraits {
 // ---- one GEMM pass over this thread's NKB producer blocks x UT rows.  The 128 four-term dot products of an output (one
 //      per producer block kb) are combined in ONE fixed order for every G: pairwise by bit 0, 1, 2 of kb (inside the thread
 //      while it owns the pair, by warp shuffle otherwise; 8 consecutive kb per warp for every G), then the 16 warps in
-//      sequence (push_part_sum).  A row's result is therefore bit-identical whatever batch it is generated in (G = 4 ... 32),
+//      sequence (push_part_sum).  A row's result is therefore bit-identical whatever batch it is generated in (G = 8 ... 32),
 //      which is what lets N ranks reproduce the single-rank labels exactly.  Partials to part[(warp*ROWS + r)*G + u]. -------
 template <int G>
 __device__ __forceinline__ void push_load(const float* vecbase, float4 (&a)[PushTraits<G>::NL], int ul, int kq, PollGuard& pg) {
@@ -243,8 +247,7 @@ __device__ __forceinline__ void push_mma(const float* __restrict__ W /*[ROWS][51
 #pragma unroll
     for (int j = 0; j < UT; ++j) {
       if constexpr (NKB == 4) acc[r][j] = (leaf[0][j] + leaf[1][j]) + (leaf[2][j] + leaf[3][j]);
-      else if constexpr (NKB == 2) acc[r][j] = leaf[0][j] + leaf[1][j];
-      else acc[r][j] = leaf[0][j];
+      else acc[r][j] = leaf[0][j] + leaf[1][j];
     }
   }
   // the remaining levels of the 8-block tree: k queues that share the warp sit at lanes ul + NU*m

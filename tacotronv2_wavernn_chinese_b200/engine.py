@@ -237,8 +237,7 @@ class WaveRNNEngine:
     def launch_count(self) -> int:
         return int(self.lib.b200tts_wavernn_launch_count(self._h))
 
-    KERNEL_NAMES = {0: None, 1: 'wavernn_utt_kernel', 2: 'wavernn_grid_kernel', 3: 'wavernn_push_kernel', 4: 'wavernn_pushmg_kernel',
-                    5: 'wavernn_tc_kernel'}
+    KERNEL_NAMES = {0: None, 1: 'wavernn_utt_kernel', 2: 'wavernn_grid_kernel', 3: 'wavernn_push_kernel', 5: 'wavernn_tc_kernel'}
 
     def last_kernel(self):
         """Name of the step kernel the last generate call ran."""

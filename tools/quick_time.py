@@ -17,10 +17,7 @@ for k in kernels:
             ms = eng.last_kernel_ms()
         if os.environ.get('B200TTS_GRID_PROF') and k == 'grid':
             pc = eng.debug_phase_cycles() / steps
-            if 32 < B <= 256 and os.environ.get('B200TTS_PUSH', '1') != '0':  # multi-group push kernel: one slot per phase loop
-                names = ['P01', 'P2+hh1', 'P3+hh2', 'P4+cond', 'P5']
-                print('   cycles/step:', ' '.join(f'{n}={v:.0f}' for n, v in zip(names, pc.reshape(-1))), f' total {pc.sum():.0f}')
-            elif B <= 32 and os.environ.get('B200TTS_PUSH', '1') != '0':      # push kernel: 11 slots of thread 0 (see PUSH_MARK)
+            if B <= 32:                                      # push kernel: 11 slots of thread 0 (see PUSH_MARK)
                 names = ['P01poll', 'P01gate', 'P2gemm', 'P2gate', 'hh1', 'P3gemm', 'P3gate+hh2', 'P4gemm', 'P4gate+cond', 'P5gemm', 'P5sample', '-']
                 print('   cycles/step:', ' '.join(f'{n}={v:.0f}' for n, v in zip(names, pc.reshape(-1))), f' total {pc.sum():.0f}')
             else:
