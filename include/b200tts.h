@@ -221,6 +221,18 @@ int b200tts_taco_decode_forced(b200tts_taco* ctx, const float* d_memory, const i
                                const b200tts_taco_dropout* dropout, int n_steps, int window, const float* d_states,
                                float* d_frames, float* d_stop, float* d_align, int32_t* d_nsteps, void* stream);
 
+/* Ground-truth-aligned (GTA) decoding, the teacher-forced loop of wavernn_preprocess.py (TacoTrainingHelper, helpers.py:111-151):
+ * the step-t input is d_targets[b][t-1] (the zero GO frame at t = 0) instead of the previous output, and exactly
+ * clamp(d_target_lengths[b], 0, Ty_max) steps run.  No stop rule, no inference window (the reference builds this attention with
+ * is_training = True), no stop output; prenet dropout stays on and draws the same stream as b200tts_taco_decode, so fed a free
+ * run's own raw frames with the same dropout descriptor this replays that run.  One thread block per sentence at every B.
+ * d_targets [B][Ty_max][num_mels] used as given (the reference clips them to +-max_abs_value first); d_frames
+ * [B][Ty_max][num_mels] raw decoder outputs; d_align [B][Ty_max][Tx_max] or NULL; EXT masks [B][Ty_max][2][prenet_units].
+ * Rows at or beyond a sentence's step count are left untouched.  Bad arguments return B200TTS_EINVAL and launch nothing. */
+int b200tts_taco_decode_gta(b200tts_taco* ctx, const float* d_memory, const int32_t* d_lengths, int B, int Tx_max,
+                            const b200tts_taco_dropout* dropout, const float* d_targets, const int32_t* d_target_lengths,
+                            int Ty_max, float* d_frames, float* d_align, void* stream);
+
 /* Run-once neighbours of the decoder loop (available when b200tts_taco_create also received the encoder / postnet
  * variables):
  *   b200tts_taco_encode   <- embedding lookup + EncoderConvolutions + EncoderRNN   tacotron.py:44-57, modules.py:145-217

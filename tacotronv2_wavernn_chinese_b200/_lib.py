@@ -108,6 +108,8 @@ SIGNATURES = {
     'b200tts_taco_state_floats': (C.c_int, [C.c_void_p, C.c_int]),
     'b200tts_taco_decode_forced': (C.c_int, [C.c_void_p, C.c_void_p, C.c_void_p, C.c_int, C.c_int, C.POINTER(TacoDropout), C.c_int,
                                              C.c_int, C.c_void_p, C.c_void_p, C.c_void_p, C.c_void_p, C.c_void_p, C.c_void_p]),
+    'b200tts_taco_decode_gta': (C.c_int, [C.c_void_p, C.c_void_p, C.c_void_p, C.c_int, C.c_int, C.POINTER(TacoDropout), C.c_void_p,
+                                          C.c_void_p, C.c_int, C.c_void_p, C.c_void_p, C.c_void_p]),
     'b200tts_taco_encode': (C.c_int, [C.c_void_p, C.c_void_p, C.c_void_p, C.c_int, C.c_int, C.c_void_p, C.c_void_p]),
     'b200tts_taco_postnet': (C.c_int, [C.c_void_p, C.c_void_p, C.c_void_p, C.c_int, C.c_int, C.c_void_p, C.c_void_p]),
     'b200tts_taco_philox_masks': (C.c_int, [C.c_int, C.c_uint64, C.c_uint64, C.c_int, C.c_int, C.c_int, C.c_void_p, C.c_void_p]),

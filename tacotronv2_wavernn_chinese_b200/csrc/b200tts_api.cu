@@ -1553,6 +1553,13 @@ extern "C" void b200tts_taco_destroy(b200tts_taco* ctx) {
   delete ctx;
 }
 
+// dynamic shared memory of taco_decoder_kernel (its carve-up, plus 16 K floats of split-K partials)
+static size_t taco_decoder_smem_bytes(const TacoWeights& w) {
+  const size_t fl = 128 + w.P + (w.P + w.E + w.U) + 2 * w.U + 4 * w.U + 2 * w.U + (w.U + w.E) + w.A + 3 * kTacoMaxTx + 96 + 64 +
+                    (size_t)w.KW * w.NF + (size_t)w.NF * w.A + 16384;
+  return fl * sizeof(float);
+}
+
 static int taco_decode_impl(b200tts_taco* ctx, const float* d_memory, const int32_t* d_lengths, int B, int Tx_max,
                             const b200tts_taco_dropout* dropout, int max_steps, int window, const float* d_forced, float* d_frames,
                             float* d_stop, float* d_align, int32_t* d_nsteps, void* stream) {
@@ -1608,11 +1615,9 @@ static int taco_decode_impl(b200tts_taco* ctx, const float* d_memory, const int3
     ctx->launches += 4;
     return B200TTS_OK;
   }
-  size_t fl = 128 + w.P + (w.P + w.E + w.U) + 2 * w.U + 4 * w.U + 2 * w.U + (w.U + w.E) + w.A + 3 * kTacoMaxTx + 96 + 64 +
-              (size_t)w.KW * w.NF + (size_t)w.NF * w.A + 16384;
-  size_t smem = fl * sizeof(float);
-  B200_CUDA(cudaFuncSetAttribute(taco_decoder_kernel, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)smem));
-  taco_decoder_kernel<<<B, kTacoThreads, smem, st>>>(w, a);
+  const size_t smem = taco_decoder_smem_bytes(w);
+  B200_CUDA(cudaFuncSetAttribute(taco_decoder_kernel<false>, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)smem));
+  taco_decoder_kernel<false><<<B, kTacoThreads, smem, st>>>(w, a, TacoGtaArgs{});
   B200_CUDA(cudaGetLastError());
   ctx->launches += 2;
   API_END
@@ -1639,6 +1644,37 @@ extern "C" int b200tts_taco_decode_forced(b200tts_taco* ctx, const float* d_memo
   }
   return taco_decode_impl(ctx, d_memory, d_lengths, B, Tx_max, dropout, n_steps, window, d_states, d_frames, d_stop, d_align, d_nsteps,
                           stream);
+}
+
+extern "C" int b200tts_taco_decode_gta(b200tts_taco* ctx, const float* d_memory, const int32_t* d_lengths, int B, int Tx_max,
+                                       const b200tts_taco_dropout* dropout, const float* d_targets, const int32_t* d_target_lengths,
+                                       int Ty_max, float* d_frames, float* d_align, void* stream) {
+  API_BEGIN
+  REQUIRE(ctx && d_memory && d_lengths && dropout && d_targets && d_target_lengths && d_frames, B200TTS_EINVAL, "null argument");
+  REQUIRE(B >= 1 && Tx_max >= 1 && Tx_max <= kTacoMaxTx && Ty_max >= 1, B200TTS_EINVAL, "B, Tx_max (<= 512), Ty_max out of range");
+  const b200tts_taco_dropout d = *dropout;
+  REQUIRE(d.mode == B200TTS_TACO_DROPOUT_PHILOX || (d.mode == B200TTS_TACO_DROPOUT_EXT && d.d_masks), B200TTS_EINVAL,
+          "bad dropout descriptor");
+  DeviceGuard dg(ctx->device);
+  cudaStream_t st = (cudaStream_t)stream;
+  const TacoWeights& w = ctx->tw;
+  ctx->keys.ensure((size_t)B * Tx_max * w.A * sizeof(float));
+  taco_keys_kernel<<<B * Tx_max, 128, w.E * sizeof(float), st>>>(d_memory, w.mem_k, B * Tx_max, w.E, w.A, ctx->keys.as<float>());
+  B200_CUDA(cudaGetLastError());
+  // one CTA per sentence at every B: a batch job, so the single-sentence grid decoder is not taught the fed frame
+  TacoArgs a{};
+  a.memory = d_memory; a.keys = ctx->keys.as<float>(); a.lengths = d_lengths;
+  a.B = B; a.Tx_max = Tx_max; a.max_steps = Ty_max; a.window = 0;
+  a.rng_mode = d.mode; a.seed = d.seed; a.utt_offset = d.utterance_offset; a.masks = d.d_masks;
+  a.frames = d_frames; a.align = d_align;
+  TacoGtaArgs g{};
+  g.targets = d_targets; g.target_lengths = d_target_lengths;
+  const size_t smem = taco_decoder_smem_bytes(w);
+  B200_CUDA(cudaFuncSetAttribute(taco_decoder_kernel<true>, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)smem));
+  taco_decoder_kernel<true><<<B, kTacoThreads, smem, st>>>(w, a, g);
+  B200_CUDA(cudaGetLastError());
+  ctx->launches += 2;
+  API_END
 }
 
 extern "C" int b200tts_taco_philox_masks(int device, uint64_t seed, uint64_t utterance_offset, int B, int steps, int prenet_units,

@@ -1,6 +1,7 @@
 // Tacotron-2 forward-attention decoder loop on the GPU: one persistent CTA per sentence runs the whole
 // dynamic_decode while-loop (prenet -> 2 x zoneout LSTM -> forward location-sensitive attention -> frame / stop
-// projections -> feed the frame back) until its own stop token fires.
+// projections -> feed the frame back) until its own stop token fires.  The teacher-forced instantiation (kTeacher = true) runs
+// the same step with the recorded mel fed back instead, for a fixed number of steps: ground-truth-aligned (GTA) mels.
 //
 // Replaces (reference paths relative to the reference root):
 //   TacotronDecoderCell.__call__        tacotron/models/Architecture_wrappers.py:175-218
@@ -9,6 +10,7 @@
 //   ForwardLocationSensitiveAttention   tacotron/models/attention.py:119-231  (+ window mode forward_attention.py:171-215)
 //   FrameProjection / StopProjection    tacotron/models/modules.py:304, :334-342
 //   CustomDecoder.step + TacoTestHelper tacotron/models/custom_decoder.py:105-135, helpers.py:36-66
+//   TacoTrainingHelper (kTeacher)       helpers.py:111-151 (next input = targets[:, time], exactly len(targets) steps)
 // Weights stay in TensorFlow's [in, out] layout: thread j of a matvec reads K[i][4j..4j+3] -- coalesced as is.
 // ~6.9 MB of weights are streamed from L2 per step per CTA (first correct version; the weight-stationary multi-CTA
 // form used for WaveRNN is the planned optimisation).
@@ -50,6 +52,12 @@ struct TacoArgs {
   // step and the stop rule is ignored (exactly max_steps steps run): [B][max_steps][taco_state_floats(Tx_max)] laid out as
   //   x[mels] | ctx[E] | c1[U] | h1[U] | c2[U] | h2[U] | mu | max_att | pos_rec | 0 | cum[Tx_max] | alpha[Tx_max]
   const float* forced;
+};
+// Teacher forcing from a recorded mel (GTA, wavernn_preprocess.py): its own struct, so that TacoArgs -- and with it the code of
+// the free-running instantiation -- stays as it was.
+struct TacoGtaArgs {
+  const float* targets;         // [B][max_steps][mels]: the step-t input is targets[b][t-1] (the zero GO frame at t = 0)
+  const int* target_lengths;    // [B]: steps run = clamp(target_lengths[b], 0, max_steps); no stop rule, no stop output
 };
 __host__ __device__ inline int taco_state_floats(int mels, int E, int U, int Tx_max) { return mels + E + 4 * U + 4 + 2 * Tx_max; }
 
@@ -141,12 +149,15 @@ __device__ __forceinline__ float block_max(float v, float* red) {
   return red[0];
 }
 
-__global__ void __launch_bounds__(kTacoThreads, 1) taco_decoder_kernel(TacoWeights W, TacoArgs A) {
+// kTeacher = false: free running (b200tts_taco_decode / _decode_forced).  kTeacher = true: GTA (b200tts_taco_decode_gta) --
+// no forced-state reload, no window, no stop projection or rule, no stop / nsteps outputs (A.stop, A.nsteps unused).
+template <bool kTeacher>
+__global__ void __launch_bounds__(kTacoThreads, 1) taco_decoder_kernel(TacoWeights W, TacoArgs A, TacoGtaArgs G) {
   extern __shared__ __align__(16) float sm[];
   const int b = blockIdx.x, tid = threadIdx.x;
   const int Tx = min(A.lengths[b], A.Tx_max);
   if (Tx < 1) {                                        // empty sentence: nothing to attend to
-    if (tid == 0) A.nsteps[b] = 0;
+    if (!kTeacher && tid == 0) A.nsteps[b] = 0;
     return;
   }
   const int P = W.P, U = W.U, E = W.E, AD = W.A, NF = W.NF, KW = W.KW, M = W.mels;
@@ -187,9 +198,10 @@ __global__ void __launch_bounds__(kTacoThreads, 1) taco_decoder_kernel(TacoWeigh
   const float* keys = A.keys + (size_t)b * A.Tx_max * AD;
   const float zo = W.zoneout, zk = 1.f - W.zoneout;
 
+  const int n_steps = kTeacher ? min(max(G.target_lengths[b], 0), A.max_steps) : A.max_steps;
   int step = 0;
-  for (; step < A.max_steps; ++step) {
-    if (A.forced) {                                        // teacher forcing: reload the whole state (see TacoArgs::forced)
+  for (; step < n_steps; ++step) {
+    if (!kTeacher && A.forced) {                                        // teacher forcing: reload the whole state (see TacoArgs::forced)
       const float* st = A.forced + ((size_t)b * A.max_steps + step) * taco_state_floats(M, E, U, A.Tx_max);
       for (int i = tid; i < M; i += kTacoThreads) x[i] = st[i];
       for (int i = tid; i < E; i += kTacoThreads) ctxv[i] = st[M + i];
@@ -299,7 +311,7 @@ __global__ void __launch_bounds__(kTacoThreads, 1) taco_decoder_kernel(TacoWeigh
       fs += v;
     }
     __syncthreads();
-    if (A.window) {                                                            // forward_attention.py:171-215
+    if (!kTeacher && A.window) {                                               // forward_attention.py:171-215
       if (tid == 0) {
         int am = 0; float best = al[0];
         for (int t = 1; t < Tx; ++t) if (al[t] > best) { best = al[t]; am = t; }
@@ -355,7 +367,15 @@ __global__ void __launch_bounds__(kTacoThreads, 1) taco_decoder_kernel(TacoWeigh
     }
     // mu' = sigmoid([context | query_in] . Wmu + b)   (attention.py:229: concat order is [context, query])
     // stop = sigmoid([o2 | context] . Ws + b)          (Architecture_wrappers.py:196-199)
-    {
+    if constexpr (kTeacher) {
+      float pm = 0.f;
+      for (int i = tid; i < U + E; i += kTacoThreads) {
+        const int mi = (i < U) ? (E + i) : (i - U);
+        pm = fmaf(pin[i], W.mu_k[mi], pm);
+      }
+      const float sm_ = block_sum(pm, red);
+      if (tid == 0) s_mu = sigmoidf_acc(sm_ + W.mu_b[0]);
+    } else {
       float pm = 0.f, ps = 0.f;
       for (int i = tid; i < U + E; i += kTacoThreads) {
         const float vin = pin[i];                       // i < U: o2[i] ; else context[i-U]
@@ -372,13 +392,22 @@ __global__ void __launch_bounds__(kTacoThreads, 1) taco_decoder_kernel(TacoWeigh
     for (int i = tid; i < M; i += kTacoThreads) {
       const float v = fo[i];
       A.frames[((size_t)b * A.max_steps + step) * M + i] = v;
-      x[i] = v;                                          // next input = this frame (r = 1, helpers.py:64)
+      if constexpr (kTeacher)
+        x[i] = G.targets[((size_t)b * A.max_steps + step) * M + i];   // next input = the recorded frame (helpers.py:142)
+      else
+        x[i] = v;                                        // next input = this frame (r = 1, helpers.py:64)
     }
-    if (tid == 0) A.stop[(size_t)b * A.max_steps + step] = s_stop;
+    if constexpr (!kTeacher) {
+      if (tid == 0) A.stop[(size_t)b * A.max_steps + step] = s_stop;
+    }
     __syncthreads();
-    if (s_stop > 0.5f && !A.forced) { ++step; break; }   // finished = round(stop) (half-to-even -> strictly > 0.5)
+    if constexpr (!kTeacher) {
+      if (s_stop > 0.5f && !A.forced) { ++step; break; }   // finished = round(stop) (half-to-even -> strictly > 0.5)
+    }
   }
-  if (tid == 0) A.nsteps[b] = step;
+  if constexpr (!kTeacher) {
+    if (tid == 0) A.nsteps[b] = step;
+  }
 }
 
 // keep flags the PHILOX mode uses, [B][steps][2][P] (lets a test replay them through the oracle)

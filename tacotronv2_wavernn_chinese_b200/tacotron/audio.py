@@ -26,6 +26,8 @@ tacotron/datasets/preprocessor.py:52-121, without the file I/O):
   4. melspectrogram: |stft|^2, Slaney filterbank, 20 log10(max(1e-5, .)) - 20, symmetric +-4 with clipping  (:95-102)
   5. the training audio: the rescaled trimmed wav zero-padded to T * 275 samples                          (preprocessor :100-111)
 `melspectrogram(wav, hparams)` is step 4 alone, as in the reference.
+
+`encode_mu_law` is the vocoder-training quantiser wavernn_preprocess.py applies to that training audio (audio.py:8-11).
 """
 from __future__ import annotations
 
@@ -243,3 +245,18 @@ def preprocess_batch(wavs, hparams, device=None):
 def preprocess_wav(wav, hparams):
     """One signal through `preprocess_batch`: (mel [T][num_mels], out [T * hop], (start, end))."""
     return preprocess_batch([wav], hparams)[0]
+
+
+def encode_mu_law(x, mu=2**10):
+    """The reference's `audio.encode_mu_law` (tacotron/datasets/audio.py:8-11): floor((F(x) + 1) / 2 * (mu - 1) + 0.5), F the
+    mu-law companding curve with mu - 1, as float values in [0, mu - 1].  The reference ran under numpy 1.x, where
+    `... / np.log(1 + mu)` divides a float32 array by a float64 scalar that value-based casting demotes to float32; so for the
+    float32 training audio every operation is float32, and the result is float32.  numpy 2 would promote that statement to
+    float64, which rounds some samples to the neighbouring level (tests/test_tacotron_gta_pins.py counts them), so the
+    arithmetic is spelled out here in the input's own float type (float64 for anything that is not float32)."""
+    x = np.asarray(x)
+    f = np.float32 if x.dtype == np.float32 else np.float64
+    x = x.astype(f, copy=False)
+    m = mu - 1
+    fx = np.sign(x) * np.log(f(1) + f(m) * np.abs(x)) / f(np.log(1 + m))
+    return np.floor((fx + f(1)) / f(2) * f(m) + f(0.5))

@@ -102,6 +102,50 @@ class TacoDecoderEngine:
                     t.record_stream(torch.cuda.current_stream(self.device))
         return dict(frames=frames, stop=stop, align=align, nsteps=nsteps)
 
+    def decode_gta(self, memory, lengths, targets, target_lengths, *, masks=None, seed=0, utterance_offset=0, want_align=False):
+        """Ground-truth-aligned decoding (b200tts_taco_decode_gta): teacher-forced on `targets` [B, Ty_max, num_mels] (used as
+        given; the reference clips them to +-4 first), exactly clamp(target_lengths[b], 0, Ty_max) steps per sentence.
+        memory [B, Tx, enc_dim]; lengths [B] or None (= Tx); target_lengths [B] or None (= Ty_max).  masks: optional uint8 keep
+        flags [B, Ty_max, 2, prenet_units] (EXT mode) else Philox(seed), the stream `decode` draws.  Returns dict(frames
+        [B, Ty_max, 80] raw decoder outputs, align [B, Ty_max, Tx] or None, nsteps [B] int32) as CUDA tensors; rows at or
+        beyond nsteps are zero."""
+        dev = self._dev()
+        m = torch.as_tensor(memory).to(device=dev, dtype=torch.float32).contiguous()
+        if m.dim() != 3 or m.shape[2] != self.cfg['enc_dim']:
+            raise ValueError(f'memory must be [B, Tx, {self.cfg["enc_dim"]}]')
+        B, Tx, _ = m.shape
+        tg = torch.as_tensor(targets).to(device=dev, dtype=torch.float32).contiguous()
+        if tg.dim() != 3 or tg.shape[0] != B or tg.shape[2] != self.cfg['num_mels'] or tg.shape[1] < 1:
+            raise ValueError(f'targets must be [{B}, Ty_max >= 1, {self.cfg["num_mels"]}]')
+        Ty = tg.shape[1]
+        ln = torch.full((B,), Tx, dtype=torch.int32) if lengths is None else torch.as_tensor(lengths, dtype=torch.int32)
+        if tuple(ln.shape) != (B,) or int(ln.max()) > Tx or int(ln.min()) < 1:
+            raise ValueError('lengths must be [B] in [1, Tx]')
+        tl = torch.full((B,), Ty, dtype=torch.int32) if target_lengths is None else torch.as_tensor(target_lengths, dtype=torch.int32)
+        if tuple(tl.shape) != (B,):
+            raise ValueError('target_lengths must be [B]')
+        tl = tl.clamp(0, Ty)
+        ln, tl = ln.to(dev), tl.to(dev)
+        with torch.cuda.device(self.device):
+            frames = torch.zeros(B, Ty, self.cfg['num_mels'], device=dev, dtype=torch.float32)
+            align = torch.zeros(B, Ty, Tx, device=dev, dtype=torch.float32) if want_align else None
+            d = TacoDropout()
+            d.seed = int(seed) & 0xFFFFFFFFFFFFFFFF
+            d.utterance_offset = int(utterance_offset)
+            md = None
+            if masks is not None:
+                md = torch.as_tensor(masks).to(device=dev, dtype=torch.uint8).contiguous()
+                if tuple(md.shape) != (B, Ty, 2, self.cfg['prenet_units']):
+                    raise ValueError('masks must be [B, Ty_max, 2, prenet_units]')
+                d.mode = 1
+                d.d_masks = md.data_ptr()
+            _lib.check(self.lib.b200tts_taco_decode_gta(self._h, _ptr(m), _ptr(ln), B, Tx, C.byref(d), _ptr(tg), _ptr(tl), Ty,
+                                                        _ptr(frames), _ptr(align), self._stream()))
+            for t in (m, ln, tg, tl, md):
+                if t is not None:
+                    t.record_stream(torch.cuda.current_stream(self.device))
+        return dict(frames=frames, align=align, nsteps=tl)
+
     def state_floats(self, Tx: int) -> int:
         return int(self.lib.b200tts_taco_state_floats(self._h, int(Tx)))
 

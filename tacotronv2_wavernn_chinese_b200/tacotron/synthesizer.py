@@ -7,6 +7,11 @@ Encoder, decoder loop and postnet all run through libb200tts (b200tts_taco_encod
 the reference's TF bundle read without TensorFlow (tacotron/ckpt.py).  The Griffin-Lim preview wav (:110-112) is written by
 tacotron_synthesize.py --griffin_lim from the saved mel (tacotron/audio.py inv_mel_spectrogram, on the GPU).  Not reproduced:
 the matplotlib PNGs the reference also writes (:111, :118-125) -- plotting is out of scope.
+
+Ground-truth-aligned mels for vocoder training (the reference's wavernn_preprocess.py, its own `Synthesizer`):
+
+    mels = synth.gta_mels(['m ao2 ...'], [target_mel])                        # teacher-forced on the recorded mel
+    synth.synthesize_gta(hanzi, 'mel-000001.npy', out_dir, '000001')          # writes mel-000001-pred.npy
 """
 from __future__ import annotations
 
@@ -17,6 +22,7 @@ import torch
 
 from . import ckpt
 from .engine import TacoDecoderEngine
+from .pinyin import get_pyin
 from .text import Symbols, build_symbols
 
 MAX_ABS_VALUE = 4.0          # tacotron_hparams.py:99, symmetric_mels=True -> T2_output_range = (-4, 4)
@@ -85,3 +91,44 @@ class Synthesizer:
         alignment_path = os.path.join(out_dir, f'step-{step}-{idx}-align.npy')
         np.save(alignment_path, align, allow_pickle=False)
         return pred_mel_path, alignment_path
+
+    def gta_mels(self, texts, targets, seed=0, utterance_offset=0):
+        """Ground-truth-aligned mels (wavernn_preprocess.py:72-120): pinyin strings + their recorded mels [T_b, 80] on the +-4
+        scale -> list of np.float32 [T_b, 80] in [0, 1].  Per sentence: the target is clipped to +-4 (:79; r = 1, so no
+        padding, :82), the decoder runs teacher-forced for exactly T_b steps (b200tts_taco_decode_gta), then the postnet; its
+        mel is clipped to +-4, cropped to T_b and mapped with clip((m + 4) / 8, 0, 1) (:101-106).  Prenet dropout is Philox
+        keyed by (seed, utterance_offset + b, step, unit): a sentence's mel does not depend on the batch it is decoded in."""
+        if len(texts) != len(targets) or not texts:
+            raise ValueError('need one target mel per text, and at least one text')
+        seqs = [self.symbols.text_to_sequence(t) for t in texts]
+        tg = [np.clip(np.asarray(t, dtype=np.float32), -MAX_ABS_VALUE, MAX_ABS_VALUE) for t in targets]
+        for t in tg:
+            if t.ndim != 2 or t.shape[1] != 80 or t.shape[0] < 1:
+                raise ValueError(f'target mels must be [T >= 1, 80], got {t.shape}')
+        B, Tx, Ty = len(seqs), max(len(s) for s in seqs), max(t.shape[0] for t in tg)
+        ids = np.zeros((B, Tx), dtype=np.int32)
+        tpad = np.zeros((B, Ty, 80), dtype=np.float32)
+        for b, (s, t) in enumerate(zip(seqs, tg)):
+            ids[b, :len(s)] = s
+            tpad[b, :t.shape[0]] = t
+        lengths = np.array([len(s) for s in seqs], dtype=np.int32)
+        tlen = np.array([t.shape[0] for t in tg], dtype=np.int32)
+        eng = self.engine
+        mem = eng.encode(ids, lengths)
+        dec = eng.decode_gta(mem, lengths, tpad, tlen, seed=seed, utterance_offset=utterance_offset)
+        mel_h = eng.postnet(dec['frames'], dec['nsteps']).cpu().numpy()
+        out = []
+        for b in range(B):
+            m = np.clip(mel_h[b, :tlen[b]], -MAX_ABS_VALUE, MAX_ABS_VALUE)
+            out.append(np.clip((m + MAX_ABS_VALUE) / (2 * MAX_ABS_VALUE), 0, 1).astype(np.float32))
+        return out
+
+    def synthesize_gta(self, text, mel_path, out_dir, idx, seed=0, utterance_offset=0):
+        """wavernn_preprocess.py:72-120 `Synthesizer.synthesize(text, mel, out_dir, idx)`: Hanzi text (through get_pyin, :85),
+        target mel `.npy` -> out_dir/mel-{idx}-pred.npy.  Returns (pred_mel_path, None): the alignment PNG is not drawn."""
+        pyin, _ = get_pyin(text)
+        mel = self.gta_mels([pyin], [np.load(mel_path)], seed=seed, utterance_offset=utterance_offset)[0]
+        os.makedirs(out_dir, exist_ok=True)
+        pred_mel_path = os.path.join(out_dir, f'mel-{idx}-pred.npy')
+        np.save(pred_mel_path, mel, allow_pickle=False)
+        return pred_mel_path, None
