@@ -163,8 +163,9 @@ struct b200tts_wavernn {
   PushModel pm{};                 // small-batch push kernel (wavernn_push.cuh): per-CTA blobs + conditioning-projection weights
   PushCondW pcw{};
   DeviceBuf push_blob, push_condw, push_tab, push_vec, push_best, push_prof;
-  DeviceBuf tc_wimg, tc_prm, tc_vec, tc_x1f, tc_win, tc_cnt, tc_cond;     // tensor-core pipeline (wavernn_tc.cuh)
+  DeviceBuf tc_wimg, tc_prm, tc_vec, tc_x1f, tc_win, tc_cnt, tc_cond, tc_prof;     // tensor-core pipeline (wavernn_tc.cuh)
   bool tc_ok = false;
+  bool last_tc_prof = false;      // the last tensor-core launch recorded phase counters
   int last_kernel = 0;            // 1 utterance, 2 wide grid, 3 push, 5 tensor-core pipeline
   int last_push_ncta = 0;
   int* d_grid_error = nullptr;    // set by the grid kernel when a barrier wait timed out (a peer CTA vanished)
@@ -601,6 +602,7 @@ extern "C" void b200tts_wavernn_destroy(b200tts_wavernn* ctx) {
   ctx->push_best.release();
   ctx->push_prof.release();
   ctx->tc_wimg.release(); ctx->tc_prm.release(); ctx->tc_vec.release(); ctx->tc_x1f.release(); ctx->tc_win.release(); ctx->tc_cnt.release(); ctx->tc_cond.release();
+  ctx->tc_prof.release();
   ctx->h_stage.release();
   if (ctx->ev0) cudaEventDestroy(ctx->ev0);
   if (ctx->ev1) cudaEventDestroy(ctx->ev1);
@@ -904,9 +906,9 @@ static void launch_push(b200tts_wavernn* ctx, const float* d_mel, GenArgs& ua, c
 }
 
 // ---- tensor-core pipeline (wavernn_tc.cuh): 33 ... 256 rows, plain batches ----------------------------------------------
-// Smallest batch kernel=auto gives the tensor cores.  On an H100 (80GB HBM3, 700 W) the tensor-core pipeline costs 62-66 us per
-// lock-step whatever the row count (1 or 2 groups of 128 rows in flight), the wide CUDA-core mapping 37.5 us at 64 rows, 60.9 at
-// 96-128 and 90-91 from 129 rows on (a second tile of 128).
+// Smallest batch kernel=auto gives the tensor cores.  On an H100 80GB HBM3 at a 400 W power limit the tensor-core pipeline costs
+// 38-41 us per lock-step whatever the row count (1 or 2 groups of 128 rows in flight; 64-69 us while its wgmma were serialized);
+// the wide CUDA-core mapping took 37.5 us at 64 rows, 60.9 at 96-128 and 90-91 from 129 rows on (a second tile of 128; 700 W).
 constexpr int kTcMinRows = 129;
 static bool tc_eligible(const b200tts_wavernn* ctx, int rows, bool folding, bool packing) {
   return ctx->tc_ok && ctx->pm.ok && !folding && !packing && rows >= 1 && rows <= kTcRows * kTcMaxGroups;
@@ -949,6 +951,13 @@ static void launch_tc(b200tts_wavernn* ctx, const float* d_mel, GenArgs& ua, cud
   a.NT = ctx->NT; a.B = rows; a.S = ua.S; a.T = T; a.hop = hop; a.steps = ua.steps; a.ng = ng; a.NC = ctx->NC;
   a.rng_mode = ua.rng_mode; a.seed = ua.seed; a.utt_offset = ua.utt_offset; a.utt_ids = ua.utt_ids; a.q = ua.q;
   a.teacher = ua.teacher; a.logits_out = ua.logits_out; a.labels = ua.labels;
+  a.prof = nullptr;
+  ctx->last_tc_prof = getenv("B200TTS_GRID_PROF") != nullptr;
+  if (ctx->last_tc_prof) {
+    ctx->tc_prof.ensure((size_t)kTcCtas * 12 * sizeof(long long));
+    B200_CUDA(cudaMemsetAsync(ctx->tc_prof.p, 0, (size_t)kTcCtas * 12 * sizeof(long long), st));
+    a.prof = ctx->tc_prof.as<long long>();
+  }
   ctx->last_push_ncta = 0;
   ctx->last_grid_ncta = 0;
   B200_CUDA(cudaFuncSetAttribute(wavernn_tc_kernel, cudaFuncAttributeMaxDynamicSharedMemorySize, kTcSmemBytes));
@@ -1265,9 +1274,28 @@ extern "C" int b200tts_debug_fp32_peak(int device, double* tflops) {
 
 // Debug: per-phase cycle counters of the last grid-kernel launch (needs env B200TTS_GRID_PROF=1 at generate time).
 // out[12] = mean over CTAs of {P0 compute, P0 barrier, P1 compute, P1 barrier, ...} in SM cycles.
+// Tensor-core pipeline: out[3 j + p] = cycles summed over the run of job j (GRU-2's W_ih2 . x1, fc1, fc2, fc3), phase p (exchange
+// wait, GEMM, epilogue), averaged over the CTAs of that role.
 extern "C" int b200tts_wavernn_debug_phase_cycles(b200tts_wavernn* ctx, double* out12) {
   API_BEGIN
   REQUIRE(ctx && out12, B200TTS_EINVAL, "null argument");
+  if (ctx->last_kernel == 5) {
+    REQUIRE(ctx->last_tc_prof && ctx->tc_prof.p, B200TTS_EINVAL, "no phase profile recorded");
+    DeviceGuard dg(ctx->device);
+    std::vector<long long> h((size_t)kTcCtas * 12);
+    B200_CUDA(cudaDeviceSynchronize());
+    B200_CUDA(cudaMemcpy(h.data(), ctx->tc_prof.p, h.size() * sizeof(long long), cudaMemcpyDeviceToHost));
+    int n[4] = {0, 0, 0, 0};
+    for (int i = 0; i < 12; ++i) out12[i] = 0;
+    for (int cta = 0; cta < kTcCtas; ++cta) {
+      const int j = tc_role(cta).role - 1;
+      if (j < 0) continue;
+      ++n[j];
+      for (int p = 0; p < 3; ++p) out12[3 * j + p] += (double)h[(size_t)cta * 12 + 3 * j + p];
+    }
+    for (int i = 0; i < 12; ++i) out12[i] /= n[i / 3];
+    return B200TTS_OK;
+  }
   const bool push = ctx->last_grid_ncta == 0 && ctx->last_push_ncta > 0 && ctx->push_prof.p;
   REQUIRE(push || (ctx->grid_prof.p && ctx->last_grid_ncta > 0), B200TTS_EINVAL, "no phase profile recorded");
   DeviceGuard dg(ctx->device);

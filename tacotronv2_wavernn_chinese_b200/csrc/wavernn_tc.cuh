@@ -39,6 +39,7 @@
 // (meaningless) MMAs to the end of the GEMM so that the warps of a wgmma never diverge, and the consumers leave together.
 #pragma once
 #include <cuda_fp16.h>
+#include <utility>
 #include "common.cuh"
 #include "wavernn_push.cuh"
 
@@ -48,7 +49,9 @@ constexpr int kTcConsumerWarps = 8;         // warps 0-3 / 4-7: the warpgroups o
 constexpr int kTcLoaderWarp = 8;
 constexpr int kTcCondWarp0 = 9;             // warps 9-11: conditioning (GRU-1 CTAs)
 constexpr int kTcCondWarps = 3;
-constexpr int kTcThreads = 12 * 32;         // 3 warps per SM sub-partition: up to 168 registers per thread
+constexpr int kTcThreads = 12 * 32;         // 3 warps per SM sub-partition: 168 registers per thread at launch, then
+constexpr int kTcConsumerRegs = 232;        // warpgroups 0-1 take what warpgroup 2 gives back (setmaxnreg):
+constexpr int kTcOtherRegs = 40;            // 2 x 128 x (232 - 168) = 128 x (168 - 40)
 constexpr int kTcRows = 128;                // rows per group
 constexpr int kTcMaxGroups = 2;
 constexpr int kTcStageBytes = 16384;        // K = 32 of one vector: [plane 2][k-step 2][k half 2][row group 16][8 rows][8 halves]
@@ -86,6 +89,8 @@ struct TcArgs {
   const int16_t* teacher;        // [B][S]
   float* logits_out;             // [S][B][NC]
   int16_t* labels;               // [B][S]
+  long long* prof;               // optional [128][12] cycle counters (B200TTS_GRID_PROF): slots 3 (role - 1) + {exchange wait,
+                                 // GEMM, epilogue} of one job per (step, group) -- GRU-2's x1 job, fc1, fc2, fc3 -- summed by thread 0
 };
 
 // ---- small PTX wrappers ------------------------------------------------------------------------------------------------
@@ -141,39 +146,47 @@ __device__ __forceinline__ uint64_t tc_desc(uint32_t saddr, uint32_t lbo_bytes, 
   d |= (uint64_t)(sbo_bytes >> 4) << 32;
   return d;
 }
-// D[64 x N] (+)= A[64 x 16] . B[16 x N], f16 operands from shared memory, fp32 accumulators in registers (accumulate = 0
-// overwrites D).  Fragment of a thread: D[4i + 2h + e] = (row 16 * (warp % 4) + lane / 4 + 8h, column 8i + 2 (lane % 4) + e).
-__device__ __forceinline__ void tc_wgmma32(float (&d)[16], uint64_t da, uint64_t db, uint32_t accumulate) {
-  asm volatile(
-      "{\n\t.reg .pred p;\n\tsetp.ne.b32 p, %18, 0;\n\t"
-      "wgmma.mma_async.sync.aligned.m64n32k16.f32.f16.f16 {%0,%1,%2,%3,%4,%5,%6,%7,%8,%9,%10,%11,%12,%13,%14,%15}, %16, %17, p, 1, 1, 0, 0;\n\t}\n"
+// D[64 x N] (+)= A[64 x 16] . B[16 x N], f16 operands from shared memory, fp32 accumulators in registers (ACC = 0 overwrites
+// D).  Fragment of a thread: D[4i + 2h + e] = (row 16 * (warp % 4) + lane / 4 + 8h, column 8i + 2 (lane % 4) + e).
+// The descriptors are da + AOFF and db + BOFF, added inside the asm: as plain C++ sums of loop-invariant bases the 64 B-operand
+// descriptors of a GEMM would be hoisted out of the step loop and held in registers for the whole launch.
+// Operands: DREGS, then da, db, AOFF, BOFF, ACC (I0 ... I0 + 4).
+#define TC_WGMMA_ASM(SHAPE, DREGS, A, B, AO, BO, ACC)                                                                            \
+  "{\n\t.reg .pred p;\n\t.reg .b64 da, db;\n\tsetp.ne.b32 p, " ACC ", 0;\n\t"                                                \
+  "add.s64 da, " A ", " AO ";\n\tadd.s64 db, " B ", " BO ";\n\t"                                                                 \
+  "wgmma.mma_async.sync.aligned." SHAPE ".f32.f16.f16 {" DREGS "}, da, db, p, 1, 1, 0, 0;\n\t}\n"
+template <int AOFF, int BOFF, int ACC>
+__device__ __forceinline__ void tc_wgmma32(float (&d)[16], uint64_t da, uint64_t db) {
+  asm volatile(TC_WGMMA_ASM("m64n32k16", "%0,%1,%2,%3,%4,%5,%6,%7,%8,%9,%10,%11,%12,%13,%14,%15",
+                            "%16", "%17", "%18", "%19", "%20")
       : "+f"(d[0]), "+f"(d[1]), "+f"(d[2]), "+f"(d[3]), "+f"(d[4]), "+f"(d[5]), "+f"(d[6]), "+f"(d[7]), "+f"(d[8]), "+f"(d[9]), "+f"(d[10]), "+f"(d[11]), "+f"(d[12]), "+f"(d[13]), "+f"(d[14]), "+f"(d[15])
-      : "l"(da), "l"(db), "r"(accumulate));
+      : "l"(da), "l"(db), "n"(AOFF), "n"(BOFF), "n"(ACC));
 }
-__device__ __forceinline__ void tc_wgmma48(float (&d)[24], uint64_t da, uint64_t db, uint32_t accumulate) {
-  asm volatile(
-      "{\n\t.reg .pred p;\n\tsetp.ne.b32 p, %26, 0;\n\t"
-      "wgmma.mma_async.sync.aligned.m64n48k16.f32.f16.f16 {%0,%1,%2,%3,%4,%5,%6,%7,%8,%9,%10,%11,%12,%13,%14,%15,%16,%17,%18,%19,%20,%21,%22,%23}, %24, %25, p, 1, 1, 0, 0;\n\t}\n"
+template <int AOFF, int BOFF, int ACC>
+__device__ __forceinline__ void tc_wgmma48(float (&d)[24], uint64_t da, uint64_t db) {
+  asm volatile(TC_WGMMA_ASM("m64n48k16", "%0,%1,%2,%3,%4,%5,%6,%7,%8,%9,%10,%11,%12,%13,%14,%15,%16,%17,%18,%19,%20,%21,%22,%23",
+                            "%24", "%25", "%26", "%27", "%28")
       : "+f"(d[0]), "+f"(d[1]), "+f"(d[2]), "+f"(d[3]), "+f"(d[4]), "+f"(d[5]), "+f"(d[6]), "+f"(d[7]), "+f"(d[8]), "+f"(d[9]), "+f"(d[10]), "+f"(d[11]), "+f"(d[12]), "+f"(d[13]), "+f"(d[14]), "+f"(d[15]), "+f"(d[16]), "+f"(d[17]), "+f"(d[18]), "+f"(d[19]), "+f"(d[20]), "+f"(d[21]), "+f"(d[22]), "+f"(d[23])
-      : "l"(da), "l"(db), "r"(accumulate));
+      : "l"(da), "l"(db), "n"(AOFF), "n"(BOFF), "n"(ACC));
 }
-__device__ __forceinline__ void tc_wgmma64(float (&d)[32], uint64_t da, uint64_t db, uint32_t accumulate) {
-  asm volatile(
-      "{\n\t.reg .pred p;\n\tsetp.ne.b32 p, %34, 0;\n\t"
-      "wgmma.mma_async.sync.aligned.m64n64k16.f32.f16.f16 {%0,%1,%2,%3,%4,%5,%6,%7,%8,%9,%10,%11,%12,%13,%14,%15,%16,%17,%18,%19,%20,%21,%22,%23,%24,%25,%26,%27,%28,%29,%30,%31}, %32, %33, p, 1, 1, 0, 0;\n\t}\n"
+template <int AOFF, int BOFF, int ACC>
+__device__ __forceinline__ void tc_wgmma64(float (&d)[32], uint64_t da, uint64_t db) {
+  asm volatile(TC_WGMMA_ASM("m64n64k16", "%0,%1,%2,%3,%4,%5,%6,%7,%8,%9,%10,%11,%12,%13,%14,%15,%16,%17,%18,%19,%20,%21,%22,%23,%24,%25,%26,%27,%28,%29,%30,%31",
+                            "%32", "%33", "%34", "%35", "%36")
       : "+f"(d[0]), "+f"(d[1]), "+f"(d[2]), "+f"(d[3]), "+f"(d[4]), "+f"(d[5]), "+f"(d[6]), "+f"(d[7]), "+f"(d[8]), "+f"(d[9]), "+f"(d[10]), "+f"(d[11]), "+f"(d[12]), "+f"(d[13]), "+f"(d[14]), "+f"(d[15]), "+f"(d[16]), "+f"(d[17]), "+f"(d[18]), "+f"(d[19]), "+f"(d[20]), "+f"(d[21]), "+f"(d[22]), "+f"(d[23]), "+f"(d[24]), "+f"(d[25]), "+f"(d[26]), "+f"(d[27]), "+f"(d[28]), "+f"(d[29]), "+f"(d[30]), "+f"(d[31])
-      : "l"(da), "l"(db), "r"(accumulate));
+      : "l"(da), "l"(db), "n"(AOFF), "n"(BOFF), "n"(ACC));
 }
+#undef TC_WGMMA_ASM
 template <int R>
 __device__ __forceinline__ void tc_fence_regs(float (&d)[R]) {
 #pragma unroll
   for (int i = 0; i < R; ++i) asm volatile("" : "+f"(d[i])::"memory");
 }
-template <int N>
-__device__ __forceinline__ void tc_wgmma(float (&d)[N / 2], uint64_t da, uint64_t db, uint32_t accumulate) {
-  if constexpr (N == 32) tc_wgmma32(d, da, db, accumulate);
-  else if constexpr (N == 48) tc_wgmma48(d, da, db, accumulate);
-  else tc_wgmma64(d, da, db, accumulate);
+template <int N, int AOFF, int BOFF, int ACC>
+__device__ __forceinline__ void tc_wgmma(float (&d)[N / 2], uint64_t da, uint64_t db) {
+  if constexpr (N == 32) tc_wgmma32<AOFF, BOFF, ACC>(d, da, db);
+  else if constexpr (N == 48) tc_wgmma48<AOFF, BOFF, ACC>(d, da, db);
+  else tc_wgmma64<AOFF, BOFF, ACC>(d, da, db);
 }
 __device__ __forceinline__ void tc_wg_fence() { asm volatile("wgmma.fence.sync.aligned;" ::: "memory"); }
 __device__ __forceinline__ void tc_wg_commit() { asm volatile("wgmma.commit_group.sync.aligned;" ::: "memory"); }
@@ -216,7 +229,7 @@ struct TcRoleInfo {
   int nstage;              // shared-memory stages
   int wbytes;              // weight image bytes
 };
-__device__ __forceinline__ TcRoleInfo tc_role(int cta) {
+__host__ __device__ __forceinline__ TcRoleInfo tc_role(int cta) {
   TcRoleInfo r;
   if (cta < 32) { r.role = TC_ROLE_G1; r.ci = cta; r.njobs = 1; r.nstage = kTcStages; r.wbytes = 98304; }
   else if (cta < 96) { r.role = TC_ROLE_G2; r.ci = cta - 32; r.njobs = 2; r.nstage = kTcStages; r.wbytes = 131072; }
@@ -244,9 +257,62 @@ __device__ __forceinline__ bool tc_consumers_any(bool flag) {
   return any != 0;
 }
 
+// The stage ring as one consumer warp sees it: the slot of its next stage, that slot's fill parity, the slot it consumed last.
+struct TcRing {
+  unsigned long long* full;
+  unsigned long long* empty;
+  unsigned nstage, slot, parity, prev;
+  int lane;
+  // each consumer warp releases a stage (one of kTcConsumerWarps arrivals) once its products are done
+  __device__ __forceinline__ void release(unsigned sl) const {
+    __syncwarp();
+    if (lane == 0) tc_mbar_arrive(&empty[sl]);
+  }
+};
+// Stage KS (K = 32, k-steps 2 KS and 2 KS + 1) of tc_gemm.  Everything that depends on KS -- the accumulate flags, the fold at the
+// end of a K = 128 chunk, which waits and releases follow -- is fixed at compile time: the code between a wgmma and its wait
+// has no branch, so the MMAs stay asynchronous (the previous stage's products overlap this stage's wait and issue).
+template <int N, int KS>
+__device__ __forceinline__ void tc_gemm_stage(float (&out)[N / 2], float (&acc)[N / 2], float (&crs)[N / 2], uint64_t dA0, uint64_t dB, TcRing& r,
+                                              PollGuard& pg) {
+  constexpr int K0 = 2 * KS, BT = N * 2;                // B tile of one k-step: N * 32 bytes = N * 2 descriptor units
+  const unsigned sl = r.slot;
+  tc_mbar_wait(&r.full[sl], r.parity, pg);              // after an abort: no wait, the MMAs below still run (on stale data)
+  const uint64_t dA = dA0 + (uint64_t)(sl * (unsigned)(kTcStageBytes >> 4));
+  tc_fence_regs(acc);
+  tc_fence_regs(crs);
+  tc_wg_fence();
+  // A: hi plane at + 0, lo plane at + 8192 bytes, k half h at + 4096 h;  B: hi k-step K at K * N * 32, lo at (32 + K) * N * 32
+  tc_wgmma<N, 0, K0 * BT, (K0 & 7) ? 1 : 0>(acc, dA, dB);
+  tc_wgmma<N, 0, (32 + K0) * BT, K0 ? 1 : 0>(crs, dA, dB);
+  tc_wgmma<N, 512, K0 * BT, 1>(crs, dA, dB);
+  tc_wgmma<N, 256, (K0 + 1) * BT, 1>(acc, dA, dB);
+  tc_wgmma<N, 256, (33 + K0) * BT, 1>(crs, dA, dB);
+  tc_wgmma<N, 768, (K0 + 1) * BT, 1>(crs, dA, dB);
+  tc_wg_commit();
+  if constexpr ((KS & 3) == 3) {                        // end of a K = 128 chunk: fold its hi.hi sum into out
+    tc_wg_wait<0>();
+    tc_fence_regs(acc);
+    tc_fence_regs(crs);
+#pragma unroll
+    for (int i = 0; i < N / 2; ++i) out[i] = KS == 3 ? acc[i] : __fadd_rn(out[i], acc[i]);
+    r.release(r.prev);
+    r.release(sl);
+  } else if constexpr ((KS & 3) != 0) {                 // the previous stage's products are done
+    tc_wg_wait<1>();
+    r.release(r.prev);
+  }
+  r.prev = sl;
+  if (++r.slot == r.nstage) { r.slot = 0; r.parity ^= 1u; }
+}
+template <int N, int... KS>
+__device__ __forceinline__ void tc_gemm_stages(float (&out)[N / 2], float (&acc)[N / 2], float (&crs)[N / 2], uint64_t dA0, uint64_t dB, TcRing& r,
+                                               PollGuard& pg, std::integer_sequence<int, KS...>) {
+  (tc_gemm_stage<N, KS>(out, acc, crs, dA0, dB, r, pg), ...);
+}
 // One GEMM of this warpgroup's 64 rows: out[N/2] = A (the vector image streamed through the stage ring) . W (image at w_saddr),
 // K = 512, as ((c0 + c1) + c2) + c3 + cross / 2048 with c_k the hi.hi products of k-steps 8k ... 8k+7.  `s` counts the stages
-// consumed by this CTA.  Each consumer warp releases a stage (one of kTcConsumerWarps arrivals) once its products are done.
+// consumed by this CTA.
 template <int N>
 __device__ __forceinline__ void tc_gemm(float (&out)[N / 2], uint32_t st0, uint32_t w_saddr, unsigned nstage, unsigned& s, unsigned long long* bar_full,
                                         unsigned long long* bar_empty, int wg, int lane, PollGuard& pg) {
@@ -255,45 +321,14 @@ __device__ __forceinline__ void tc_gemm(float (&out)[N / 2], uint32_t st0, uint3
   for (int i = 0; i < N / 2; ++i) { acc[i] = 0.f; crs[i] = 0.f; }
   const uint64_t dB = tc_desc(w_saddr, (uint32_t)(N / 8) * 128u, 128u);
   const uint64_t dA0 = tc_desc(st0 + (uint32_t)wg * 1024u, 2048u, 128u);      // this warpgroup's 8 row groups
-  const uint32_t btile = (uint32_t)N * 32u;                                     // bytes of one k-step tile of B
-  auto release = [&](unsigned stage) {
-    __syncwarp();
-    if (lane == 0) tc_mbar_arrive(&bar_empty[stage % nstage]);
-  };
-  for (int ks = 0; ks < kTcStagesPerVec; ++ks, ++s) {
-    const unsigned sl = s % nstage, su = s / nstage;
-    tc_mbar_wait(&bar_full[sl], su & 1u, pg);         // after an abort: no wait, the MMAs below still run (on stale data)
-    const uint64_t dA = dA0 + (uint64_t)((sl * kTcStageBytes) >> 4);
-    tc_fence_regs(acc);
-    tc_fence_regs(crs);
-    tc_wg_fence();
-#pragma unroll
-    for (int h = 0; h < 2; ++h) {
-      const int K = ks * 2 + h;
-      const uint64_t a_hi = dA + (uint64_t)((h * 4096) >> 4);
-      const uint64_t a_lo = dA + (uint64_t)((8192 + h * 4096) >> 4);
-      const uint64_t b_hi = dB + (uint64_t)(((uint32_t)K * btile) >> 4);
-      const uint64_t b_lo = dB + (uint64_t)(((uint32_t)(32 + K) * btile) >> 4);
-      tc_wgmma<N>(acc, a_hi, b_hi, (K & 7) ? 1u : 0u);
-      tc_wgmma<N>(crs, a_hi, b_lo, K ? 1u : 0u);
-      tc_wgmma<N>(crs, a_lo, b_hi, 1u);
-    }
-    tc_wg_commit();
-    if ((ks & 3) == 3) {                              // end of a K = 128 chunk: fold its hi.hi sum into out
-      tc_wg_wait<0>();
-      tc_fence_regs(acc);
-      tc_fence_regs(crs);
-#pragma unroll
-      for (int i = 0; i < N / 2; ++i) out[i] = ks == 3 ? acc[i] : __fadd_rn(out[i], acc[i]);
-      release(s - 1);
-      release(s);
-    } else if ((ks & 3) != 0) {                       // the previous stage's products are done
-      tc_wg_wait<1>();
-      release(s - 1);
-    }
-  }
+  TcRing r{bar_full, bar_empty, nstage, s % nstage, (s / nstage) & 1u, 0u, lane};
+  tc_gemm_stages<N>(out, acc, crs, dA0, dB, r, pg, std::make_integer_sequence<int, kTcStagesPerVec>{});
+  s += kTcStagesPerVec;
 #pragma unroll
   for (int i = 0; i < N / 2; ++i) out[i] = __fadd_rn(out[i], crs[i] * (1.0f / 2048.0f));
+  // every column counts as used: when a caller ignores some (GRU-2's zero columns), ptxas otherwise frees their accumulator
+  // registers inside the MMA chain and serializes every wgmma of the kernel (C7511)
+  tc_fence_regs(out);
 }
 
 __global__ void __launch_bounds__(kTcThreads, 1) wavernn_tc_kernel(TcArgs A) {
@@ -329,29 +364,10 @@ __global__ void __launch_bounds__(kTcThreads, 1) wavernn_tc_kernel(TcArgs A) {
   auto vec_img = [&](int v, int g, int par) { return A.vec + (((size_t)v * ng + g) * 2 + par) * (size_t)kTcVecBytes; };
   auto counter = [&](int g, int which) { return A.cnt + ((size_t)g * TCN_COUNT + which) * 32; };
 
-  if (warp == kTcLoaderWarp) {
-    // ================= loader: counter -> bulk copies into the stage ring =================
-    if (lane == 0) {
-      unsigned s = 0;
-      for (int t = 0; t < A.steps && !pg.aborted; ++t)
-        for (int g = 0; g < ng && !pg.aborted; ++g)
-          for (int j = 0; j < R.njobs; ++j) {
-            int v, cw, nprod;
-            tc_job(R.role, j, v, cw, nprod);
-            if (!tc_cnt_wait(counter(g, cw), (unsigned)nprod * (unsigned)(t + 1), pg)) break;
-            asm volatile("fence.proxy.async;" ::: "memory");      // generic-proxy stores of the producers -> this thread's async-proxy reads
-            const uint8_t* src = vec_img(v, g, t & 1);
-            for (int ks = 0; ks < kTcStagesPerVec; ++ks, ++s) {
-              const unsigned slot = s % (unsigned)R.nstage, use = s / (unsigned)R.nstage;
-              if (!tc_mbar_wait(&bar_empty[slot], (use & 1u) ^ 1u, pg)) break;
-              mbar_expect_tx(&bar_full[slot], kTcStageBytes);
-              tma_bulk_g2s(stages + (size_t)slot * kTcStageBytes, src + (size_t)ks * kTcStageBytes, kTcStageBytes, &bar_full[slot]);
-            }
-            if (pg.aborted) break;
-          }
-    }
-    __syncwarp();
-  } else if (warp < kTcConsumerWarps) {
+  // registers: the consumer warpgroups hold the accumulators of asynchronous MMAs, warpgroup 2 (loader + conditioning) little.
+  // setmaxnreg is executed by all warps of a warpgroup, and ptxas budgets each branch by the value it starts with.
+  if (warp < kTcConsumerWarps) {
+    asm volatile("setmaxnreg.inc.sync.aligned.u32 %0;" ::"n"(kTcConsumerRegs));
     // ================= consumers: MMA + gate math; rows ra, rb = ra + 8 of the group, column pairs 8i + 2c ================
     const int wg = warp >> 2, c = lane & 3;
     const int ra = 64 * wg + 16 * (warp & 3) + (lane >> 2);
@@ -366,6 +382,22 @@ __global__ void __launch_bounds__(kTcThreads, 1) wavernn_tc_kernel(TcArgs A) {
       // (the generic -> async proxy fence of this exchange is executed by the CONSUMER's loader thread, after its acquire)
       if (__any_sync(0xffffffffu, pg.aborted)) { pg.aborted = true; return; }
       if (lane == 0) tc_red_release(counter(g, which), 1u);
+    };
+    // phase counters (A.prof): stamp(-1) opens a job, stamp(p) adds the cycles since the last stamp to phase p.  Every consumer
+    // thread reads the clock, so no branch depends on the thread; all stamps sit between GEMMs, none inside a wgmma span.
+    long long pf[3] = {0, 0, 0}, pt = 0;
+    auto stamp = [&](int p) {
+      if (A.prof) {
+        const long long now = clock64();
+        if (p >= 0) pf[p] += now - pt;
+        pt = now;
+      }
+    };
+    auto stamp_first_full = [&]() {                   // end of the exchange wait: the job's first stage is full
+      if (A.prof) {
+        tc_mbar_wait(&bar_full[s % ns], (s / ns) & 1u, pg);
+        stamp(0);
+      }
     };
 
     if (R.role == TC_ROLE_G1) {
@@ -493,16 +525,22 @@ __global__ void __launch_bounds__(kTcThreads, 1) wavernn_tc_kernel(TcArgs A) {
               cd[h][gate][0] = v.x; cd[h][gate][1] = v.y;
             }
           }
-          float gi[16];
-          tc_gemm<32>(gi, st0, w0, ns, s, bar_full, bar_empty, wg, lane, pg);      // W_ih2 . x1(t)
-          // own units of x1 (fp32).  Its counter was complete before this CTA's GEMM could even start (the loader waited for
-          // it), so the check passes at its first poll; it gives this warp's loads their acquire
+          stamp(-1);
+          // own units of x1 (fp32), loaded while the GEMM runs.  The counter is the one this CTA's loader waits for before the
+          // GEMM's first stage; the warp's own acquire of it orders the loads.
           tc_cnt_wait_warp(counter(g, TCN_C1), (unsigned)(32 * kTcConsumerWarps) * (unsigned)(t + 1), pg, lane);
+          float2 x1v[2];
+#pragma unroll
+          for (int h = 0; h < 2; ++h)
+            x1v[h] = __ldcg(reinterpret_cast<const float2*>(A.x1f + (((size_t)g * 2 + (t & 1)) * kTcRows + rows[h]) * 512 + 8 * R.ci + 2 * c));
+          float gi[16];
+          stamp_first_full();
+          tc_gemm<32>(gi, st0, w0, ns, s, bar_full, bar_empty, wg, lane, pg);      // W_ih2 . x1(t)
+          stamp(1);
 #pragma unroll
           for (int h = 0; h < 2; ++h) {
             const int row = rows[h];
-            const float2 xa = __ldcg(reinterpret_cast<const float2*>(A.x1f + (((size_t)g * 2 + (t & 1)) * kTcRows + row) * 512 + 8 * R.ci + 2 * c));
-            const float x1[2] = {xa.x, xa.y};
+            const float x1[2] = {x1v[h].x, x1v[h].y};
             float hnew[2], x2[2];
 #pragma unroll
             for (int e = 0; e < 2; ++e) {
@@ -517,6 +555,7 @@ __global__ void __launch_bounds__(kTcThreads, 1) wavernn_tc_kernel(TcArgs A) {
             tc_store2(vec_img(TV_X2, g, t & 1), 8 * R.ci + 2 * c, row, x2[0], x2[1]);
           }
           publish(g, TCN_C2);
+          stamp(2);
           // W_hh2 . h2(t) for step t+1
           tc_gemm<32>(ghs[g], st0, w0 + 65536u, ns, s, bar_full, bar_empty, wg, lane, pg);
         }
@@ -529,20 +568,29 @@ __global__ void __launch_bounds__(kTcThreads, 1) wavernn_tc_kernel(TcArgs A) {
       for (int t = 0; t < A.steps; ++t) {
         const int fr = t / A.hop;
         for (int g = 0; g < ng; ++g) {
-          float a[32];
-          tc_gemm<64>(a, st0, w0, ns, s, bar_full, bar_empty, wg, lane, pg);
+          stamp(-1);
+          // aux projection + bias of this thread's units, loaded while the GEMM runs (the first step of a frame misses L2)
+          float2 cd[2][8];
 #pragma unroll
           for (int h = 0; h < 2; ++h) {
-            const int row = rows[h], src = min(g * kTcRows + row, A.B - 1);
+            const int src = min(g * kTcRows + rows[h], A.B - 1);
             const float* tb = A.tab + (((size_t)src * (A.T + 1) + fr) * 128 + 16 * R.ci + (c >> 1)) * kPushCondRows + trow + 2 * (c & 1);
 #pragma unroll
-            for (int i = 0; i < 8; ++i) {
-              const float2 cd = __ldg(reinterpret_cast<const float2*>(tb + (size_t)(2 * i) * kPushCondRows));
-              tc_store2(vec_img(vout, g, t & 1), 64 * R.ci + 8 * i + 2 * c, row, fmaxf(a[4 * i + 2 * h] + cd.x, 0.f),
-                        fmaxf(a[4 * i + 2 * h + 1] + cd.y, 0.f));
-            }
+            for (int i = 0; i < 8; ++i) cd[h][i] = __ldg(reinterpret_cast<const float2*>(tb + (size_t)(2 * i) * kPushCondRows));
+          }
+          float a[32];
+          stamp_first_full();
+          tc_gemm<64>(a, st0, w0, ns, s, bar_full, bar_empty, wg, lane, pg);
+          stamp(1);
+#pragma unroll
+          for (int h = 0; h < 2; ++h) {
+#pragma unroll
+            for (int i = 0; i < 8; ++i)
+              tc_store2(vec_img(vout, g, t & 1), 64 * R.ci + 8 * i + 2 * c, rows[h], fmaxf(a[4 * i + 2 * h] + cd[h][i].x, 0.f),
+                        fmaxf(a[4 * i + 2 * h + 1] + cd[h][i].y, 0.f));
           }
           publish(g, cout);
+          stamp(2);
           if (tc_consumers_any(pg.aborted)) { pg.aborted = true; break; }
         }
         if (pg.aborted) break;
@@ -578,7 +626,10 @@ __global__ void __launch_bounds__(kTcThreads, 1) wavernn_tc_kernel(TcArgs A) {
             }
           }
           float l[32];
+          stamp(-1);
+          stamp_first_full();
           tc_gemm<64>(l, st0, w0, ns, s, bar_full, bar_empty, wg, lane, pg);
+          stamp(1);
 #pragma unroll
           for (int h = 0; h < 2; ++h) {
             const int row = rows[h], grow = g * kTcRows + row;
@@ -606,57 +657,85 @@ __global__ void __launch_bounds__(kTcThreads, 1) wavernn_tc_kernel(TcArgs A) {
             }
           }
           publish(g, TCN_W);
+          stamp(2);
           if (tc_consumers_any(pg.aborted)) { pg.aborted = true; break; }
         }
         if (pg.aborted) break;
       }
     }
-  } else if (warp >= kTcCondWarp0 && R.role == TC_ROLE_G1) {
-    // ================= conditioning warps (GRU-1 CTAs): the 64 conditioned values of every row, a BLOCK of <= 8 steps at a time ========
-    // Within a frame the <= 7 table rows an output combines do not change, only the FIR phase does: they are loaded once per block
-    // and combined for every step of it (8x fewer table loads than step by step).  The results go to a small ring in global
-    // memory (two block buffers per CTA, L2 resident) that the gate threads read back one step at a time.
-    // lane = value: lanes 0-15 / 16-31 take the 16 table entries (kind*4 + unit%4) of two adjacent 4-unit table blocks.
-    const int cwarp = warp - kTcCondWarp0;
-    const int half = lane >> 4, i16 = lane & 15;
-    const size_t fstride = (size_t)128 * kPushCondRows;
-    float* cring = A.condg + (size_t)R.ci * 2 * ng * kTcCondBlk * kTcCondSlot;
-    int b = 0;
-    for (int t0 = 0; t0 < A.steps && !pg.aborted; ++b) {
-      const int fr = t0 / A.hop, ph0 = t0 - fr * A.hop;
-      const int t1 = min(min(t0 + kTcCondBlk, (fr + 1) * A.hop), A.steps), n = t1 - t0;
-      if (!tc_mbar_wait(&bar_condempty[b & 1], ((unsigned)(b >> 1) & 1u) ^ 1u, pg)) break;
-      for (int g = 0; g < ng; ++g) {
-        float* dst = cring + (size_t)((b & 1) * ng + g) * kTcCondBlk * kTcCondSlot;
-#pragma unroll 2
-        for (int row = cwarp; row < kTcRows; row += kTcCondWarps) {   // 2 rows x 2 blocks x 7 table loads in flight per lane
-          const int src = min(g * kTcRows + row, A.B - 1);
-#pragma unroll
-          for (int p = 0; p < 2; ++p) {
-            const int c4l = 2 * p + half;                                        // 4-unit block inside this CTA's 16 units
-            const float* base = A.tab + (((size_t)src * (A.T + 1) + fr) * 128 + 4 * R.ci + c4l) * kPushCondRows;
-            const float v0 = __ldg(base + 16 + i16);
-            float pm[kMaxTaps];
-#pragma unroll
-            for (int j = 0; j < kMaxTaps; ++j) {
-              const int f = fr + j - A.NT / 2;
-              pm[j] = (j < A.NT && f >= 0 && f < A.T) ? __ldg(base + (ptrdiff_t)(f - fr) * (ptrdiff_t)fstride + i16) : 0.f;
+    if (A.prof && tid == 0 && R.role != TC_ROLE_G1)
+      for (int i = 0; i < 3; ++i) A.prof[(size_t)blockIdx.x * 12 + 3 * (R.role - 1) + i] = pf[i];
+  } else {
+    asm volatile("setmaxnreg.dec.sync.aligned.u32 %0;" ::"n"(kTcOtherRegs));
+    if (warp == kTcLoaderWarp) {
+      // ================= loader: counter -> bulk copies into the stage ring =================
+      if (lane == 0) {
+        unsigned s = 0;
+        for (int t = 0; t < A.steps && !pg.aborted; ++t)
+          for (int g = 0; g < ng && !pg.aborted; ++g)
+            for (int j = 0; j < R.njobs; ++j) {
+              int v, cw, nprod;
+              tc_job(R.role, j, v, cw, nprod);
+              if (!tc_cnt_wait(counter(g, cw), (unsigned)nprod * (unsigned)(t + 1), pg)) break;
+              asm volatile("fence.proxy.async;" ::: "memory");      // generic-proxy stores of the producers -> this thread's async-proxy reads
+              const uint8_t* src = vec_img(v, g, t & 1);
+              for (int ks = 0; ks < kTcStagesPerVec; ++ks, ++s) {
+                const unsigned slot = s % (unsigned)R.nstage, use = s / (unsigned)R.nstage;
+                if (!tc_mbar_wait(&bar_empty[slot], (use & 1u) ^ 1u, pg)) break;
+                mbar_expect_tx(&bar_full[slot], kTcStageBytes);
+                tma_bulk_g2s(stages + (size_t)slot * kTcStageBytes, src + (size_t)ks * kTcStageBytes, kTcStageBytes, &bar_full[slot]);
+              }
+              if (pg.aborted) break;
             }
-            float* o = dst + (size_t)row * 64 + (i16 >> 2) * 16 + c4l * 4 + (i16 & 3);
-            for (int sidx = 0; sidx < n; ++sidx) {
-              const float* fc = fir_s + (ph0 + sidx) * A.NT;
-              float v = v0;
+      }
+      __syncwarp();
+    } else if (R.role == TC_ROLE_G1) {
+      // ================= conditioning warps (GRU-1 CTAs): the 64 conditioned values of every row, a BLOCK of <= 8 steps at a time ========
+      // Within a frame the <= 7 table rows an output combines do not change, only the FIR phase does: they are loaded once per block
+      // and combined for every step of it (8x fewer table loads than step by step).  The results go to a small ring in global
+      // memory (two block buffers per CTA, L2 resident) that the gate threads read back one step at a time.
+      // lane = value: lanes 0-15 / 16-31 take the 16 table entries (kind*4 + unit%4) of two adjacent 4-unit table blocks.
+      const int cwarp = warp - kTcCondWarp0;
+      const int half = lane >> 4, i16 = lane & 15;
+      const size_t fstride = (size_t)128 * kPushCondRows;
+      float* cring = A.condg + (size_t)R.ci * 2 * ng * kTcCondBlk * kTcCondSlot;
+      int b = 0;
+      for (int t0 = 0; t0 < A.steps && !pg.aborted; ++b) {
+        const int fr = t0 / A.hop, ph0 = t0 - fr * A.hop;
+        const int t1 = min(min(t0 + kTcCondBlk, (fr + 1) * A.hop), A.steps), n = t1 - t0;
+        if (!tc_mbar_wait(&bar_condempty[b & 1], ((unsigned)(b >> 1) & 1u) ^ 1u, pg)) break;
+        for (int g = 0; g < ng; ++g) {
+          float* dst = cring + (size_t)((b & 1) * ng + g) * kTcCondBlk * kTcCondSlot;
+#pragma unroll 2
+          for (int row = cwarp; row < kTcRows; row += kTcCondWarps) {   // 2 rows x 2 blocks x 7 table loads in flight per lane
+            const int src = min(g * kTcRows + row, A.B - 1);
 #pragma unroll
-              for (int j = 0; j < kMaxTaps; ++j)
-                if (j < A.NT) v = fmaf(fc[j], pm[j], v);      // an absent frame contributes fir * 0 = 0 exactly (same order as push_cond16)
-              o[(size_t)sidx * kTcCondSlot] = v;
+            for (int p = 0; p < 2; ++p) {
+              const int c4l = 2 * p + half;                                        // 4-unit block inside this CTA's 16 units
+              const float* base = A.tab + (((size_t)src * (A.T + 1) + fr) * 128 + 4 * R.ci + c4l) * kPushCondRows;
+              const float v0 = __ldg(base + 16 + i16);
+              float pm[kMaxTaps];
+#pragma unroll
+              for (int j = 0; j < kMaxTaps; ++j) {
+                const int f = fr + j - A.NT / 2;
+                pm[j] = (j < A.NT && f >= 0 && f < A.T) ? __ldg(base + (ptrdiff_t)(f - fr) * (ptrdiff_t)fstride + i16) : 0.f;
+              }
+              float* o = dst + (size_t)row * 64 + (i16 >> 2) * 16 + c4l * 4 + (i16 & 3);
+              for (int sidx = 0; sidx < n; ++sidx) {
+                const float* fc = fir_s + (ph0 + sidx) * A.NT;
+                float v = v0;
+#pragma unroll
+                for (int j = 0; j < kMaxTaps; ++j)
+                  if (j < A.NT) v = fmaf(fc[j], pm[j], v);      // an absent frame contributes fir * 0 = 0 exactly (same order as push_cond16)
+                o[(size_t)sidx * kTcCondSlot] = v;
+              }
             }
           }
         }
+        __syncwarp();
+        if (lane == 0) tc_mbar_arrive(&bar_condfull[b & 1]);
+        t0 = t1;
       }
-      __syncwarp();
-      if (lane == 0) tc_mbar_arrive(&bar_condfull[b & 1]);
-      t0 = t1;
     }
   }
   __syncthreads();

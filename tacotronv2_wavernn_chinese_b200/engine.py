@@ -217,7 +217,8 @@ class WaveRNNEngine:
         return q
 
     def debug_phase_cycles(self):
-        """[6][2] mean cycles (compute, barrier) per phase of the last grid launch; needs B200TTS_GRID_PROF=1."""
+        """[6][2] mean cycles (compute, barrier) per phase of the last grid launch; needs B200TTS_GRID_PROF=1.  After a
+        tensor-core launch the 12 values are (exchange wait, GEMM, epilogue) of GRU-2's x1 job, fc1, fc2 and fc3."""
         out = (C.c_double * 12)()
         _lib.check(self.lib.b200tts_wavernn_debug_phase_cycles(self._h, out))
         return np.array(list(out)).reshape(6, 2)

@@ -22,4 +22,9 @@ for k in kernels:
                 print('   cycles/step:', ' '.join(f'{n}={v:.0f}' for n, v in zip(names, pc.reshape(-1))), f' total {pc.sum():.0f}')
             else:
                 print('   cycles/step per phase (compute, barrier):', ' | '.join(f'P{i}: {a:.0f},{b:.0f}' for i, (a, b) in enumerate(pc)), f' total {pc.sum():.0f}')
+        if os.environ.get('B200TTS_GRID_PROF') and k == 'tc':
+            # per job (mean over the CTAs of its role): exchange wait, GEMM, epilogue; summed over the groups of a step
+            pc = (eng.debug_phase_cycles() / steps).reshape(4, 3)
+            print('   cycles/step (wait, gemm, epilogue):', ' | '.join(f'{n}: {a:.0f},{b:.0f},{c:.0f}' for n, (a, b, c) in
+                                                                zip(['GRU-2 x1', 'fc1', 'fc2', 'fc3'], pc)))
         print(f'kernel={k} B={B} steps={steps}: {ms:.1f} ms -> {ms*1e3/steps:.1f} us/step, {B*steps/ms*1e3/1e6:.3f} M samples/s', flush=True)
