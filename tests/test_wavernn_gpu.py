@@ -12,6 +12,8 @@ from tacotronv2_wavernn_chinese_b200 import synth
 pytestmark = pytest.mark.gpu
 
 KERNELS = ['utterance', 'grid']
+# plain batches also run on the tensor-core pipeline (kernel='tc' refuses folding and packed rows)
+PLAIN_KERNELS = KERNELS + ['tc']
 
 
 @pytest.fixture(scope='module')
@@ -92,7 +94,7 @@ def _explain_divergence(p, mels, q, ref_labels, t, b):
     return (top[1] - top[0]) < 1e-3 * max(1.0, abs(top[1]))
 
 
-@pytest.mark.parametrize('kernel', KERNELS)
+@pytest.mark.parametrize('kernel', PLAIN_KERNELS)
 @pytest.mark.parametrize('name', ['wavernn_synth_T24', 'wavernn_ckpt_T24'])
 def test_generate_vs_reference_golden(torch_cuda, name, kernel):
     g = _golden(name)
@@ -125,7 +127,7 @@ def test_generate_vs_reference_golden(torch_cuda, name, kernel):
         np.testing.assert_allclose(out['wave'].cpu().numpy()[0], g['wave0'], rtol=0, atol=1e-12)
 
 
-@pytest.mark.parametrize('kernel', KERNELS)
+@pytest.mark.parametrize('kernel', PLAIN_KERNELS)
 def test_generate_config1_shape_vs_reference(torch_cuda, kernel):
     """BASELINE config 1 shape (80 frames, 22 000 steps) on the shipped checkpoint vs the reference's own labels."""
     g = _golden('wavernn_ckpt_T80')
@@ -148,7 +150,7 @@ def test_generate_config1_shape_vs_reference(torch_cuda, kernel):
         assert np.abs(lg[s] - g['gen_logits'][i]).max() <= 5e-6 * scale + 1e-4
 
 
-@pytest.mark.parametrize('kernel', KERNELS)
+@pytest.mark.parametrize('kernel', PLAIN_KERNELS)
 def test_philox_stream_matches_oracle(torch_cuda, kernel):
     """Production RNG: dump the Philox Exp(1) stream the kernel draws and replay it through the oracle."""
     eng, p = engine_for('synth5')
@@ -167,10 +169,11 @@ def test_philox_stream_matches_oracle(torch_cuda, kernel):
         np.testing.assert_allclose(out['wave'].cpu().numpy(), ref['wave'], rtol=0, atol=1e-12)
 
 
-@pytest.mark.parametrize('kernel', KERNELS)
+@pytest.mark.parametrize('kernel', PLAIN_KERNELS)
 def test_batch_composition_invariance(torch_cuda, kernel):
     """Philox is keyed by the GLOBAL utterance index, so a row's output cannot depend on what it is batched with
-    (this is what makes multi-GPU sharding reproduce the single-GPU result).  Covers the G=1,2,4,8 row-group variants."""
+    (this is what makes multi-GPU sharding reproduce the single-GPU result).  Covers the G=1,2,4,8 row-group variants, and for the
+    tensor-core kernel a row that sits at another position than alone."""
     eng, _ = engine_for('synth5')
     T, seed = 21, 99
     for B in (3, 9):
@@ -328,8 +331,9 @@ def _distinct_cond(p, B, T, seed, distinct=16):
     return tile(mels), (tile(up), tile(aux))
 
 
-# the tensor-core pipeline (wavernn_tc.cuh, kernel='tc'): two full groups, a partial second group, one group, a partial group
-TC_BATCHES = [256, 200, 128, 100, 40]
+# the tensor-core pipeline (wavernn_tc.cuh, kernel='tc'): two full groups, a partial second group (255, 200, and 129 with one live
+# row in group 1), one full group, partial single groups (127, 100, 40, 33) and a single row
+TC_BATCHES = [256, 255, 200, 129, 128, 127, 100, 40, 33, 1]
 
 
 @pytest.mark.parametrize('B', TC_BATCHES)
