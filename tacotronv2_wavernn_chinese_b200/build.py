@@ -10,13 +10,16 @@ import os
 import shutil
 import subprocess
 import sys
+import tempfile
+from concurrent.futures import ThreadPoolExecutor
 
 PKG = os.path.dirname(os.path.abspath(__file__))
 CSRC = os.path.join(PKG, 'csrc')
 LIB = os.path.join(CSRC, 'libb200tts.so')
-SOURCES = ['b200tts_api.cu', 'resample.cu']
+# One translation unit per model stage, so that no stage's device code can change the code ptxas generates for another's.
+SOURCES = ['api.cu', 'wavernn.cu', 'tacotron.cu', 'griffin_lim.cu', 'mel_analysis.cu', 'resample.cu']
 NVCC_FLAGS = ['-gencode', 'arch=compute_90a,code=sm_90a', '-lineinfo', '-O3', '-std=c++17',
-              '-shared', '-Xcompiler', '-fPIC', '--expt-relaxed-constexpr']
+              '-Xcompiler', '-fPIC', '--expt-relaxed-constexpr']
 
 
 def _nvcc() -> str:
@@ -35,17 +38,29 @@ def _stale() -> bool:
     return any(os.path.getmtime(d) > t for d in deps if os.path.isfile(d))
 
 
-def build_lib(force: bool = False, verbose: bool = False) -> str:
-    """Compiles the CUDA library if it is missing or older than its sources; returns its path."""
-    if not force and not _stale():
-        return LIB
-    cmd = [_nvcc()] + NVCC_FLAGS + (['-Xptxas', '-v'] if verbose else []) + \
-          ['-o', LIB + '.tmp'] + [os.path.join(CSRC, s) for s in SOURCES]
+def _run(cmd: list[str]) -> str:
     res = subprocess.run(cmd, capture_output=True, text=True)
     if res.returncode != 0:
         raise RuntimeError('nvcc failed:\n' + ' '.join(cmd) + '\n' + res.stdout + res.stderr)
+    return res.stderr
+
+
+def build_lib(force: bool = False, verbose: bool = False) -> str:
+    """Compiles the CUDA library if it is missing or older than its sources; returns its path.
+
+    The translation units compile concurrently into objects in a temporary directory, then link into one shared library."""
+    if not force and not _stale():
+        return LIB
+    nvcc = _nvcc()
+    flags = NVCC_FLAGS + (['-Xptxas', '-v'] if verbose else [])
+    with tempfile.TemporaryDirectory(prefix='b200tts_build_') as tmp:
+        objs = [os.path.join(tmp, os.path.splitext(s)[0] + '.o') for s in SOURCES]
+        cmds = [[nvcc] + flags + ['-c', '-o', o, os.path.join(CSRC, s)] for s, o in zip(SOURCES, objs)]
+        with ThreadPoolExecutor(max_workers=len(cmds)) as pool:
+            logs = list(pool.map(_run, cmds))
+        logs.append(_run([nvcc, '-shared', '-gencode', 'arch=compute_90a,code=sm_90a', '-o', LIB + '.tmp'] + objs))
     if verbose:
-        print(res.stderr)
+        print(''.join(logs))
     os.replace(LIB + '.tmp', LIB)
     return LIB
 

@@ -6,18 +6,14 @@
 //                        frames (overlap-add / window sum-square, zero outside the row's signal), window, rfft, unit phasor,
 //                        times S, irfft, window -> the frame's windowed time signal.  kInit: the phasor comes from u instead.
 //   gl_finish_kernel     one CTA per row: overlap-add, envelope, inverse pre-emphasis (chunked scan with carries), zero tail
-// The 2048-point real FFT is a 1024-point complex radix-2 Stockham FFT in shared memory (even samples in .x, odd in .y) plus the
-// real split step; the inverse mirrors it.  Twiddles are fp64-computed at create time and stored as fp32.  No atomics: every
-// value a row produces depends only on that row's inputs.
+// The 2048-point real FFT is fft2048.cuh's; the inverse mirrors it.  No atomics: every value a row produces depends only on
+// that row's inputs.
 #pragma once
 #include "common.cuh"
+#include "fft2048.cuh"
 
 namespace b200tts {
 
-constexpr int kGlN = 2048;           // n_fft (the only size the FFT below implements)
-constexpr int kGlHalf = kGlN / 2;    // complex FFT length
-constexpr int kGlBins = kGlHalf + 1; // rfft bins
-constexpr int kGlThreads = 256;
 constexpr int kGlMagFrames = 16;     // frames per CTA of the magnitude GEMV (the pinv basis is read once per 16 frames)
 constexpr int kGlMaxMels = 128;
 constexpr int kGlFinishThreads = 1024;
@@ -60,42 +56,7 @@ __device__ __forceinline__ float gl_phase_u(float x, float y) {     // np.angle 
   return u >= 1.f ? 0.f : u;
 }
 
-__device__ __forceinline__ float2 cmul(float2 a, float2 b) { return make_float2(a.x * b.x - a.y * b.y, a.x * b.y + a.y * b.x); }
 __device__ __forceinline__ float2 conjf2(float2 a) { return make_float2(a.x, -a.y); }
-
-// Radix-2 Stockham, 10 stages, src -> (ping-pong) -> src.  Forward uses tw, inverse its conjugate; unnormalised.
-template <bool kInverse>
-__device__ __forceinline__ void gl_fft1024(float2* a, float2* b, const float2* __restrict__ tw) {
-  float2* src = a;
-  float2* dst = b;
-#pragma unroll 1
-  for (int Ns = 1; Ns < kGlHalf; Ns <<= 1) {
-    const int shift = kGlHalf / 2 / Ns;
-#pragma unroll
-    for (int r = 0; r < kGlHalf / 2 / kGlThreads; ++r) {
-      const int j = threadIdx.x + r * kGlThreads;
-      const int k = j & (Ns - 1);
-      float2 w = __ldg(tw + k * shift);
-      if (kInverse) w.y = -w.y;
-      const float2 x0 = src[j], x1 = cmul(src[j + kGlHalf / 2], w);
-      const int o = ((j - k) << 1) + k;
-      dst[o] = make_float2(x0.x + x1.x, x0.y + x1.y);
-      dst[o + Ns] = make_float2(x0.x - x1.x, x0.y - x1.y);
-    }
-    __syncthreads();
-    float2* t = src; src = dst; dst = t;
-  }
-}
-
-// Real split step of the forward 2048-point rfft: Z = FFT1024 of the even/odd-packed signal, za = Z[k], zb = Z[(1024-k) mod
-// 1024], w = e^{-2 pi i k / 2048}  ->  rfft bins *X0 = X[k] and *X1 = X[1024-k], 0 <= k <= 512.
-__device__ __forceinline__ void gl_forward_split(float2 za, float2 zb, float2 w, float2* X0, float2* X1) {
-  const float2 fe = make_float2(0.5f * (za.x + zb.x), 0.5f * (za.y - zb.y));   // (Z[k] + conj Z[N-k]) / 2
-  const float2 fo = make_float2(0.5f * (za.y + zb.y), -0.5f * (za.x - zb.x));  // (Z[k] - conj Z[N-k]) / 2i
-  const float2 wf = cmul(w, fo);
-  *X0 = make_float2(fe.x + wf.x, fe.y + wf.y);          // X[k]
-  *X1 = make_float2(fe.x - wf.x, -(fe.y - wf.y));       // X[N-k] = conj(fe - w fo)
-}
 
 // Spectrum pair (k, 1024-k) -> inverse-split inputs Z'[k], Z'[1024-k] (irfft of Y = (Y[0..1024]) as a 1024-point complex IFFT).
 // Y0/Y1 are Y[k], Y[1024-k]; for k = 0 they are Y[0], Y[1024] (imaginary parts already dropped, as irfft does).

@@ -9,18 +9,19 @@
 //   ma_audio_kernel       the rescaled trimmed wav zero-padded to T * hop samples (the training audio `out`)
 // Pre-emphasis is never materialised: p[n] = x[n] + (-k) x[n-1] (x[-1] = 0) is recomputed in fp64 where it is needed, with
 // the roundings scipy's lfilter makes, so the STFT input equals the reference's float64 signal until the gathered frame is
-// rounded to fp32.  The FFT is griffin_lim.cuh's.  No atomics: every value depends on its own row only.
+// rounded to fp32.  The FFT is fft2048.cuh's.  No atomics: every value depends on its own row only.
 #pragma once
 #include <climits>
 
 #include "common.cuh"
-#include "griffin_lim.cuh"
+#include "fft2048.cuh"
 
 namespace b200tts {
 
 constexpr int kMaThreads = 256;
 constexpr int kMaBoundsThreads = 1024;
 constexpr int kMaTrimWarps = kMaThreads / 32;      // trim frames per CTA of ma_trim_power_kernel
+constexpr int kMaMaxMels = 128;                     // the mel bands Griffin-Lim can invert (kGlMaxMels)
 
 enum : int { kMaTrim = 1, kMaPreemphasis = 2, kMaRescale = 4 };
 

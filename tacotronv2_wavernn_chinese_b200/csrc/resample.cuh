@@ -33,12 +33,6 @@ struct RsArgs {
   int* out_len;         // [B] ceil(len * ratio)
 };
 
-// Host side, defined in resample.cu.  rs_kernel and its launch are a translation unit of their own (compiled when
-// B200TTS_RS_KERNEL is defined), so that adding them changed no code ptxas generates for the kernels of b200tts_api.cu.
-cudaError_t rs_set_max_smem(int bytes);
-cudaError_t rs_launch(const RsArgs& a, unsigned grid_x, unsigned grid_y, size_t smem, cudaStream_t st);
-
-#ifdef B200TTS_RS_KERNEL
 // One wing: sum_{i < imax} (tab[off + i*step].x + eta * tab[...].y) * x[n -/+ ...], accumulated in resampy's order.
 template <int kDir>
 __device__ __forceinline__ float rs_wing(const RsArgs& A, const double* __restrict__ xs, int base, int i0, int imax,
@@ -97,6 +91,5 @@ __global__ void __launch_bounds__(kRsThreads) rs_kernel(RsArgs A) {
   }
   y[t] = acc;
 }
-#endif  // B200TTS_RS_KERNEL
 
 }  // namespace b200tts

@@ -153,7 +153,7 @@ __device__ __forceinline__ float block_max(float v, float* red) {
 // no forced-state reload, no window, no stop projection or rule, no stop / nsteps outputs (A.stop, A.nsteps unused).
 template <bool kTeacher>
 __global__ void __launch_bounds__(kTacoThreads, 1) taco_decoder_kernel(TacoWeights W, TacoArgs A, TacoGtaArgs G) {
-  extern __shared__ __align__(16) float sm[];
+  extern __shared__ __align__(1024) float sm[];   // 1024: the base these kernels were settled with (tacotron.cu)
   const int b = blockIdx.x, tid = threadIdx.x;
   const int Tx = min(A.lengths[b], A.Tx_max);
   if (Tx < 1) {                                        // empty sentence: nothing to attend to

@@ -76,7 +76,7 @@ __global__ void __launch_bounds__(kTacoThreads, 1) taco_bilstm_kernel(const floa
                                                                        const float* __restrict__ Kfw, const float* __restrict__ bfw,
                                                                        const float* __restrict__ Kbw, const float* __restrict__ bbw,
                                                                        float zoneout, float* __restrict__ memory /*[B][Tmax][2U]*/) {
-  extern __shared__ __align__(16) float sm[];
+  extern __shared__ __align__(1024) float sm[];   // 1024: the base these kernels were settled with (tacotron.cu)
   float* in = sm;               // [Cin + U]   x_t | h
   float* z = in + Cin + U;      // [4U]
   float* c = z + 4 * U;         // [U]

@@ -5,7 +5,7 @@
 // block c of 128 (cooperative launch, 512 threads) keeps in shared memory the columns that produce
 //     prenet units 2c, 2c+1 (both layers)   .   LSTM-1 and LSTM-2 units 2c, 2c+1 (all four gates)   .   attention dimension c
 //     context columns 4c ... 4c+3           .   mel column c (c < 80)
-// and the six vectors a step needs from everybody travel through L2 as FLAG-IN-DATA records (wavernn_push.cuh: the
+// and the six vectors a step needs from everybody travel through L2 as FLAG-IN-DATA records (exchange.cuh: the
 // value is the flag, a sentinel NaN marks "not yet", parity copies re-armed one step ahead):
 //     P1, P2  prenet layer outputs (dropout applied)           L1  LSTM-1 output o1 | zoned h1          L2  o2 | zoned h2
 //     EN      per-dimension partial energies e_c[t] = v_c tanh(keys[t][c] + q_c + loc_c[t] + b_c)        CTX context
@@ -20,7 +20,7 @@
 #pragma once
 #include "common.cuh"
 #include "taco_decoder.cuh"
-#include "wavernn_push.cuh"
+#include "exchange.cuh"
 
 namespace b200tts {
 
@@ -140,7 +140,7 @@ __device__ __forceinline__ void tg_gather(const float* src, int n4, PollGuard& p
 }
 
 __global__ void __launch_bounds__(kTgThreads, 1) taco_grid_kernel(TacoGridModel Md, TacoGridArgs A) {
-  extern __shared__ __align__(16) float sm[];
+  extern __shared__ __align__(1024) float sm[];   // 1024: the base these kernels were settled with (tacotron.cu)
   const int tid = threadIdx.x, c = blockIdx.x;
   const int M = Md.M, P = Md.P, U = Md.U, E = Md.E, KW = Md.KW;
   const int Tx = min(A.lengths[0], A.Tx), Txp = A.Txp;

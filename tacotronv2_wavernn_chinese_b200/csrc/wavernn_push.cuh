@@ -35,6 +35,7 @@
 //                    P5  f2 -> fc3 (8 x 512)  -> Gumbel-max over the CTA's 8 classes -> publish winner
 #pragma once
 #include "common.cuh"
+#include "exchange.cuh"
 #include "wavernn_upsample.cuh"
 #include "wavernn_grid.cuh"
 
@@ -43,7 +44,6 @@ namespace b200tts {
 constexpr int kPushThreads = 512;
 constexpr int kPushWarps = kPushThreads / 32;
 constexpr int kPushMaxRows = 32;    // rows of the widest variant, wavernn_push_kernel<32>; larger batches run other kernels
-constexpr uint32_t kPushSentinel = 0xFFFFFFFFu;
 constexpr int kPushCondRows = 52;   // per CTA and frame: 16 mel projections | 16 + 12 + 4 + 4 aux projections (+ bias)
 constexpr int kPushVecs = 6;        // h1, x1, h2, x2, f1, f2
 enum { PV_H1 = 0, PV_X1, PV_H2, PV_X2, PV_F1, PV_F2 };
@@ -101,50 +101,6 @@ __device__ __forceinline__ void push_row_next(const PushArgs& A, const PushRowSt
   utt = (A.pack_utt && u < A.pack_rows && k1 < A.pack_segs) ? A.pack_utt[u * A.pack_segs + k1] : -1;
   n = t1 - R.end[u];
 }
-
-// ---- L2-coherent accessors ---------------------------------------------------------------------------------------
-__device__ __forceinline__ float4 ld_relaxed_f4(const float* p) {
-  float4 v;
-  asm volatile("ld.relaxed.gpu.global.v4.f32 {%0,%1,%2,%3}, [%4];" : "=f"(v.x), "=f"(v.y), "=f"(v.z), "=f"(v.w) : "l"(p) : "memory");
-  return v;
-}
-__device__ __forceinline__ unsigned long long ld_relaxed_u64(const unsigned long long* p) {
-  unsigned long long v;
-  asm volatile("ld.relaxed.gpu.global.u64 %0, [%1];" : "=l"(v) : "l"(p) : "memory");
-  return v;
-}
-__device__ __forceinline__ void st_relaxed_f32(float* p, float v) {
-  asm volatile("st.relaxed.gpu.global.f32 [%0], %1;" ::"l"(p), "f"(v) : "memory");
-}
-__device__ __forceinline__ void st_relaxed_u32(float* p, uint32_t v) {
-  asm volatile("st.relaxed.gpu.global.u32 [%0], %1;" ::"l"(p), "r"(v) : "memory");
-}
-__device__ __forceinline__ void st_relaxed_u64(unsigned long long* p, unsigned long long v) {
-  asm volatile("st.relaxed.gpu.global.u64 [%0], %1;" ::"l"(p), "l"(v) : "memory");
-}
-__device__ __forceinline__ bool f4_ready(const float4& v) {
-  return __float_as_uint(v.x) != kPushSentinel && __float_as_uint(v.y) != kPushSentinel &&
-         __float_as_uint(v.z) != kPushSentinel && __float_as_uint(v.w) != kPushSentinel;
-}
-
-// A poll gives up after ~2 s (a peer CTA is gone) or as soon as any CTA has raised the global error flag.
-struct PollGuard {
-  int* error;
-  long long t0;
-  unsigned spins;
-  bool aborted;
-  __device__ __forceinline__ void begin() { spins = 0; }
-  __device__ __forceinline__ bool expired() {
-    if ((++spins & 1023u) != 0u) return false;
-    if (spins == 1024u) t0 = clock64();
-    if (*reinterpret_cast<volatile int*>(error) != 0 || clock64() - t0 > 4000000000LL) {
-      atomicExch(error, 1);
-      aborted = true;
-      return true;
-    }
-    return false;
-  }
-};
 
 // ---- exchange protocol ------------------------------------------------------------------------------------------
 // Compared in isolation on the previous GPU (tools/exchange_bench.cu; all-to-all exchange of a [128][G][4] vector by 128
@@ -628,7 +584,7 @@ __global__ void __launch_bounds__(kPushThreads, 1) wavernn_push_kernel(PushModel
 }
 
 // ---- conditioning tables: tab[u][f][c][52] for f in [0, T]; frame T carries the bias only (zero conditioning) ------------
-// cw: per CTA [16][feat] mel rows | [36][aux] aux rows | [36] bias   (floats; see pack in b200tts_api.cu)
+// cw: per CTA [16][feat] mel rows | [36][aux] aux rows | [36] bias   (floats; packed by b200tts_wavernn_create, wavernn.cu)
 struct PushCondW {
   const float* wm;      // [ncta][16][feat]
   const float* wa;      // [ncta][36][aux]

@@ -71,7 +71,7 @@ enum { TCN_C1 = 0, TCN_C2, TCN_F1, TCN_F2, TCN_W, TCN_COUNT = 8 };
 enum { TC_ROLE_G1 = 0, TC_ROLE_G2, TC_ROLE_F1, TC_ROLE_F2, TC_ROLE_F3 };
 
 struct TcArgs {
-  const uint8_t* wimg;           // [128][kTcWimgBytes] fp16 B-operand images (b200tts_api.cu: tc_pack)
+  const uint8_t* wimg;           // [128][kTcWimgBytes] fp16 B-operand images (packed by b200tts_wavernn_create, wavernn.cu)
   const float* prm;              // [128][128]
   uint8_t* vec;                  // [TV_COUNT][ng][2][kTcVecBytes]
   float* x1f;                    // [ng][2][128][512] fp32 copy of x1 (GRU-2 CTAs add their h2 to it: x2 = x1 + h2)
