@@ -159,7 +159,8 @@ struct Packer {
 inline int round4(int x) { return (x + 3) & ~3; }
 
 // push_init_kernel (wavernn_push.cuh, compiled in wavernn.cu): fills `nvec` words of a flag-in-data exchange buffer with the
-// sentinel, clears `nbest` winner words and the error flag.  The Tacotron grid decoder arms its exchange buffers with it too.
+// sentinel, clears `nbest` winner words and the error flag if `error` is not null.  The Tacotron grid decoder arms its exchange
+// buffers with it too.
 void launch_push_init(uint32_t* vec, size_t nvec, unsigned long long* best, size_t nbest, int* error, int grid, cudaStream_t st);
 
 }  // namespace b200tts

@@ -18,24 +18,23 @@ using namespace b200tts;
 struct b200tts_wavernn {
   int device = 0;
   b200tts_wavernn_cfg cfg{};
-  int aux = 0, NC = 0, NT = 0, sm_count = 0;
-  DeviceBuf weights;          // packed blob
+  int NC = 0, NT = 0, sm_count = 0;
+  DeviceBuf weights;          // original layouts, one blob (pack_original)
   StepWeights sw{};
   ResnetParams rp{};
   const float* d_fir = nullptr;   // [hop][NT]
   GridModel gm{};                 // per-CTA weight blobs of the grid kernel
-  DeviceBuf grid_blob, mels_T, aux_T, grid_sync, grid_prof, fold_mels, fold_aux;
+  DeviceBuf grid_blob, mels_T, aux_T, grid_sync, fold_mels, fold_aux;
   PushModel pm{};                 // small-batch push kernel (wavernn_push.cuh): per-CTA blobs + conditioning-projection weights
   PushCondW pcw{};
-  DeviceBuf push_blob, push_condw, push_tab, push_vec, push_best, push_prof;
-  DeviceBuf tc_wimg, tc_prm, tc_vec, tc_x1f, tc_win, tc_cnt, tc_cond, tc_prof;     // tensor-core pipeline (wavernn_tc.cuh)
+  DeviceBuf push_blob, push_condw, push_tab, push_vec, push_best;
+  DeviceBuf tc_wimg, tc_prm, tc_vec, tc_x1f, tc_win, tc_cnt, tc_cond;     // tensor-core pipeline (wavernn_tc.cuh)
   bool tc_ok = false;
-  bool last_tc_prof = false;      // the last tensor-core launch recorded phase counters
-  int last_kernel = 0;            // 1 utterance, 2 wide grid, 3 push, 5 tensor-core pipeline
-  int last_push_ncta = 0;
-  int* d_grid_error = nullptr;    // set by the grid kernel when a barrier wait timed out (a peer CTA vanished)
-  int last_grid_ncta = 0;
-  int coop = 0;
+  // the last launch of a step kernel
+  int last_kernel = 0;            // its StepKernel; 0 before the first
+  DeviceBuf prof;                 // its phase counters [prof_ncta][12] (B200TTS_GRID_PROF)
+  int prof_ncta = 0;              // 0: it recorded none
+  DeviceBuf error;                // one int, zeroed per generate call; set by any of its kernels that gave up waiting for a peer CTA
   // scratch
   DeviceBuf mels_up, aux_frames, labels, mel_in, wave, grid_scratch;
   HostPinned h_stage;
@@ -97,42 +96,14 @@ static std::vector<double> composite_fir(const b200tts_wavernn_cfg& c, const std
   return fir;
 }
 
-extern "C" int b200tts_wavernn_create(b200tts_wavernn** out, int device, const b200tts_wavernn_cfg* cfg,
-                                      const b200tts_tensor* weights, int n_weights) {
-  API_BEGIN
-  REQUIRE(out && cfg && weights && n_weights > 0, B200TTS_EINVAL, "null argument");
-  *out = nullptr;
-  const b200tts_wavernn_cfg& c = *cfg;
-  REQUIRE(c.n_upsample >= 1 && c.n_upsample <= 4, B200TTS_EINVAL, "n_upsample must be 1..4");
-  int prod = 1;
-  for (int j = 0; j < c.n_upsample; ++j) {
-    REQUIRE(c.upsample_factors[j] >= 1, B200TTS_EINVAL, "bad upsample factor");
-    prod *= c.upsample_factors[j];
-  }
-  REQUIRE(prod == c.hop_length, B200TTS_EINVAL, "prod(upsample_factors) != hop_length (wavernn_train.py:67 asserts the same)");
-  REQUIRE(c.res_out_dims % 4 == 0, B200TTS_EINVAL, "res_out_dims must be divisible by 4");
-  REQUIRE(c.rnn_dims % 128 == 0 && c.fc_dims % 128 == 0, B200TTS_EINVAL, "rnn_dims / fc_dims must be multiples of 128");
-  REQUIRE(c.bits >= 2 && c.bits <= 15, B200TTS_EINVAL, "bits must be 2..15 (labels are int16)");
-  REQUIRE(c.compute_dims <= 1024 && c.res_out_dims <= 1024, B200TTS_EINVAL, "compute/res_out dims too large");
-  const int R = c.rnn_dims, F = c.fc_dims, AUX = c.res_out_dims / 4, FEAT = c.feat_dims, NC = 1 << c.bits;
+// The original layouts: step weights (rows of I padded to ldI), MelResNet transposed to [in][out] with its BatchNorms folded, and
+// the composite FIR.  Uploads them as one blob and points ctx->sw, ctx->rp and ctx->d_fir into it; returns the step weights as
+// pointers into the host copy `pk`, from which the grid kernel's blobs are cut.
+static StepWeights pack_original(b200tts_wavernn* ctx, const TensorMap& tm, Packer& pk) {
+  const b200tts_wavernn_cfg& c = ctx->cfg;
+  const int R = c.rnn_dims, F = c.fc_dims, AUX = c.res_out_dims / 4, FEAT = c.feat_dims, NC = ctx->NC;
   const int C = c.compute_dims, O = c.res_out_dims, K = 2 * c.pad + 1;
-  REQUIRE(AUX % 4 == 0, B200TTS_EINVAL, "aux dims (res_out_dims/4) must be a multiple of 4");
-  check_device(device);
-  DeviceGuard dg(device);
-
-  TensorMap tm;
-  for (int i = 0; i < n_weights; ++i)
-    if (weights[i].name) tm[weights[i].name] = &weights[i];
-
-  std::unique_ptr<b200tts_wavernn> ctx(new b200tts_wavernn());
-  ctx->device = device;
-  ctx->cfg = c;
-  ctx->aux = AUX;
-  ctx->NC = NC;
-  B200_CUDA(cudaDeviceGetAttribute(&ctx->sm_count, cudaDevAttrMultiProcessorCount, device));
-
-  Packer pk;
-  // ---- step weights, original layouts ----
+  // ---- step weights ----
   const int nin = 1 + FEAT + AUX, ldI = round4(nin);
   const float* Iw = need(tm, "I.weight", {R, nin})->data;
   size_t oI = pk.add((size_t)R * ldI);
@@ -207,221 +178,90 @@ extern "C" int b200tts_wavernn_create(b200tts_wavernn** out, int device, const b
 
   ctx->weights.ensure(pk.h.size() * sizeof(float));
   B200_CUDA(cudaMemcpy(ctx->weights.p, pk.h.data(), pk.h.size() * sizeof(float), cudaMemcpyHostToDevice));
+  auto step_weights = [&](const float* base) {
+    StepWeights sw{};
+    sw.I_w = base + oI; sw.I_b = base + oIb;
+    sw.ih1_w = base + o_ih1; sw.hh1_w = base + o_hh1; sw.ih1_b = base + o_bih1; sw.hh1_b = base + o_bhh1;
+    sw.ih2_w = base + o_ih2; sw.hh2_w = base + o_hh2; sw.ih2_b = base + o_bih2; sw.hh2_b = base + o_bhh2;
+    sw.fc1_w = base + o_fc1; sw.fc1_b = base + o_fc1b; sw.fc2_w = base + o_fc2; sw.fc2_b = base + o_fc2b;
+    sw.fc3_w = base + o_fc3; sw.fc3_b = base + o_fc3b;
+    sw.R = R; sw.F = F; sw.aux = AUX; sw.feat = FEAT; sw.NC = NC; sw.ldI = ldI;
+    return sw;
+  };
   const float* base = ctx->weights.as<float>();
-  StepWeights& sw = ctx->sw;
-  sw.I_w = base + oI; sw.I_b = base + oIb;
-  sw.ih1_w = base + o_ih1; sw.hh1_w = base + o_hh1; sw.ih1_b = base + o_bih1; sw.hh1_b = base + o_bhh1;
-  sw.ih2_w = base + o_ih2; sw.hh2_w = base + o_hh2; sw.ih2_b = base + o_bih2; sw.hh2_b = base + o_bhh2;
-  sw.fc1_w = base + o_fc1; sw.fc1_b = base + o_fc1b; sw.fc2_w = base + o_fc2; sw.fc2_b = base + o_fc2b;
-  sw.fc3_w = base + o_fc3; sw.fc3_b = base + o_fc3b;
-  sw.R = R; sw.F = F; sw.aux = AUX; sw.feat = FEAT; sw.NC = NC; sw.ldI = ldI;
+  ctx->sw = step_weights(base);
   ResnetParams& rp = ctx->rp;
   rp.conv_in_t = base + o_cin; rp.bn_scale = base + o_bns; rp.bn_shift = base + o_bnh; rp.res_w_t = base + o_res;
   rp.conv_out_t = base + o_cout; rp.conv_out_b = base + o_coutb;
   rp.feat = FEAT; rp.k = K; rp.C = C; rp.O = O; rp.blocks = c.res_blocks; rp.pad = c.pad;
   ctx->d_fir = base + o_fir;
+  return step_weights(pk.h.data());
+}
 
-  // ---- weight-stationary per-CTA blobs for the grid kernel (wavernn_grid.cuh) ----
-  {
-    GridModel& g = ctx->gm;
-    g.R = R; g.F = F; g.AUX = AUX; g.FEAT = FEAT; g.NC = NC;
-    g.ldC = FEAT + AUX; g.ldX = R + AUX; g.ldF = F + AUX;
-    g.ncta = R / kUPC;
-    g.ok = (R == F) && (R % kUPC == 0) && (NC == g.ncta * kCPC) && (FEAT % 4 == 0) && (g.ncta <= ctx->sm_count);
-    // the narrow mapping stages [x1|aux], [f1|aux], [mel|aux] in a 640*G-float area and h in a 512*G-float area
-    if (R + AUX > 640 || F + AUX > 640 || FEAT + AUX > 640 || R > 512) g.ok = 0;
-    int off = 0;
-    auto take = [&](int n) { int o = off; off += (n + 3) & ~3; return o; };
-    g.oA_w = take(16 * g.ldC); g.oA_x = take(16); g.oA_b = take(16);
-    g.ohh1 = take(3 * kUPC * R); g.oih2 = take(3 * kUPC * g.ldX); g.ohh2 = take(3 * kUPC * R);
-    g.ofc1 = take(kUPC * g.ldX); g.ofc2 = take(kUPC * g.ldF); g.ofc3 = take(kCPC * F);
-    g.obhh1 = take(3 * kUPC); g.obih2 = take(3 * kUPC); g.obhh2 = take(3 * kUPC);
-    g.obfc1 = take(kUPC); g.obfc2 = take(kUPC); g.obfc3 = take(kCPC);
-    g.blob = off;
-    constexpr int kMaxScratch = std::max({MapTraits<0, 4, 1>::kScratchFloats, MapTraits<1, 1, 1>::kScratchFloats,
-                                          MapTraits<2, 1, 1>::kScratchFloats, MapTraits<4, 1, 1>::kScratchFloats,
-                                          MapTraits<4, 1, 2>::kScratchFloats});   // every variant launch_grid can dispatch
-    size_t smem_need = ((size_t)g.blob + (size_t)kMaxScratch) * sizeof(float) + 2048;
-    if (smem_need > 227 * 1024) g.ok = 0;
-    B200_CUDA(cudaDeviceGetAttribute(&ctx->coop, cudaDevAttrCooperativeLaunch, device));
-    if (!ctx->coop) g.ok = 0;
-    if (g.ok) {
-      std::vector<float> hb((size_t)g.ncta * g.blob, 0.f);
-      std::vector<double> fold_acc(1 + g.ldC);
-      const float* P = pk.h.data();
-      for (int cta = 0; cta < g.ncta; ++cta) {
-        float* b = &hb[(size_t)cta * g.blob];
-        for (int j = 0; j < kUPC; ++j) {
-          const int row = cta * kUPC + j;
-          const float* src = P + oI + (size_t)row * ldI;          // [x | feat | aux] padded
-          b[g.oA_x + j] = src[0];
-          std::memcpy(b + g.oA_w + (size_t)j * g.ldC, src + 1, sizeof(float) * g.ldC);
-          b[g.oA_b + j] = P[oIb + row];
-          std::memcpy(b + g.ofc1 + (size_t)j * g.ldX, P + o_fc1 + (size_t)row * g.ldX, sizeof(float) * g.ldX);
-          std::memcpy(b + g.ofc2 + (size_t)j * g.ldF, P + o_fc2 + (size_t)row * g.ldF, sizeof(float) * g.ldF);
-          b[g.obfc1 + j] = P[o_fc1b + row];
-          b[g.obfc2 + j] = P[o_fc2b + row];
-          for (int gate = 0; gate < 3; ++gate) {
-            const int srow = gate * R + row, drow = gate * kUPC + j;
-            // folded input projection of GRU 1: row srow of W_ih1.W_I (x column | cond columns) and W_ih1.b_I + b_ih1, in double
-            {
-              const float* wr = P + o_ih1 + (size_t)srow * R;
-              double bacc = (double)P[o_bih1 + srow];
-              std::vector<double>& accv = fold_acc;
-              std::fill(accv.begin(), accv.end(), 0.0);
-              for (int k = 0; k < R; ++k) {
-                const double wk = (double)wr[k];
-                const float* irow = P + oI + (size_t)k * ldI;
-                for (int col = 0; col < 1 + g.ldC; ++col) accv[col] += wk * (double)irow[col];
-                bacc += wk * (double)P[oIb + k];
-              }
-              b[g.oA_x + 4 + drow] = (float)accv[0];
-              for (int col = 0; col < g.ldC; ++col) b[g.oA_w + (size_t)(4 + drow) * g.ldC + col] = (float)accv[1 + col];
-              b[g.oA_b + 4 + drow] = (float)bacc;
-            }
-            std::memcpy(b + g.ohh1 + (size_t)drow * R, P + o_hh1 + (size_t)srow * R, sizeof(float) * R);
-            std::memcpy(b + g.oih2 + (size_t)drow * g.ldX, P + o_ih2 + (size_t)srow * g.ldX, sizeof(float) * g.ldX);
-            std::memcpy(b + g.ohh2 + (size_t)drow * R, P + o_hh2 + (size_t)srow * R, sizeof(float) * R);
-            b[g.obhh1 + drow] = P[o_bhh1 + srow];
-            b[g.obih2 + drow] = P[o_bih2 + srow]; b[g.obhh2 + drow] = P[o_bhh2 + srow];
-          }
-        }
-        for (int r = 0; r < kCPC; ++r) {
-          const int row = cta * kCPC + r;
-          std::memcpy(b + g.ofc3 + (size_t)r * F, P + o_fc3 + (size_t)row * F, sizeof(float) * F);
-          b[g.obfc3 + r] = P[o_fc3b + row];
-        }
-      }
-      ctx->grid_blob.ensure(hb.size() * sizeof(float));
-      B200_CUDA(cudaMemcpy(ctx->grid_blob.p, hb.data(), hb.size() * sizeof(float), cudaMemcpyHostToDevice));
+template <class V>
+static void upload(DeviceBuf& d, const V& h) {
+  if (h.empty()) return;
+  d.ensure(h.size() * sizeof(h[0]));
+  B200_CUDA(cudaMemcpy(d.p, h.data(), h.size() * sizeof(h[0]), cudaMemcpyHostToDevice));
+}
 
-      // ---- push kernel (wavernn_push.cuh): recurrent / feed-forward rows only; the conditioned columns become tables ----
-      PushModel& pm = ctx->pm;
-      pm.ncta = g.ncta; pm.R = R; pm.F = F; pm.NC = NC;
-      int poff = 0;
-      auto ptake = [&](int n) { int o = poff; poff += (n + 3) & ~3; return o; };
-      // W_ih2 (12 rows) | fc1 (4 rows) | W_hh2 (12 rows) are contiguous: x1 is multiplied by the first 16 rows in one pass, h2 by the
-      // last 16 (fc1, then W_hh2) from one set of registers
-      pm.ohh1 = ptake(12 * R); pm.oih2 = ptake(12 * R); pm.ofc1 = ptake(4 * R); pm.ohh2 = ptake(12 * R);
-      pm.ofc2 = ptake(4 * F); pm.ofc3 = ptake(8 * F);
-      pm.oAx = ptake(16); pm.obhh1 = ptake(12); pm.obhh2 = ptake(12); pm.obfc3 = ptake(8);
-      pm.blob = poff;
-      const size_t push_smem = ((size_t)pm.blob + (size_t)PushTraits<32>::scratch_floats(c.hop_length, NT)) * sizeof(float) + 1024;
-      pm.ok = (R == 512 && F == 512 && g.ncta == 128 && NC <= 1024 && push_smem <= 227 * 1024) ? 1 : 0;
-      if (pm.ok) {
-        std::vector<float> pb((size_t)g.ncta * pm.blob, 0.f);
-        std::vector<float> cw((size_t)g.ncta * (16 * FEAT + 36 * AUX + 36), 0.f);
-        float* wm = cw.data();
-        float* wa = wm + (size_t)g.ncta * 16 * FEAT;
-        float* cb = wa + (size_t)g.ncta * 36 * AUX;
-        for (int cta = 0; cta < g.ncta; ++cta) {
-          const float* b = &hb[(size_t)cta * g.blob];
-          float* d = &pb[(size_t)cta * pm.blob];
-          for (int r = 0; r < 12; ++r) {
-            std::memcpy(d + pm.ohh1 + (size_t)r * R, b + g.ohh1 + (size_t)r * R, sizeof(float) * R);
-            std::memcpy(d + pm.oih2 + (size_t)r * R, b + g.oih2 + (size_t)r * g.ldX, sizeof(float) * R);
-            std::memcpy(d + pm.ohh2 + (size_t)r * R, b + g.ohh2 + (size_t)r * R, sizeof(float) * R);
-            d[pm.obhh1 + r] = b[g.obhh1 + r];
-            d[pm.obhh2 + r] = b[g.obhh2 + r];
-            std::memcpy(wa + ((size_t)cta * 36 + 16 + r) * AUX, b + g.oih2 + (size_t)r * g.ldX + R, sizeof(float) * AUX);
-            cb[(size_t)cta * 36 + 16 + r] = b[g.obih2 + r];
-          }
-          for (int j = 0; j < 4; ++j) {
-            std::memcpy(d + pm.ofc1 + (size_t)j * R, b + g.ofc1 + (size_t)j * g.ldX, sizeof(float) * R);
-            std::memcpy(d + pm.ofc2 + (size_t)j * F, b + g.ofc2 + (size_t)j * g.ldF, sizeof(float) * F);
-            std::memcpy(wa + ((size_t)cta * 36 + 28 + j) * AUX, b + g.ofc1 + (size_t)j * g.ldX + R, sizeof(float) * AUX);
-            std::memcpy(wa + ((size_t)cta * 36 + 32 + j) * AUX, b + g.ofc2 + (size_t)j * g.ldF + F, sizeof(float) * AUX);
-            cb[(size_t)cta * 36 + 28 + j] = b[g.obfc1 + j];
-            cb[(size_t)cta * 36 + 32 + j] = b[g.obfc2 + j];
-          }
-          for (int r = 0; r < 8; ++r) {
-            std::memcpy(d + pm.ofc3 + (size_t)r * F, b + g.ofc3 + (size_t)r * F, sizeof(float) * F);
-            d[pm.obfc3 + r] = b[g.obfc3 + r];
-          }
-          for (int r = 0; r < 16; ++r) {          // I rows 0-3, folded GRU-1 rows 4-15: [mel | a1] columns, x coefficient, bias
-            d[pm.oAx + r] = b[g.oA_x + r];
-            std::memcpy(wm + ((size_t)cta * 16 + r) * FEAT, b + g.oA_w + (size_t)r * g.ldC, sizeof(float) * FEAT);
-            std::memcpy(wa + ((size_t)cta * 36 + r) * AUX, b + g.oA_w + (size_t)r * g.ldC + FEAT, sizeof(float) * AUX);
-            cb[(size_t)cta * 36 + r] = b[g.oA_b + r];
-          }
-        }
-        ctx->push_blob.ensure(pb.size() * sizeof(float));
-        B200_CUDA(cudaMemcpy(ctx->push_blob.p, pb.data(), pb.size() * sizeof(float), cudaMemcpyHostToDevice));
-        ctx->push_condw.ensure(cw.size() * sizeof(float));
-        B200_CUDA(cudaMemcpy(ctx->push_condw.p, cw.data(), cw.size() * sizeof(float), cudaMemcpyHostToDevice));
-        const float* cwd = ctx->push_condw.as<float>();
-        ctx->pcw.wm = cwd;
-        ctx->pcw.wa = cwd + (size_t)g.ncta * 16 * FEAT;
-        ctx->pcw.bias = ctx->pcw.wa + (size_t)g.ncta * 36 * AUX;
-        ctx->pcw.ncta = g.ncta; ctx->pcw.feat = FEAT; ctx->pcw.aux = AUX;
-
-        // ---- tensor-core pipeline (wavernn_tc.cuh): per-CTA B-operand images, every weight split into two fp16 planes
-        //      (hi, lo' = (w - hi) * 2048) in the wgmma K-major no-swizzle layout [plane][k-step 32][k half 2][N/8][8 cols][8 halves]
-        if (NC == 1024 && ctx->sm_count >= kTcCtas) {
-          std::vector<uint16_t> img((size_t)kTcCtas * kTcWimgBytes / 2, 0);
-          std::vector<float> prm((size_t)kTcCtas * kTcPrm, 0.f);
-          auto put = [&](uint16_t* base, int N, int col, const float* wrow) {     // one weight row (K = 512) -> column `col` of an image
-            for (int k = 0; k < 512; ++k) {
-              const float w = wrow[k];
-              const __half hi = __float2half_rn(w);
-              const __half lo = __float2half_rn((w - __half2float(hi)) * 2048.0f);
-              const size_t off = ((size_t)(k >> 4) * 2 + ((k >> 3) & 1)) * ((size_t)N * 8) + (size_t)(col >> 3) * 64 + (size_t)(col & 7) * 8 + (k & 7);
-              base[off] = __half_as_ushort(hi);
-              base[(size_t)32 * N * 16 + off] = __half_as_ushort(lo);
-            }
-          };
-          auto unit_blob = [&](int unit) { return &pb[(size_t)(unit >> 2) * pm.blob]; };
-          for (int cta = 0; cta < kTcCtas; ++cta) {
-            uint16_t* wi = &img[(size_t)cta * kTcWimgBytes / 2];
-            float* pr = &prm[(size_t)cta * kTcPrm];
-            if (cta < 32) {                                   // GRU-1: 16 units, columns gate*16 + i
-              for (int i = 0; i < 16; ++i) {
-                const int unit = 16 * cta + i, j = unit & 3;
-                const float* b = unit_blob(unit);
-                for (int gate = 0; gate < 3; ++gate) {
-                  put(wi, 48, gate * 16 + i, b + pm.ohh1 + (size_t)(gate * 4 + j) * R);
-                  pr[64 + gate * 16 + i] = b[pm.obhh1 + gate * 4 + j];
-                }
-                for (int kind = 0; kind < 4; ++kind) pr[kind * 16 + i] = b[pm.oAx + kind * 4 + j];
-              }
-            } else if (cta < 96) {                            // GRU-2: 8 units, W_ih2 image then W_hh2 image, columns gate*8 + i (24-31 zero)
-              const int ci = cta - 32;
-              for (int i = 0; i < 8; ++i) {
-                const int unit = 8 * ci + i, j = unit & 3;
-                const float* b = unit_blob(unit);
-                for (int gate = 0; gate < 3; ++gate) {
-                  put(wi, 32, gate * 8 + i, b + pm.oih2 + (size_t)(gate * 4 + j) * R);
-                  put(wi + 32768, 32, gate * 8 + i, b + pm.ohh2 + (size_t)(gate * 4 + j) * R);
-                  pr[gate * 8 + i] = b[pm.obhh2 + gate * 4 + j];
-                }
-              }
-            } else if (cta < 112) {                           // fc1 / fc2: 64 units
-              const bool first = cta < 104;
-              const int ci = first ? cta - 96 : cta - 104;
-              for (int i = 0; i < 64; ++i) {
-                const int unit = 64 * ci + i, j = unit & 3;
-                const float* b = unit_blob(unit);
-                put(wi, 64, i, b + (first ? pm.ofc1 : pm.ofc2) + (size_t)j * R);
-              }
-            } else {                                          // fc3: 64 classes
-              const int ci = cta - 112;
-              for (int i = 0; i < 64; ++i) {
-                const int cls = 64 * ci + i;
-                const float* b = &pb[(size_t)(cls >> 3) * pm.blob];
-                put(wi, 64, i, b + pm.ofc3 + (size_t)(cls & 7) * F);
-                pr[i] = b[pm.obfc3 + (cls & 7)];
-              }
-            }
-          }
-          ctx->tc_wimg.ensure(img.size() * sizeof(uint16_t));
-          B200_CUDA(cudaMemcpy(ctx->tc_wimg.p, img.data(), img.size() * sizeof(uint16_t), cudaMemcpyHostToDevice));
-          ctx->tc_prm.ensure(prm.size() * sizeof(float));
-          B200_CUDA(cudaMemcpy(ctx->tc_prm.p, prm.data(), prm.size() * sizeof(float), cudaMemcpyHostToDevice));
-          ctx->tc_ok = true;
-        }
-      }
-    }
+extern "C" int b200tts_wavernn_create(b200tts_wavernn** out, int device, const b200tts_wavernn_cfg* cfg,
+                                      const b200tts_tensor* weights, int n_weights) {
+  API_BEGIN
+  REQUIRE(out && cfg && weights && n_weights > 0, B200TTS_EINVAL, "null argument");
+  *out = nullptr;
+  const b200tts_wavernn_cfg& c = *cfg;
+  REQUIRE(c.n_upsample >= 1 && c.n_upsample <= 4, B200TTS_EINVAL, "n_upsample must be 1..4");
+  int prod = 1;
+  for (int j = 0; j < c.n_upsample; ++j) {
+    REQUIRE(c.upsample_factors[j] >= 1, B200TTS_EINVAL, "bad upsample factor");
+    prod *= c.upsample_factors[j];
   }
+  REQUIRE(prod == c.hop_length, B200TTS_EINVAL, "prod(upsample_factors) != hop_length (wavernn_train.py:67 asserts the same)");
+  REQUIRE(c.res_out_dims % 4 == 0, B200TTS_EINVAL, "res_out_dims must be divisible by 4");
+  REQUIRE(c.rnn_dims % 128 == 0 && c.fc_dims % 128 == 0, B200TTS_EINVAL, "rnn_dims / fc_dims must be multiples of 128");
+  REQUIRE(c.bits >= 2 && c.bits <= 15, B200TTS_EINVAL, "bits must be 2..15 (labels are int16)");
+  REQUIRE(c.compute_dims <= 1024 && c.res_out_dims <= 1024, B200TTS_EINVAL, "compute/res_out dims too large");
+  const int AUX = c.res_out_dims / 4, FEAT = c.feat_dims;
+  REQUIRE(AUX % 4 == 0, B200TTS_EINVAL, "aux dims (res_out_dims/4) must be a multiple of 4");
+  check_device(device);
+  DeviceGuard dg(device);
+
+  TensorMap tm;
+  for (int i = 0; i < n_weights; ++i)
+    if (weights[i].name) tm[weights[i].name] = &weights[i];
+
+  std::unique_ptr<b200tts_wavernn> ctx(new b200tts_wavernn());
+  ctx->device = device;
+  ctx->cfg = c;
+  ctx->NC = 1 << c.bits;
+  int coop = 0;
+  B200_CUDA(cudaDeviceGetAttribute(&ctx->sm_count, cudaDevAttrMultiProcessorCount, device));
+  B200_CUDA(cudaDeviceGetAttribute(&coop, cudaDevAttrCooperativeLaunch, device));
+
+  // Each kernel's weights are cut from the host blobs of the one before it (grid -> push -> tensor cores), so each capability
+  // implies the previous one.
+  Packer pk;
+  const StepWeights hw = pack_original(ctx.get(), tm, pk);
+  const std::vector<float> gb = pack_grid_model(hw, ctx->sm_count, coop != 0, ctx->gm);
+  upload(ctx->grid_blob, gb);
+  std::vector<float> cw;
+  const std::vector<float> pb = pack_push_model(ctx->gm, gb, c.hop_length, ctx->NT, ctx->pm, cw);
+  upload(ctx->push_blob, pb);
+  upload(ctx->push_condw, cw);
+  if (ctx->pm.ok) {
+    const int n = ctx->pm.ncta;
+    const float* cwd = ctx->push_condw.as<float>();
+    ctx->pcw = PushCondW{cwd, cwd + (size_t)n * 16 * FEAT, cwd + (size_t)n * (16 * FEAT + 36 * AUX), n, FEAT, AUX};
+  }
+  std::vector<uint16_t> img;
+  std::vector<float> prm;
+  ctx->tc_ok = pack_tc_images(ctx->pm, pb, ctx->sm_count, c.hop_length * ctx->NT, img, prm);
+  upload(ctx->tc_wimg, img);
+  upload(ctx->tc_prm, prm);
+
+  ctx->error.ensure(sizeof(int));
+  B200_CUDA(cudaMemset(ctx->error.p, 0, sizeof(int)));
   B200_CUDA(cudaEventCreate(&ctx->ev0));
   B200_CUDA(cudaEventCreate(&ctx->ev1));
   *out = ctx.release();
@@ -450,12 +290,10 @@ extern "C" double b200tts_wavernn_last_kernel_ms(b200tts_wavernn* ctx) {
     g_err = std::string("cudaEventElapsedTime: ") + cudaGetErrorString(e);
     return -1.0;
   }
-  if (ctx->d_grid_error) {
-    int flag = 0;
-    if (cudaMemcpy(&flag, ctx->d_grid_error, sizeof(int), cudaMemcpyDeviceToHost) == cudaSuccess && flag) {
-      g_err = "grid kernel: a grid-barrier wait timed out (co-resident CTA missing); results are invalid";
-      return -1.0;
-    }
+  int flag = 0;
+  if (cudaMemcpy(&flag, ctx->error.p, sizeof(int), cudaMemcpyDeviceToHost) == cudaSuccess && flag) {
+    g_err = "grid kernel: a grid-barrier wait timed out (co-resident CTA missing); results are invalid";
+    return -1.0;
   }
   return (double)ms;
 }
@@ -509,6 +347,39 @@ extern "C" int b200tts_wavernn_upsample(b200tts_wavernn* ctx, const float* d_mel
 }
 
 // ---- generation -----------------------------------------------------------------------------------
+// The step kernel a launch runs; the values are those b200tts_wavernn_last_kernel reports.
+enum StepKernel { SK_UTTERANCE = 1, SK_GRID = 2, SK_PUSH = 3, SK_TC = 5 };
+
+// The fields every step kernel's arguments take from GenArgs as they are: noise, debug buffers, labels.
+template <class Args>
+static void copy_gen_fields(Args& a, const GenArgs& g) {
+  a.rng_mode = g.rng_mode; a.seed = g.seed; a.utt_offset = g.utt_offset; a.utt_ids = g.utt_ids; a.q = g.q;
+  a.teacher = g.teacher; a.logits_out = g.logits_out; a.labels = g.labels;
+}
+
+// Zeroed phase counters [ncta][12] for the launch when `prof`, else null; records what the launch will leave in ctx->prof.
+static long long* phase_counters(b200tts_wavernn* ctx, bool prof, int ncta, cudaStream_t st) {
+  if (!prof) return nullptr;
+  const size_t bytes = (size_t)ncta * 12 * sizeof(long long);
+  ctx->prof.ensure(bytes);
+  B200_CUDA(cudaMemsetAsync(ctx->prof.p, 0, bytes, st));
+  ctx->prof_ncta = ncta;
+  return ctx->prof.as<long long>();
+}
+
+// Cooperative launch of a persistent step kernel whose `ncta` CTAs must all be resident at once, timed by ev0 / ev1.
+static void coop_launch(b200tts_wavernn* ctx, const void* kern, const char* what, int ncta, int threads, size_t smem, void** args,
+                        cudaStream_t st) {
+  B200_CUDA(cudaFuncSetAttribute(kern, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)smem));
+  int per_sm = 0;
+  B200_CUDA(cudaOccupancyMaxActiveBlocksPerMultiprocessor(&per_sm, kern, threads, smem));
+  REQUIRE(per_sm * ctx->sm_count >= ncta, B200TTS_EINVAL, std::string(what) + " cannot be made co-resident on this device");
+  B200_CUDA(cudaEventRecord(ctx->ev0, st));
+  B200_CUDA(cudaLaunchCooperativeKernel(kern, dim3(ncta), dim3(threads), args, smem, st));
+  ctx->launches++;
+  B200_CUDA(cudaEventRecord(ctx->ev1, st));
+}
+
 template <int G>
 static void launch_utt(b200tts_wavernn* ctx, const GenArgs& a, cudaStream_t st) {
   const StepWeights& w = ctx->sw;
@@ -517,38 +388,11 @@ static void launch_utt(b200tts_wavernn* ctx, const GenArgs& a, cudaStream_t st) 
   REQUIRE(smem <= 227 * 1024, B200TTS_EINVAL, "model too large for the utterance kernel's shared memory");
   B200_CUDA(cudaFuncSetAttribute(wavernn_utt_kernel<G>, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)smem));
   int grid = (a.B + G - 1) / G;
+  B200_CUDA(cudaEventRecord(ctx->ev0, st));
   wavernn_utt_kernel<G><<<grid, kUttThreads, smem, st>>>(w, a);
   B200_CUDA(cudaGetLastError());
   ctx->launches++;
-}
-
-template <int U, int UW, int GROUPS>
-static void launch_grid_t(b200tts_wavernn* ctx, GridArgs& a, cudaStream_t st) {
-  const GridModel& g = ctx->gm;
-  using MT = MapTraits<U, UW, GROUPS>;
-  constexpr int kThreads = MT::NW * 32;
-  size_t smem = ((size_t)g.blob + (size_t)MT::kScratchFloats) * sizeof(float);
-  auto kern = wavernn_grid_kernel<U, UW, GROUPS>;
-  B200_CUDA(cudaFuncSetAttribute(kern, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)smem));
-  int per_sm = 0;
-  B200_CUDA(cudaOccupancyMaxActiveBlocksPerMultiprocessor(&per_sm, kern, kThreads, smem));
-  REQUIRE(per_sm * ctx->sm_count >= g.ncta, B200TTS_EINVAL, "grid kernel cannot be made co-resident on this device");
-  GridModel gm = g;
-  void* args[] = {(void*)&gm, (void*)&a};
-  B200_CUDA(cudaLaunchCooperativeKernel((const void*)kern, dim3(g.ncta), dim3(kThreads), args, smem, st));
-  ctx->launches++;
-}
-
-// Mapping for B utterances: returns the padded batch; variant = index into the dispatch table below.
-enum { GV_N4, GV_W1, GV_W2, GV_W4, GV_W4x2 };
-static int grid_variant(int B, int* variant) {
-  if (B <= 4) { *variant = GV_N4; return 4; }
-  if (B <= 32) { *variant = GV_W1; return 32; }     // 5..8 utterances too: on the previous GPU the 8-row narrow mapping
-                                                    // measured 30.7 us/step against 29.4 us for this one
-  if (B <= 64) { *variant = GV_W2; return 64; }
-  if (B <= 128) { *variant = GV_W4; return 128; }
-  *variant = GV_W4x2;
-  return (B + 255) / 256 * 256;
+  B200_CUDA(cudaEventRecord(ctx->ev1, st));
 }
 
 struct FoldGeom {           // fold_with_overlap geometry (fatchord_version.py:319-330)
@@ -566,13 +410,58 @@ static FoldGeom fold_geometry(int S, int target, int overlap) {
   return g;
 }
 
+// `fold` != null: `a` describes the folded problem (B = nfold, S = T = L, hop = 1); the conditioning of the single source utterance
+// of S0 samples, in ctx->mels_up [S0][feat] / ctx->aux_frames [T0][O], is cut into the per-fold rows this kernel reads first.
+static void launch_utterance(b200tts_wavernn* ctx, GenArgs a, cudaStream_t st, const FoldGeom* fold, int S0) {
+  const b200tts_wavernn_cfg& c = ctx->cfg;
+  if (fold) {
+    const int O = c.res_out_dims;
+    ctx->fold_mels.ensure((size_t)a.B * a.S * c.feat_dims * sizeof(float));
+    ctx->fold_aux.ensure((size_t)a.B * a.S * O * sizeof(float));
+    size_t n = (size_t)a.B * a.S * (c.feat_dims + O);
+    unsigned grid = (unsigned)std::min<size_t>((n + 255) / 256, (size_t)ctx->sm_count * 32);
+    fold_cond_kernel<<<grid, 256, 0, st>>>(ctx->mels_up.as<float>(), ctx->aux_frames.as<float>(), S0, c.hop_length, c.feat_dims, O,
+                                           fold->L, fold->stride, fold->nfold, ctx->fold_mels.as<float>(), ctx->fold_aux.as<float>());
+    B200_CUDA(cudaGetLastError());
+    ctx->launches++;
+    a.mels_up = ctx->fold_mels.as<float>();
+    a.aux_frames = ctx->fold_aux.as<float>();
+  }
+  // utterances per CTA: enough CTAs to cover the SMs first, then amortise the L2 weight stream over more rows
+  int per = (a.B + ctx->sm_count - 1) / ctx->sm_count;
+  if (per <= 1) launch_utt<1>(ctx, a, st);
+  else if (per <= 2) launch_utt<2>(ctx, a, st);
+  else if (per <= 4) launch_utt<4>(ctx, a, st);
+  else launch_utt<8>(ctx, a, st);
+}
+
+template <int U, int UW, int GROUPS>
+static void launch_grid_t(b200tts_wavernn* ctx, GridArgs& a, cudaStream_t st) {
+  using MT = MapTraits<U, UW, GROUPS>;
+  GridModel gm = ctx->gm;
+  size_t smem = ((size_t)gm.blob + (size_t)MT::kScratchFloats) * sizeof(float);
+  void* args[] = {(void*)&gm, (void*)&a};
+  coop_launch(ctx, (const void*)wavernn_grid_kernel<U, UW, GROUPS>, "grid kernel", gm.ncta, MT::NW * 32, smem, args, st);
+}
+
+// Mapping for B utterances: returns the padded batch; variant = index into the dispatch table below.
+enum { GV_N4, GV_W1, GV_W2, GV_W4, GV_W4x2 };
+static int grid_variant(int B, int* variant) {
+  if (B <= 4) { *variant = GV_N4; return 4; }
+  if (B <= 32) { *variant = GV_W1; return 32; }     // 5..8 utterances too: on the previous GPU the 8-row narrow mapping
+                                                    // measured 30.7 us/step against 29.4 us for this one
+  if (B <= 64) { *variant = GV_W2; return 64; }
+  if (B <= 128) { *variant = GV_W4; return 128; }
+  *variant = GV_W4x2;
+  return (B + 255) / 256 * 256;
+}
+
 // `fold` != null: `ua` already describes the folded problem (B = nfold, S = T = L, hop = 1) and the conditioning of the
 // single source utterance is in ctx->mels_up [S0][feat] / ctx->aux_frames [T0][O].
-static void launch_grid(b200tts_wavernn* ctx, const float* d_mel, GenArgs& ua, cudaStream_t st, const FoldGeom* fold = nullptr,
-                        int S0 = 0) {
+static void launch_grid(b200tts_wavernn* ctx, const float* d_mel, const GenArgs& ua, bool prof, cudaStream_t st,
+                        const FoldGeom* fold, int S0) {
   const b200tts_wavernn_cfg& c = ctx->cfg;
   const GridModel& g = ctx->gm;
-  REQUIRE(g.ok, B200TTS_EINVAL, "this model/device cannot run the grid kernel (use B200TTS_KERNEL_UTTERANCE)");
   int variant = 0;
   const int B = ua.B, T = ua.T, S = ua.S, O = c.res_out_dims;
   const int Bp = grid_variant(B, &variant);
@@ -613,21 +502,12 @@ static void launch_grid(b200tts_wavernn* ctx, const float* d_mel, GenArgs& ua, c
   a.f1 = base + 6 * RB; a.f2 = base + 7 * RB;
   a.best = ctx->grid_sync.as<unsigned long long>();
   a.barrier = reinterpret_cast<unsigned int*>(ctx->grid_sync.as<char>() + 2 * (size_t)Bp * sizeof(unsigned long long));
-  a.error = reinterpret_cast<int*>(a.barrier + 96);
-  ctx->d_grid_error = a.error;
+  a.error = ctx->error.as<int>();
   a.mels_T = ctx->mels_T.as<float>();
   a.aux_T = ctx->aux_T.as<float>();
   a.B = B; a.Bp = Bp; a.S = S; a.T = T; a.hop = ua.hop; a.steps = ua.steps;
-  a.rng_mode = ua.rng_mode; a.seed = ua.seed; a.utt_offset = ua.utt_offset; a.utt_ids = ua.utt_ids; a.q = ua.q;
-  a.teacher = ua.teacher; a.logits_out = ua.logits_out; a.labels = ua.labels;
-  a.prof = nullptr;
-  if (getenv("B200TTS_GRID_PROF")) {
-    ctx->grid_prof.ensure((size_t)g.ncta * 12 * sizeof(long long));
-    B200_CUDA(cudaMemsetAsync(ctx->grid_prof.p, 0, (size_t)g.ncta * 12 * sizeof(long long), st));
-    a.prof = ctx->grid_prof.as<long long>();
-    ctx->last_grid_ncta = g.ncta;
-  }
-  B200_CUDA(cudaEventRecord(ctx->ev0, st));
+  copy_gen_fields(a, ua);
+  a.prof = phase_counters(ctx, prof, g.ncta, st);
   switch (variant) {
     case GV_N4: launch_grid_t<0, 4, 1>(ctx, a, st); break;
     case GV_W1: launch_grid_t<1, 1, 1>(ctx, a, st); break;
@@ -636,34 +516,35 @@ static void launch_grid(b200tts_wavernn* ctx, const float* d_mel, GenArgs& ua, c
     case GV_W4x2: launch_grid_t<4, 1, 2>(ctx, a, st); break;
     default: REQUIRE(false, B200TTS_EINVAL, "internal: unknown grid variant");
   }
-  B200_CUDA(cudaEventRecord(ctx->ev1, st));
+}
+
+// Conditioning tables [tab_rows][T+1][ncta][52] of the push and tensor-core kernels from the first `src_rows` utterances of the
+// mels / frame-rate aux; table rows past them are zero.
+static const float* launch_cond_table(b200tts_wavernn* ctx, const float* d_mel, const float* aux_frames, int src_rows, int tab_rows,
+                                      int T, cudaStream_t st) {
+  const b200tts_wavernn_cfg& c = ctx->cfg;
+  constexpr int FT = 8;
+  ctx->push_tab.ensure((size_t)tab_rows * (T + 1) * ctx->pm.ncta * kPushCondRows * sizeof(float));
+  dim3 grid((T + 1 + FT - 1) / FT, tab_rows);
+  size_t smem = (size_t)(c.feat_dims + c.res_out_dims) * FT * sizeof(float);
+  push_cond_table_kernel<FT><<<grid, 256, smem, st>>>(ctx->pcw, d_mel, aux_frames, src_rows, T, ctx->push_tab.as<float>());
+  B200_CUDA(cudaGetLastError());
+  ctx->launches++;
+  return ctx->push_tab.as<float>();
 }
 
 // ---- small-batch push kernel (wavernn_push.cuh) --------------------------------------------------------------------------
 template <int G>
 static void launch_push_t(b200tts_wavernn* ctx, PushArgs& a, cudaStream_t st) {
-  const PushModel& pm = ctx->pm;
-  using PT = PushTraits<G>;
-  size_t smem = ((size_t)pm.blob + (size_t)PT::scratch_floats(a.hop, a.NT)) * sizeof(float);
-  auto kern = wavernn_push_kernel<G>;
-  B200_CUDA(cudaFuncSetAttribute(kern, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)smem));
-  int per_sm = 0;
-  B200_CUDA(cudaOccupancyMaxActiveBlocksPerMultiprocessor(&per_sm, kern, kPushThreads, smem));
-  REQUIRE(per_sm * ctx->sm_count >= pm.ncta, B200TTS_EINVAL, "push kernel cannot be made co-resident on this device");
-  PushModel m = pm;
-  void* args[] = {(void*)&m, (void*)&a};
-  B200_CUDA(cudaLaunchCooperativeKernel((const void*)kern, dim3(pm.ncta), dim3(kPushThreads), args, smem, st));
-  ctx->launches++;
+  PushModel pm = ctx->pm;
+  size_t smem = ((size_t)pm.blob + (size_t)PushTraits<G>::scratch_floats(a.hop, a.NT)) * sizeof(float);
+  void* args[] = {(void*)&pm, (void*)&a};
+  coop_launch(ctx, (const void*)wavernn_push_kernel<G>, "push kernel", pm.ncta, kPushThreads, smem, args, st);
 }
 
 // rows of the push kernel variant: up to 8 rows run the 8-row variant (on the previous GPU a 4-row variant was slower, its
 // 64 hot L2 lines being polled by 65 536 threads)
 static inline int push_rows(int B) { return B <= 8 ? 8 : (B <= 16 ? 16 : kPushMaxRows); }
-
-// Can this call take the push kernel?
-static bool push_eligible(const b200tts_wavernn* ctx, int rows) {
-  return ctx->pm.ok && ctx->gm.ok && rows <= kPushMaxRows;
-}
 
 // `fold` != null: rows are the folds of ONE source utterance of T0 frames (conditioning tables of utterance 0, row u
 // starts at sample u * stride); otherwise row u is utterance u.
@@ -672,95 +553,52 @@ struct PackInfo {            // gen_opts.d_pack_*: kernel rows run queues of utt
   const int* start;
   int rows, segs, steps, n_utt;
 };
-static void launch_push(b200tts_wavernn* ctx, const float* d_mel, GenArgs& ua, cudaStream_t st, const FoldGeom* fold, int T0,
-                        const PackInfo* pack = nullptr) {
-  const b200tts_wavernn_cfg& c = ctx->cfg;
+static void launch_push(b200tts_wavernn* ctx, const float* d_mel, const GenArgs& ua, bool prof, cudaStream_t st,
+                        const FoldGeom* fold, int T0, const PackInfo* pack) {
   const PushModel& pm = ctx->pm;
   const int rows = pack ? pack->rows : ua.B;
   const int G = push_rows(rows);
-  const int T = fold ? T0 : ua.T, hop = c.hop_length;
+  const int T = fold ? T0 : ua.T, hop = ctx->cfg.hop_length;
   const int tab_rows = fold ? 1 : (pack ? pack->n_utt : G), src_rows = fold ? 1 : (pack ? pack->n_utt : rows);
-  // conditioning tables [tab_rows][T+1][ncta][52]
-  ctx->push_tab.ensure((size_t)tab_rows * (T + 1) * pm.ncta * kPushCondRows * sizeof(float));
-  {
-    constexpr int FT = 8;
-    dim3 grid((T + 1 + FT - 1) / FT, tab_rows);
-    size_t smem = (size_t)(c.feat_dims + c.res_out_dims) * FT * sizeof(float);
-    push_cond_table_kernel<FT><<<grid, 256, smem, st>>>(ctx->pcw, d_mel, ua.aux_frames, src_rows, T, ctx->push_tab.as<float>());
-    B200_CUDA(cudaGetLastError());
-    ctx->launches++;
-  }
+  PushArgs a{};
+  a.tab = launch_cond_table(ctx, d_mel, ua.aux_frames, src_rows, tab_rows, T, st);
   const size_t nvec = (size_t)kPushVecs * 2 * pm.ncta * G * 4, nbest = (size_t)pm.ncta * G;
   ctx->push_vec.ensure(nvec * sizeof(float));
-  ctx->push_best.ensure(nbest * sizeof(unsigned long long) + 64);
-  int* d_err = reinterpret_cast<int*>(ctx->push_best.as<unsigned long long>() + nbest);
-  launch_push_init(ctx->push_vec.as<uint32_t>(), nvec, ctx->push_best.as<unsigned long long>(), nbest, d_err, ctx->sm_count, st);
+  ctx->push_best.ensure(nbest * sizeof(unsigned long long));
+  launch_push_init(ctx->push_vec.as<uint32_t>(), nvec, ctx->push_best.as<unsigned long long>(), nbest, nullptr, ctx->sm_count, st);
   ctx->launches++;
-  ctx->d_grid_error = d_err;
-  PushArgs a{};
   a.wblob = ctx->push_blob.as<float>();
   a.vec = ctx->push_vec.as<float>();
   a.best = ctx->push_best.as<unsigned long long>();
-  a.error = d_err;
-  a.tab = ctx->push_tab.as<float>();
+  a.error = ctx->error.as<int>();
   a.fir = ctx->d_fir;
   a.NT = ctx->NT;
   a.B = pack ? pack->n_utt : rows; a.S = ua.S; a.T = T; a.hop = hop; a.steps = pack ? pack->steps : ua.steps;
   if (pack) { a.pack_utt = pack->utt; a.pack_start = pack->start; a.pack_segs = pack->segs; a.pack_rows = pack->rows; }
   a.row_stride = fold ? fold->stride : 0;
   a.S_src = T * hop;
-  a.rng_mode = ua.rng_mode; a.seed = ua.seed; a.utt_offset = ua.utt_offset; a.utt_ids = ua.utt_ids; a.q = ua.q;
-  a.teacher = ua.teacher; a.logits_out = ua.logits_out; a.labels = ua.labels;
-  a.prof = nullptr;
-  if (getenv("B200TTS_GRID_PROF")) {
-    ctx->push_prof.ensure((size_t)pm.ncta * 12 * sizeof(long long));
-    B200_CUDA(cudaMemsetAsync(ctx->push_prof.p, 0, (size_t)pm.ncta * 12 * sizeof(long long), st));
-    a.prof = ctx->push_prof.as<long long>();
-    ctx->last_push_ncta = pm.ncta;
-    ctx->last_grid_ncta = 0;
-  }
-  B200_CUDA(cudaEventRecord(ctx->ev0, st));
+  copy_gen_fields(a, ua);
+  a.prof = phase_counters(ctx, prof, pm.ncta, st);
   switch (G) {
     case 8: launch_push_t<8>(ctx, a, st); break;
     case 16: launch_push_t<16>(ctx, a, st); break;
     default: launch_push_t<32>(ctx, a, st); break;
   }
-  B200_CUDA(cudaEventRecord(ctx->ev1, st));
 }
 
-// ---- tensor-core pipeline (wavernn_tc.cuh): 33 ... 256 rows, plain batches ----------------------------------------------
-// Smallest batch kernel=auto gives the tensor cores.  On an H100 80GB HBM3 at a 400 W power limit the tensor-core pipeline costs
-// 38-41 us per lock-step whatever the row count (1 or 2 groups of 128 rows in flight; 64-69 us while its wgmma were serialized);
-// the wide CUDA-core mapping took 37.5 us at 64 rows, 60.9 at 96-128 and 90-91 from 129 rows on (a second tile of 128; 700 W).
-constexpr int kTcMinRows = 129;
-static bool tc_eligible(const b200tts_wavernn* ctx, int rows, bool folding, bool packing) {
-  return ctx->tc_ok && ctx->pm.ok && !folding && !packing && rows >= 1 && rows <= kTcRows * kTcMaxGroups;
-}
-static void launch_tc(b200tts_wavernn* ctx, const float* d_mel, GenArgs& ua, cudaStream_t st) {
-  const b200tts_wavernn_cfg& c = ctx->cfg;
-  const PushModel& pm = ctx->pm;
-  const int rows = ua.B, T = ua.T, hop = c.hop_length;
+// ---- tensor-core pipeline (wavernn_tc.cuh): plain batches of up to 256 rows ----------------------------------------------
+static void launch_tc(b200tts_wavernn* ctx, const float* d_mel, const GenArgs& ua, bool prof, cudaStream_t st) {
+  const int rows = ua.B, T = ua.T;
   const int ng = (rows + kTcRows - 1) / kTcRows;
-  ctx->push_tab.ensure((size_t)rows * (T + 1) * pm.ncta * kPushCondRows * sizeof(float));
-  {
-    constexpr int FT = 8;
-    dim3 grid((T + 1 + FT - 1) / FT, rows);
-    size_t smem = (size_t)(c.feat_dims + c.res_out_dims) * FT * sizeof(float);
-    push_cond_table_kernel<FT><<<grid, 256, smem, st>>>(ctx->pcw, d_mel, ua.aux_frames, rows, T, ctx->push_tab.as<float>());
-    B200_CUDA(cudaGetLastError());
-    ctx->launches++;
-  }
+  TcArgs a{};
+  a.tab = launch_cond_table(ctx, d_mel, ua.aux_frames, rows, rows, T, st);
   ctx->tc_vec.ensure((size_t)TV_COUNT * ng * 2 * kTcVecBytes);
   ctx->tc_x1f.ensure((size_t)ng * 2 * kTcRows * 512 * sizeof(float));
   ctx->tc_win.ensure((size_t)ng * 2 * kTcWinCopies * kTcRows * 16 * sizeof(unsigned long long));
   ctx->tc_cond.ensure((size_t)32 * 2 * ng * kTcCondBlk * kTcCondSlot * sizeof(float));
-  REQUIRE((size_t)hop * ctx->NT * sizeof(float) <= (size_t)kTcFirMaxBytes, B200TTS_EINVAL, "tensor-core kernel: FIR table does not fit its shared-memory slot");
-  const size_t ncnt = (size_t)ng * TCN_COUNT * 32;
-  ctx->tc_cnt.ensure((ncnt + 32) * sizeof(unsigned));
-  B200_CUDA(cudaMemsetAsync(ctx->tc_cnt.p, 0, (ncnt + 32) * sizeof(unsigned), st));
-  int* d_err = reinterpret_cast<int*>(ctx->tc_cnt.as<unsigned>() + ncnt);
-  ctx->d_grid_error = d_err;
-  TcArgs a{};
+  const size_t cnt_bytes = (size_t)ng * TCN_COUNT * 32 * sizeof(unsigned);
+  ctx->tc_cnt.ensure(cnt_bytes);
+  B200_CUDA(cudaMemsetAsync(ctx->tc_cnt.p, 0, cnt_bytes, st));
   a.wimg = ctx->tc_wimg.as<uint8_t>();
   a.prm = ctx->tc_prm.as<float>();
   a.vec = ctx->tc_vec.as<uint8_t>();
@@ -768,49 +606,66 @@ static void launch_tc(b200tts_wavernn* ctx, const float* d_mel, GenArgs& ua, cud
   a.winners = ctx->tc_win.as<unsigned long long>();
   a.cnt = ctx->tc_cnt.as<unsigned>();
   a.condg = ctx->tc_cond.as<float>();
-  a.error = d_err;
-  a.tab = ctx->push_tab.as<float>();
+  a.error = ctx->error.as<int>();
   a.fir = ctx->d_fir;
-  a.NT = ctx->NT; a.B = rows; a.S = ua.S; a.T = T; a.hop = hop; a.steps = ua.steps; a.ng = ng; a.NC = ctx->NC;
-  a.rng_mode = ua.rng_mode; a.seed = ua.seed; a.utt_offset = ua.utt_offset; a.utt_ids = ua.utt_ids; a.q = ua.q;
-  a.teacher = ua.teacher; a.logits_out = ua.logits_out; a.labels = ua.labels;
-  a.prof = nullptr;
-  ctx->last_tc_prof = getenv("B200TTS_GRID_PROF") != nullptr;
-  if (ctx->last_tc_prof) {
-    ctx->tc_prof.ensure((size_t)kTcCtas * 12 * sizeof(long long));
-    B200_CUDA(cudaMemsetAsync(ctx->tc_prof.p, 0, (size_t)kTcCtas * 12 * sizeof(long long), st));
-    a.prof = ctx->tc_prof.as<long long>();
-  }
-  ctx->last_push_ncta = 0;
-  ctx->last_grid_ncta = 0;
-  B200_CUDA(cudaFuncSetAttribute(wavernn_tc_kernel, cudaFuncAttributeMaxDynamicSharedMemorySize, kTcSmemBytes));
-  int per_sm = 0;
-  B200_CUDA(cudaOccupancyMaxActiveBlocksPerMultiprocessor(&per_sm, wavernn_tc_kernel, kTcThreads, (size_t)kTcSmemBytes));
-  REQUIRE(per_sm * ctx->sm_count >= kTcCtas, B200TTS_EINVAL, "tensor-core kernel cannot be made co-resident on this device");
-  B200_CUDA(cudaEventRecord(ctx->ev0, st));
+  a.NT = ctx->NT; a.B = rows; a.S = ua.S; a.T = T; a.hop = ctx->cfg.hop_length; a.steps = ua.steps; a.ng = ng; a.NC = ctx->NC;
+  copy_gen_fields(a, ua);
+  a.prof = phase_counters(ctx, prof, kTcCtas, st);
   void* args[] = {(void*)&a};
-  B200_CUDA(cudaLaunchCooperativeKernel((const void*)wavernn_tc_kernel, dim3(kTcCtas), dim3(kTcThreads), args, (size_t)kTcSmemBytes, st));
-  ctx->launches++;
-  B200_CUDA(cudaEventRecord(ctx->ev1, st));
+  coop_launch(ctx, (const void*)wavernn_tc_kernel, "tensor-core kernel", kTcCtas, kTcThreads, kTcSmemBytes, args, st);
 }
 
-// After the stream has been synchronised: did the last grid launch abandon a barrier?
-static void check_grid_error(b200tts_wavernn* ctx) {
-  if (!ctx->d_grid_error) return;
+// After the stream has been synchronised: did a kernel of the last generate call give up waiting for a peer CTA?
+static void check_call_error(b200tts_wavernn* ctx) {
   int flag = 0;
-  B200_CUDA(cudaMemcpy(&flag, ctx->d_grid_error, sizeof(int), cudaMemcpyDeviceToHost));
+  B200_CUDA(cudaMemcpy(&flag, ctx->error.p, sizeof(int), cudaMemcpyDeviceToHost));
   REQUIRE(flag == 0, B200TTS_ECUDA, "grid kernel: a grid-barrier wait timed out (co-resident CTA missing); results are invalid");
 }
 
-static void run_generate_rows(b200tts_wavernn* ctx, const float* d_mel, int B, int T, const b200tts_rng* rng,
-                              const b200tts_gen_opts* opts, int16_t* d_labels, double* d_wave, cudaStream_t st) {
+// Smallest batch kernel=auto gives the tensor cores.  On an H100 80GB HBM3 at a 400 W power limit the tensor-core pipeline costs
+// 38-41 us per lock-step whatever the row count (1 or 2 groups of 128 rows in flight; 64-69 us while its wgmma were serialized);
+// the wide CUDA-core mapping took 37.5 us at 64 rows, 60.9 at 96-128 and 90-91 from 129 rows on (a second tile of 128; 700 W).
+constexpr int kTcMinRows = 129;
+
+// The step kernel for `rows` kernel rows (folds when folding) under `o`, or a refusal.  Every capability it reads is fixed at
+// create time, so a refused call has launched nothing.
+static StepKernel choose_kernel(b200tts_wavernn* ctx, int rows, const b200tts_gen_opts& o) {
+  const bool packing = o.d_pack_utt != nullptr;
+  // tc_ok implies pm.ok implies gm.ok (pack_tc_images, pack_push_model)
+  const bool tc = ctx->tc_ok && o.fold_target == 0 && !packing && rows <= kTcRows * kTcMaxGroups;
+  const bool push = ctx->pm.ok && (packing ? o.pack_rows : rows) <= kPushMaxRows;
+  int kernel = o.kernel;
+  if (kernel == B200TTS_KERNEL_AUTO) {
+    if (tc && rows >= kTcMinRows) return SK_TC;       // fold mode and packed rows stay on the other kernels
+    if (!ctx->gm.ok && !ctx->warned_fallback) {      // never silently: this path is ~4x slower
+      ctx->warned_fallback = true;
+      fprintf(stderr, "libb200tts: these hparams / this device cannot run the weight-stationary grid kernel; kernel=auto falls "
+                      "back to the L2-streaming utterance kernel (about 4x slower at large batch)\n");
+    }
+    kernel = ctx->gm.ok ? B200TTS_KERNEL_GRID : B200TTS_KERNEL_UTTERANCE;
+  }
+  switch (kernel) {
+    case B200TTS_KERNEL_TC:
+      REQUIRE(tc, B200TTS_EINVAL, "kernel=tc needs rnn_dims = fc_dims = 512, 10-bit classes, hop_length x FIR taps <= 8192, "
+                                  ">= 128 SMs, 1..256 rows, no folding / packing");
+      return SK_TC;
+    case B200TTS_KERNEL_GRID:
+      if (push) return SK_PUSH;
+      break;
+    case B200TTS_KERNEL_UTTERANCE: break;
+    default: throw Error(B200TTS_EINVAL, "unknown kernel selector");
+  }
+  REQUIRE(!packing, B200TTS_EINVAL, "packed generation needs the push kernel (kernel=auto/grid, rnn_dims = fc_dims = 512)");
+  if (kernel == B200TTS_KERNEL_UTTERANCE) return SK_UTTERANCE;
+  REQUIRE(ctx->gm.ok, B200TTS_EINVAL, "kernel=grid was requested but this model/device cannot run the weight-stationary grid kernel "
+                                      "(needs rnn_dims == fc_dims, n_classes == 2*rnn_dims, cooperative launch, R/4 <= SM count)");
+  return SK_GRID;
+}
+
+static void run_generate_rows(b200tts_wavernn* ctx, const float* d_mel, int B, int T, const b200tts_rng& r,
+                              const b200tts_gen_opts& o, bool prof, int16_t* d_labels, double* d_wave, cudaStream_t st) {
   const b200tts_wavernn_cfg& c = ctx->cfg;
   const int hop = c.hop_length, S = T * hop, O = c.res_out_dims;
-  b200tts_gen_opts o{};
-  if (opts) o = *opts;
-  else o.mu_law = 1;
-  b200tts_rng r{};
-  if (rng) r = *rng;
   REQUIRE(r.mode == B200TTS_RNG_PHILOX || r.mode == B200TTS_RNG_EXT_EXPONENTIAL, B200TTS_EINVAL, "unknown rng mode");
   REQUIRE(r.mode != B200TTS_RNG_EXT_EXPONENTIAL || r.d_q, B200TTS_EINVAL, "EXT_EXPONENTIAL needs d_q");
   REQUIRE(o.max_steps >= 0 && o.max_steps <= S, B200TTS_EINVAL, "max_steps out of range");
@@ -822,17 +677,6 @@ static void run_generate_rows(b200tts_wavernn* ctx, const float* d_mel, int B, i
     REQUIRE(wave_len >= fade_len, B200TTS_EINVAL,
             "T must be >= 21 frames: the reference's 20-hop fade-out (fatchord_version.py:256-258) fails below that");
   }
-  int kernel = o.kernel;
-  if (kernel == B200TTS_KERNEL_AUTO) {
-    kernel = ctx->gm.ok ? B200TTS_KERNEL_GRID : B200TTS_KERNEL_UTTERANCE;
-    if (!ctx->gm.ok && !ctx->warned_fallback) {      // never silently: this path is ~4x slower
-      ctx->warned_fallback = true;
-      fprintf(stderr, "libb200tts: these hparams / this device cannot run the weight-stationary grid kernel; kernel=auto falls "
-                      "back to the L2-streaming utterance kernel (about 4x slower at large batch)\n");
-    }
-  }
-  REQUIRE(kernel == B200TTS_KERNEL_UTTERANCE || kernel == B200TTS_KERNEL_GRID || kernel == B200TTS_KERNEL_TC, B200TTS_EINVAL,
-          "unknown kernel selector");
   const bool folding = o.fold_target > 0;
   FoldGeom fg{};
   if (folding) {
@@ -840,6 +684,7 @@ static void run_generate_rows(b200tts_wavernn* ctx, const float* d_mel, int B, i
     REQUIRE(o.fold_overlap >= 2 && o.fold_target >= 1, B200TTS_EINVAL, "fold target/overlap out of range");
     REQUIRE(steps == S, B200TTS_EINVAL, "max_steps is not supported together with folding");
     REQUIRE(S > o.fold_overlap, B200TTS_EINVAL, "utterance shorter than the fold overlap");
+    REQUIRE(!r.d_utterance_ids, B200TTS_EINVAL, "d_utterance_ids cannot be combined with fold-with-overlap generation");
     fg = fold_geometry(S, o.fold_target, o.fold_overlap);
     REQUIRE(fg.nfold >= 1 && fg.nfold <= 65535, B200TTS_EINVAL, "fold count out of range");
   }
@@ -852,29 +697,17 @@ static void run_generate_rows(b200tts_wavernn* ctx, const float* d_mel, int B, i
   }
   const int GB = folding ? fg.nfold : B;            // rows the generation kernels see
   const int GS = folding ? fg.L : S;                // steps per row
+  const StepKernel kernel = choose_kernel(ctx, GB, o);
+  ctx->last_kernel = kernel;
+  ctx->prof_ncta = 0;
   ctx->aux_frames.ensure((size_t)B * T * O * sizeof(float));
   int16_t* labels = d_labels;
   if (!labels) {
     ctx->labels.ensure((size_t)GB * GS * sizeof(int16_t));
     labels = ctx->labels.as<int16_t>();
   }
-  bool use_tc = false;
-  // kernel=auto: the tensor cores take kTcMinRows rows and more.  Fold mode and packed rows stay on the other kernels.
-  if (o.kernel == B200TTS_KERNEL_AUTO && kernel == B200TTS_KERNEL_GRID && GB >= kTcMinRows && tc_eligible(ctx, GB, folding, packing))
-    kernel = B200TTS_KERNEL_TC;
-  if (kernel == B200TTS_KERNEL_TC) {
-    REQUIRE(tc_eligible(ctx, GB, folding, packing), B200TTS_EINVAL,
-            "kernel=tc needs rnn_dims = fc_dims = 512, 10-bit classes, >= 128 SMs, 1..256 rows, no folding / packing");
-    use_tc = true;
-    kernel = B200TTS_KERNEL_GRID;
-  }
-  const bool use_push = !use_tc && kernel == B200TTS_KERNEL_GRID && push_eligible(ctx, packing ? o.pack_rows : GB);
-  REQUIRE(!packing || use_push, B200TTS_EINVAL, "packed generation needs the push kernel (kernel=auto/grid, rnn_dims = fc_dims = 512)");
-  if (kernel == B200TTS_KERNEL_GRID && !ctx->gm.ok)
-    throw Error(B200TTS_EINVAL, "kernel=grid was requested but this model/device cannot run the weight-stationary grid kernel "
-                                "(needs rnn_dims == fc_dims, n_classes == 2*rnn_dims, cooperative launch, R/4 <= SM count)");
   float* mels_up = nullptr;
-  if (kernel == B200TTS_KERNEL_UTTERANCE || (folding && !use_push)) {
+  if (kernel == SK_UTTERANCE || (folding && kernel == SK_GRID)) {
     ctx->mels_up.ensure((size_t)B * S * c.feat_dims * sizeof(float));
     mels_up = ctx->mels_up.as<float>();
   }
@@ -886,49 +719,25 @@ static void run_generate_rows(b200tts_wavernn* ctx, const float* d_mel, int B, i
   a.B = GB; a.S = GS; a.T = folding ? GS : T; a.hop = folding ? 1 : hop; a.steps = folding ? GS : steps;
   a.rng_mode = r.mode; a.seed = r.seed; a.utt_offset = r.utterance_offset; a.q = r.d_q;
   a.utt_ids = reinterpret_cast<const unsigned long long*>(r.d_utterance_ids);
-  REQUIRE(!(folding && r.d_utterance_ids), B200TTS_EINVAL, "d_utterance_ids cannot be combined with fold-with-overlap generation");
   a.teacher = o.d_teacher; a.logits_out = o.d_logits; a.labels = labels;
 
-  ctx->last_kernel = kernel == B200TTS_KERNEL_UTTERANCE ? 1 : (use_tc ? 5 : (use_push ? 3 : 2));
-  if (kernel == B200TTS_KERNEL_UTTERANCE) {
-    if (folding) {   // per-fold conditioning in the row-major layout this kernel reads, aux per sample (hop = 1)
-      ctx->fold_mels.ensure((size_t)GB * GS * c.feat_dims * sizeof(float));
-      ctx->fold_aux.ensure((size_t)GB * GS * O * sizeof(float));
-      size_t n = (size_t)GB * GS * (c.feat_dims + O);
-      unsigned grid = (unsigned)std::min<size_t>((n + 255) / 256, (size_t)ctx->sm_count * 32);
-      fold_cond_kernel<<<grid, 256, 0, st>>>(ctx->mels_up.as<float>(), ctx->aux_frames.as<float>(), S, hop, c.feat_dims, O, fg.L,
-                                             fg.stride, fg.nfold, ctx->fold_mels.as<float>(), ctx->fold_aux.as<float>());
-      B200_CUDA(cudaGetLastError());
-      ctx->launches++;
-      a.mels_up = ctx->fold_mels.as<float>();
-      a.aux_frames = ctx->fold_aux.as<float>();
-    }
-    ctx->d_grid_error = nullptr;
-    B200_CUDA(cudaEventRecord(ctx->ev0, st));
-    // utterances per CTA: enough CTAs to cover the SMs first, then amortise the L2 weight stream over more rows
-    int per = (GB + ctx->sm_count - 1) / ctx->sm_count;
-    if (per <= 1) launch_utt<1>(ctx, a, st);
-    else if (per <= 2) launch_utt<2>(ctx, a, st);
-    else if (per <= 4) launch_utt<4>(ctx, a, st);
-    else launch_utt<8>(ctx, a, st);
-    B200_CUDA(cudaEventRecord(ctx->ev1, st));
-  } else if (use_tc) {
-    launch_tc(ctx, d_mel, a, st);
-  } else if (use_push) {
-    PackInfo pi{o.d_pack_utt, o.d_pack_start, o.pack_rows, o.pack_segs, o.pack_steps, B};
-    launch_push(ctx, d_mel, a, st, folding ? &fg : nullptr, T, packing ? &pi : nullptr);
-  } else {
-    launch_grid(ctx, d_mel, a, st, folding ? &fg : nullptr, S);
+  const FoldGeom* fold = folding ? &fg : nullptr;
+  const PackInfo pi{o.d_pack_utt, o.d_pack_start, o.pack_rows, o.pack_segs, o.pack_steps, B};
+  switch (kernel) {
+    case SK_UTTERANCE: launch_utterance(ctx, a, st, fold, S); break;
+    case SK_GRID: launch_grid(ctx, d_mel, a, prof, st, fold, S); break;
+    case SK_PUSH: launch_push(ctx, d_mel, a, prof, st, fold, T, packing ? &pi : nullptr); break;
+    case SK_TC: launch_tc(ctx, d_mel, a, prof, st); break;
   }
   ctx->ev_valid = true;
   if (d_wave) {
     if (folding) {
       xfade_unfold_kernel<<<(wave_len + 255) / 256, 256, 0, st>>>(labels, fg.nfold, fg.L, o.fold_target, o.fold_overlap, wave_len,
-                                                                  fade_len, ctx->NC, o.mu_law, ctx->d_grid_error, d_wave);
+                                                                  fade_len, ctx->NC, o.mu_law, ctx->error.as<int>(), d_wave);
     } else {
       dim3 grid((wave_len + 255) / 256, B);
-      finish_wave_kernel<<<grid, 256, 0, st>>>(labels, S, wave_len, fade_len, ctx->NC, o.mu_law, o.d_utt_frames, hop, ctx->d_grid_error,
-                                               d_wave);
+      finish_wave_kernel<<<grid, 256, 0, st>>>(labels, S, wave_len, fade_len, ctx->NC, o.mu_law, o.d_utt_frames, hop,
+                                               ctx->error.as<int>(), d_wave);
     }
     B200_CUDA(cudaGetLastError());
     ctx->launches++;
@@ -941,36 +750,37 @@ static void run_generate_rows(b200tts_wavernn* ctx, const float* d_mel, int B, i
 // (Not for the debug modes whose buffers are indexed [step][row]: external noise, logits.)
 static void run_generate(b200tts_wavernn* ctx, const float* d_mel, int B, int T, const b200tts_rng* rng,
                          const b200tts_gen_opts* opts, int16_t* d_labels, double* d_wave, cudaStream_t st) {
+  b200tts_rng r{};
+  if (rng) r = *rng;
+  b200tts_gen_opts o{};
+  if (opts) o = *opts;
+  else o.mu_law = 1;
+  const bool prof = getenv("B200TTS_GRID_PROF") != nullptr;
+  B200_CUDA(cudaMemsetAsync(ctx->error.p, 0, sizeof(int), st));    // one error word for every slice of the call
   const double budget = getenv("B200TTS_MAX_COND_BYTES") ? atof(getenv("B200TTS_MAX_COND_BYTES")) : 8e9;   // read per call
   const b200tts_wavernn_cfg& c = ctx->cfg;
   const double per_row = (double)T * c.hop_length * c.feat_dims * sizeof(float);
-  const bool debug_bufs = (rng && rng->mode == B200TTS_RNG_EXT_EXPONENTIAL) || (opts && opts->d_logits);
-  const bool folding = opts && opts->fold_target > 0;
-  const bool packing = opts && opts->d_pack_utt;
+  const bool whole = r.mode == B200TTS_RNG_EXT_EXPONENTIAL || o.d_logits || o.fold_target > 0 || o.d_pack_utt || !d_labels;
   // kernel=auto and more than 256 rows: launches of 256 rows through the tensor-core pipeline (66 us per lock-step each on an H100)
   // beat the wide mapping on the whole batch (91 us per 256 rows); the noise is keyed by the global row, so the result does not change
-  const bool tc_slices = B > kTcRows * kTcMaxGroups && (!opts || opts->kernel == B200TTS_KERNEL_AUTO) && !debug_bufs && d_labels &&
-                         tc_eligible(ctx, kTcRows * kTcMaxGroups, folding, packing);
-  const bool sliceable = tc_slices || B > 256 || per_row * 256 > budget;
-  if (!sliceable || debug_bufs || folding || packing || (!tc_slices && per_row * ((B + 255) / 256 * 256) <= budget) || !d_labels) {
-    run_generate_rows(ctx, d_mel, B, T, rng, opts, d_labels, d_wave, st);
+  constexpr int kTcSlice = kTcRows * kTcMaxGroups;
+  const bool tc_slices = !whole && B > kTcSlice && o.kernel == B200TTS_KERNEL_AUTO && choose_kernel(ctx, kTcSlice, o) == SK_TC;
+  if (whole || (!tc_slices && per_row * ((B + 255) / 256 * 256) <= budget)) {
+    run_generate_rows(ctx, d_mel, B, T, r, o, prof, d_labels, d_wave, st);
     return;
   }
-  int rows = tc_slices ? kTcRows * kTcMaxGroups : (int)(budget / per_row);
+  int rows = tc_slices ? kTcSlice : (int)(budget / per_row);
   if (!tc_slices) rows = rows >= 256 ? rows / 256 * 256 : (rows >= 32 ? 32 : std::max(rows, 1));
   const size_t S = (size_t)T * c.hop_length, wave_len = (size_t)(T - 1) * c.hop_length;
   for (int r0 = 0; r0 < B; r0 += rows) {
     const int nb = std::min(rows, B - r0);
-    b200tts_rng r{};
-    if (rng) r = *rng;
-    if (r.d_utterance_ids) r.d_utterance_ids += r0;
-    else r.utterance_offset += (uint64_t)r0;
-    b200tts_gen_opts o{};
-    if (opts) o = *opts;
-    else o.mu_law = 1;
-    if (o.d_teacher) o.d_teacher += (size_t)r0 * S;
-    if (o.d_utt_frames) o.d_utt_frames += r0;
-    run_generate_rows(ctx, d_mel + (size_t)r0 * c.feat_dims * T, nb, T, &r, &o, d_labels + (size_t)r0 * S,
+    b200tts_rng rs = r;
+    if (rs.d_utterance_ids) rs.d_utterance_ids += r0;
+    else rs.utterance_offset += (uint64_t)r0;
+    b200tts_gen_opts os = o;
+    if (os.d_teacher) os.d_teacher += (size_t)r0 * S;
+    if (os.d_utt_frames) os.d_utt_frames += r0;
+    run_generate_rows(ctx, d_mel + (size_t)r0 * c.feat_dims * T, nb, T, rs, os, prof, d_labels + (size_t)r0 * S,
                       d_wave ? d_wave + (size_t)r0 * wave_len : nullptr, st);
   }
 }
@@ -1031,7 +841,7 @@ extern "C" int b200tts_wavernn_generate_host(b200tts_wavernn* ctx, const float* 
     std::memcpy(h_wave, ctx->h_stage.p, wav_bytes);
   }
   B200_CUDA(cudaStreamSynchronize(st));
-  check_grid_error(ctx);
+  check_call_error(ctx);
   API_END
 }
 
@@ -1040,41 +850,35 @@ extern "C" int b200tts_wavernn_check(b200tts_wavernn* ctx) {
   REQUIRE(ctx, B200TTS_EINVAL, "null argument");
   DeviceGuard dg(ctx->device);
   B200_CUDA(cudaDeviceSynchronize());
-  check_grid_error(ctx);
+  check_call_error(ctx);
   API_END
 }
 
-// Debug: per-phase cycle counters of the last grid-kernel launch (needs env B200TTS_GRID_PROF=1 at generate time).
-// out[12] = mean over CTAs of {P0 compute, P0 barrier, P1 compute, P1 barrier, ...} in SM cycles.
+// Debug: per-phase cycle counters of the last step-kernel launch (needs env B200TTS_GRID_PROF=1 at generate time).
+// Grid and push kernels: out[12] = mean over CTAs of {P0 compute, P0 barrier, P1 compute, P1 barrier, ...} in SM cycles.
 // Tensor-core pipeline: out[3 j + p] = cycles summed over the run of job j (GRU-2's W_ih2 . x1, fc1, fc2, fc3), phase p (exchange
 // wait, GEMM, epilogue), averaged over the CTAs of that role.
 extern "C" int b200tts_wavernn_debug_phase_cycles(b200tts_wavernn* ctx, double* out12) {
   API_BEGIN
   REQUIRE(ctx && out12, B200TTS_EINVAL, "null argument");
-  if (ctx->last_kernel == 5) {
-    REQUIRE(ctx->last_tc_prof && ctx->tc_prof.p, B200TTS_EINVAL, "no phase profile recorded");
-    DeviceGuard dg(ctx->device);
-    std::vector<long long> h((size_t)kTcCtas * 12);
-    B200_CUDA(cudaDeviceSynchronize());
-    B200_CUDA(cudaMemcpy(h.data(), ctx->tc_prof.p, h.size() * sizeof(long long), cudaMemcpyDeviceToHost));
-    int n[4] = {0, 0, 0, 0};
-    for (int i = 0; i < 12; ++i) out12[i] = 0;
-    for (int cta = 0; cta < kTcCtas; ++cta) {
-      const int j = tc_role(cta).role - 1;
-      if (j < 0) continue;
-      ++n[j];
-      for (int p = 0; p < 3; ++p) out12[3 * j + p] += (double)h[(size_t)cta * 12 + 3 * j + p];
-    }
-    for (int i = 0; i < 12; ++i) out12[i] /= n[i / 3];
-    return B200TTS_OK;
-  }
-  const bool push = ctx->last_grid_ncta == 0 && ctx->last_push_ncta > 0 && ctx->push_prof.p;
-  REQUIRE(push || (ctx->grid_prof.p && ctx->last_grid_ncta > 0), B200TTS_EINVAL, "no phase profile recorded");
+  REQUIRE(ctx->prof_ncta > 0, B200TTS_EINVAL, "no phase profile recorded");
   DeviceGuard dg(ctx->device);
-  const int n = push ? ctx->last_push_ncta : ctx->last_grid_ncta;
+  const int n = ctx->prof_ncta;
   std::vector<long long> h((size_t)n * 12);
   B200_CUDA(cudaDeviceSynchronize());
-  B200_CUDA(cudaMemcpy(h.data(), push ? ctx->push_prof.p : ctx->grid_prof.p, h.size() * sizeof(long long), cudaMemcpyDeviceToHost));
+  B200_CUDA(cudaMemcpy(h.data(), ctx->prof.p, h.size() * sizeof(long long), cudaMemcpyDeviceToHost));
+  if (ctx->last_kernel == SK_TC) {
+    int cnt[4] = {0, 0, 0, 0};
+    for (int i = 0; i < 12; ++i) out12[i] = 0;
+    for (int cta = 0; cta < n; ++cta) {
+      const int j = tc_role(cta).role - 1;
+      if (j < 0) continue;
+      ++cnt[j];
+      for (int p = 0; p < 3; ++p) out12[3 * j + p] += (double)h[(size_t)cta * 12 + 3 * j + p];
+    }
+    for (int i = 0; i < 12; ++i) out12[i] /= cnt[i / 3];
+    return B200TTS_OK;
+  }
   for (int i = 0; i < 12; ++i) {
     double s = 0;
     for (int c = 0; c < n; ++c) s += (double)h[(size_t)c * 12 + i];

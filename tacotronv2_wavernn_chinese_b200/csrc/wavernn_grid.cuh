@@ -24,7 +24,11 @@
 // other sits in a barrier -- and "narrow" for B <= 4 (activation vector staged into shared memory in one L2 round trip,
 // lanes = k, warp-shuffle reductions) where the step is pure latency.
 #pragma once
+#include <algorithm>
+#include <cstring>
+#include <vector>
 #include "common.cuh"
+#include "wavernn_utt.cuh"
 
 namespace b200tts {
 
@@ -755,6 +759,78 @@ __global__ void aux_T_kernel(const float* __restrict__ aux_frames /*[B][T][O]*/,
     size_t f = rest / O;
     aux_T[e] = u < B ? aux_frames[((size_t)u * T + f) * O + o] : 0.f;
   }
+}
+
+// ---- host: the per-CTA weight blobs [ncta][blob], cut from the step weights in their original layouts (`w` points to host
+//      memory).  Fills the layout `g`; g.ok says whether the model and device can run this kernel, and the blobs are empty
+//      when they cannot. --------------------------------------------------------------------------------------------------
+inline std::vector<float> pack_grid_model(const StepWeights& w, int sm_count, bool coop, GridModel& g) {
+  const int R = w.R, F = w.F, AUX = w.aux, FEAT = w.feat, NC = w.NC, ldI = w.ldI;
+  g = GridModel{};
+  g.R = R; g.F = F; g.AUX = AUX; g.FEAT = FEAT; g.NC = NC;
+  g.ldC = FEAT + AUX; g.ldX = R + AUX; g.ldF = F + AUX;
+  g.ncta = R / kUPC;
+  g.ok = (R == F) && (R % kUPC == 0) && (NC == g.ncta * kCPC) && (FEAT % 4 == 0) && (g.ncta <= sm_count) && coop;
+  // the narrow mapping stages [x1|aux], [f1|aux], [mel|aux] in a 640*G-float area and h in a 512*G-float area
+  if (R + AUX > 640 || F + AUX > 640 || FEAT + AUX > 640 || R > 512) g.ok = 0;
+  int off = 0;
+  auto take = [&](int n) { int o = off; off += (n + 3) & ~3; return o; };
+  g.oA_w = take(16 * g.ldC); g.oA_x = take(16); g.oA_b = take(16);
+  g.ohh1 = take(3 * kUPC * R); g.oih2 = take(3 * kUPC * g.ldX); g.ohh2 = take(3 * kUPC * R);
+  g.ofc1 = take(kUPC * g.ldX); g.ofc2 = take(kUPC * g.ldF); g.ofc3 = take(kCPC * F);
+  g.obhh1 = take(3 * kUPC); g.obih2 = take(3 * kUPC); g.obhh2 = take(3 * kUPC);
+  g.obfc1 = take(kUPC); g.obfc2 = take(kUPC); g.obfc3 = take(kCPC);
+  g.blob = off;
+  constexpr int kMaxScratch = std::max({MapTraits<0, 4, 1>::kScratchFloats, MapTraits<1, 1, 1>::kScratchFloats,
+                                        MapTraits<2, 1, 1>::kScratchFloats, MapTraits<4, 1, 1>::kScratchFloats,
+                                        MapTraits<4, 1, 2>::kScratchFloats});   // every variant launch_grid can dispatch
+  size_t smem_need = ((size_t)g.blob + (size_t)kMaxScratch) * sizeof(float) + 2048;
+  if (smem_need > 227 * 1024) g.ok = 0;
+  if (!g.ok) return {};
+
+  std::vector<float> hb((size_t)g.ncta * g.blob, 0.f);
+  std::vector<double> fold_acc(1 + g.ldC);
+  for (int cta = 0; cta < g.ncta; ++cta) {
+    float* b = &hb[(size_t)cta * g.blob];
+    for (int j = 0; j < kUPC; ++j) {
+      const int row = cta * kUPC + j;
+      const float* src = w.I_w + (size_t)row * ldI;          // [x | feat | aux] padded
+      b[g.oA_x + j] = src[0];
+      std::memcpy(b + g.oA_w + (size_t)j * g.ldC, src + 1, sizeof(float) * g.ldC);
+      b[g.oA_b + j] = w.I_b[row];
+      std::memcpy(b + g.ofc1 + (size_t)j * g.ldX, w.fc1_w + (size_t)row * g.ldX, sizeof(float) * g.ldX);
+      std::memcpy(b + g.ofc2 + (size_t)j * g.ldF, w.fc2_w + (size_t)row * g.ldF, sizeof(float) * g.ldF);
+      b[g.obfc1 + j] = w.fc1_b[row];
+      b[g.obfc2 + j] = w.fc2_b[row];
+      for (int gate = 0; gate < 3; ++gate) {
+        const int srow = gate * R + row, drow = gate * kUPC + j;
+        // folded input projection of GRU 1: row srow of W_ih1.W_I (x column | cond columns) and W_ih1.b_I + b_ih1, in double
+        const float* wr = w.ih1_w + (size_t)srow * R;
+        double bacc = (double)w.ih1_b[srow];
+        std::fill(fold_acc.begin(), fold_acc.end(), 0.0);
+        for (int k = 0; k < R; ++k) {
+          const double wk = (double)wr[k];
+          const float* irow = w.I_w + (size_t)k * ldI;
+          for (int col = 0; col < 1 + g.ldC; ++col) fold_acc[col] += wk * (double)irow[col];
+          bacc += wk * (double)w.I_b[k];
+        }
+        b[g.oA_x + 4 + drow] = (float)fold_acc[0];
+        for (int col = 0; col < g.ldC; ++col) b[g.oA_w + (size_t)(4 + drow) * g.ldC + col] = (float)fold_acc[1 + col];
+        b[g.oA_b + 4 + drow] = (float)bacc;
+        std::memcpy(b + g.ohh1 + (size_t)drow * R, w.hh1_w + (size_t)srow * R, sizeof(float) * R);
+        std::memcpy(b + g.oih2 + (size_t)drow * g.ldX, w.ih2_w + (size_t)srow * g.ldX, sizeof(float) * g.ldX);
+        std::memcpy(b + g.ohh2 + (size_t)drow * R, w.hh2_w + (size_t)srow * R, sizeof(float) * R);
+        b[g.obhh1 + drow] = w.hh1_b[srow];
+        b[g.obih2 + drow] = w.ih2_b[srow]; b[g.obhh2 + drow] = w.hh2_b[srow];
+      }
+    }
+    for (int r = 0; r < kCPC; ++r) {
+      const int row = cta * kCPC + r;
+      std::memcpy(b + g.ofc3 + (size_t)r * F, w.fc3_w + (size_t)row * F, sizeof(float) * F);
+      b[g.obfc3 + r] = w.fc3_b[row];
+    }
+  }
+  return hb;
 }
 
 }  // namespace b200tts

@@ -584,7 +584,7 @@ __global__ void __launch_bounds__(kPushThreads, 1) wavernn_push_kernel(PushModel
 }
 
 // ---- conditioning tables: tab[u][f][c][52] for f in [0, T]; frame T carries the bias only (zero conditioning) ------------
-// cw: per CTA [16][feat] mel rows | [36][aux] aux rows | [36] bias   (floats; packed by b200tts_wavernn_create, wavernn.cu)
+// cw: per CTA [16][feat] mel rows | [36][aux] aux rows | [36] bias   (floats; packed by pack_push_model below)
 struct PushCondW {
   const float* wm;      // [ncta][16][feat]
   const float* wa;      // [ncta][36][aux]
@@ -654,13 +654,74 @@ __global__ void push_cond_table_kernel(PushCondW W, const float* __restrict__ me
   }
 }
 
-// fills the exchange buffers with the sentinel pattern and clears the winner slots / error flag
+// fills the exchange buffers with the sentinel pattern and clears the winner slots and, if given, the error flag
 __global__ void push_init_kernel(uint32_t* __restrict__ vec, size_t nvec, unsigned long long* __restrict__ best, size_t nbest,
                                  int* __restrict__ error) {
   const size_t i0 = (size_t)blockIdx.x * blockDim.x + threadIdx.x, st = (size_t)gridDim.x * blockDim.x;
   for (size_t i = i0; i < nvec; i += st) vec[i] = kPushSentinel;
   for (size_t i = i0; i < nbest; i += st) best[i] = 0ull;
-  if (i0 == 0) *error = 0;
+  if (i0 == 0 && error) *error = 0;
+}
+
+// ---- host: the per-CTA blobs [ncta][blob] and the conditioning weights (PushCondW: [ncta][16][feat] mel rows | [ncta][36][aux]
+//      aux rows | [ncta][36] bias), cut from the grid kernel's blobs `gb` (pack_grid_model): the recurrent / feed-forward rows
+//      stay, the conditioned columns become the weights of the tables.  Fills the layout `pm`; pm.ok says whether the model can
+//      run this kernel with a [hop][NT] FIR table, and both vectors are empty when it cannot. ------------------------------------
+inline std::vector<float> pack_push_model(const GridModel& g, const std::vector<float>& gb, int hop, int NT, PushModel& pm,
+                                          std::vector<float>& condw) {
+  const int R = g.R, F = g.F, NC = g.NC, FEAT = g.FEAT, AUX = g.AUX;
+  pm = PushModel{};
+  pm.ncta = g.ncta; pm.R = R; pm.F = F; pm.NC = NC;
+  int off = 0;
+  auto take = [&](int n) { int o = off; off += (n + 3) & ~3; return o; };
+  // W_ih2 (12 rows) | fc1 (4 rows) | W_hh2 (12 rows) are contiguous: x1 is multiplied by the first 16 rows in one pass, h2 by the
+  // last 16 (fc1, then W_hh2) from one set of registers
+  pm.ohh1 = take(12 * R); pm.oih2 = take(12 * R); pm.ofc1 = take(4 * R); pm.ohh2 = take(12 * R);
+  pm.ofc2 = take(4 * F); pm.ofc3 = take(8 * F);
+  pm.oAx = take(16); pm.obhh1 = take(12); pm.obhh2 = take(12); pm.obfc3 = take(8);
+  pm.blob = off;
+  const size_t smem = ((size_t)pm.blob + (size_t)PushTraits<32>::scratch_floats(hop, NT)) * sizeof(float) + 1024;
+  pm.ok = (g.ok && R == 512 && F == 512 && g.ncta == 128 && NC <= 1024 && smem <= 227 * 1024) ? 1 : 0;
+  condw.clear();
+  if (!pm.ok) return {};
+
+  std::vector<float> pb((size_t)g.ncta * pm.blob, 0.f);
+  condw.assign((size_t)g.ncta * (16 * FEAT + 36 * AUX + 36), 0.f);
+  float* wm = condw.data();
+  float* wa = wm + (size_t)g.ncta * 16 * FEAT;
+  float* cb = wa + (size_t)g.ncta * 36 * AUX;
+  for (int cta = 0; cta < g.ncta; ++cta) {
+    const float* b = &gb[(size_t)cta * g.blob];
+    float* d = &pb[(size_t)cta * pm.blob];
+    for (int r = 0; r < 12; ++r) {
+      std::memcpy(d + pm.ohh1 + (size_t)r * R, b + g.ohh1 + (size_t)r * R, sizeof(float) * R);
+      std::memcpy(d + pm.oih2 + (size_t)r * R, b + g.oih2 + (size_t)r * g.ldX, sizeof(float) * R);
+      std::memcpy(d + pm.ohh2 + (size_t)r * R, b + g.ohh2 + (size_t)r * R, sizeof(float) * R);
+      d[pm.obhh1 + r] = b[g.obhh1 + r];
+      d[pm.obhh2 + r] = b[g.obhh2 + r];
+      std::memcpy(wa + ((size_t)cta * 36 + 16 + r) * AUX, b + g.oih2 + (size_t)r * g.ldX + R, sizeof(float) * AUX);
+      cb[(size_t)cta * 36 + 16 + r] = b[g.obih2 + r];
+    }
+    for (int j = 0; j < 4; ++j) {
+      std::memcpy(d + pm.ofc1 + (size_t)j * R, b + g.ofc1 + (size_t)j * g.ldX, sizeof(float) * R);
+      std::memcpy(d + pm.ofc2 + (size_t)j * F, b + g.ofc2 + (size_t)j * g.ldF, sizeof(float) * F);
+      std::memcpy(wa + ((size_t)cta * 36 + 28 + j) * AUX, b + g.ofc1 + (size_t)j * g.ldX + R, sizeof(float) * AUX);
+      std::memcpy(wa + ((size_t)cta * 36 + 32 + j) * AUX, b + g.ofc2 + (size_t)j * g.ldF + F, sizeof(float) * AUX);
+      cb[(size_t)cta * 36 + 28 + j] = b[g.obfc1 + j];
+      cb[(size_t)cta * 36 + 32 + j] = b[g.obfc2 + j];
+    }
+    for (int r = 0; r < 8; ++r) {
+      std::memcpy(d + pm.ofc3 + (size_t)r * F, b + g.ofc3 + (size_t)r * F, sizeof(float) * F);
+      d[pm.obfc3 + r] = b[g.obfc3 + r];
+    }
+    for (int r = 0; r < 16; ++r) {          // I rows 0-3, folded GRU-1 rows 4-15: [mel | a1] columns, x coefficient, bias
+      d[pm.oAx + r] = b[g.oA_x + r];
+      std::memcpy(wm + ((size_t)cta * 16 + r) * FEAT, b + g.oA_w + (size_t)r * g.ldC, sizeof(float) * FEAT);
+      std::memcpy(wa + ((size_t)cta * 36 + r) * AUX, b + g.oA_w + (size_t)r * g.ldC + FEAT, sizeof(float) * AUX);
+      cb[(size_t)cta * 36 + r] = b[g.oA_b + r];
+    }
+  }
+  return pb;
 }
 
 }  // namespace b200tts

@@ -40,6 +40,7 @@
 #pragma once
 #include <cuda_fp16.h>
 #include <utility>
+#include <vector>
 #include "common.cuh"
 #include "wavernn_push.cuh"
 
@@ -71,7 +72,7 @@ enum { TCN_C1 = 0, TCN_C2, TCN_F1, TCN_F2, TCN_W, TCN_COUNT = 8 };
 enum { TC_ROLE_G1 = 0, TC_ROLE_G2, TC_ROLE_F1, TC_ROLE_F2, TC_ROLE_F3 };
 
 struct TcArgs {
-  const uint8_t* wimg;           // [128][kTcWimgBytes] fp16 B-operand images (packed by b200tts_wavernn_create, wavernn.cu)
+  const uint8_t* wimg;           // [128][kTcWimgBytes] fp16 B-operand images (packed by pack_tc_images below)
   const float* prm;              // [128][128]
   uint8_t* vec;                  // [TV_COUNT][ng][2][kTcVecBytes]
   float* x1f;                    // [ng][2][128][512] fp32 copy of x1 (GRU-2 CTAs add their h2 to it: x2 = x1 + h2)
@@ -739,6 +740,76 @@ __global__ void __launch_bounds__(kTcThreads, 1) wavernn_tc_kernel(TcArgs A) {
     }
   }
   __syncthreads();
+}
+
+// ---- host: the per-CTA B-operand images [kTcCtas][kTcWimgBytes] and parameters [kTcCtas][kTcPrm], cut from the push kernel's
+//      blobs `pb` (pack_push_model).  Every weight is split into two fp16 planes (hi, lo' = (w - hi) * 2048) in the wgmma
+//      K-major no-swizzle layout [plane][k-step 32][k half 2][N/8][8 cols][8 halves].  False, with nothing packed, when the
+//      model or device cannot run this kernel: it needs the push kernel's model, 1024 classes, kTcCtas SMs and a FIR table of
+//      `fir_floats` that fits its shared-memory slot. ---------------------------------------------------------------------------
+inline bool pack_tc_images(const PushModel& pm, const std::vector<float>& pb, int sm_count, int fir_floats,
+                           std::vector<uint16_t>& img, std::vector<float>& prm) {
+  img.clear();
+  prm.clear();
+  if (!(pm.ok && pm.NC == 1024 && sm_count >= kTcCtas && (size_t)fir_floats * sizeof(float) <= (size_t)kTcFirMaxBytes))
+    return false;
+  const int R = pm.R, F = pm.F;
+  img.assign((size_t)kTcCtas * kTcWimgBytes / 2, 0);
+  prm.assign((size_t)kTcCtas * kTcPrm, 0.f);
+  auto put = [&](uint16_t* base, int N, int col, const float* wrow) {     // one weight row (K = 512) -> column `col` of an image
+    for (int k = 0; k < 512; ++k) {
+      const float w = wrow[k];
+      const __half hi = __float2half_rn(w);
+      const __half lo = __float2half_rn((w - __half2float(hi)) * 2048.0f);
+      const size_t off = ((size_t)(k >> 4) * 2 + ((k >> 3) & 1)) * ((size_t)N * 8) + (size_t)(col >> 3) * 64 + (size_t)(col & 7) * 8 + (k & 7);
+      base[off] = __half_as_ushort(hi);
+      base[(size_t)32 * N * 16 + off] = __half_as_ushort(lo);
+    }
+  };
+  auto unit_blob = [&](int unit) { return &pb[(size_t)(unit >> 2) * pm.blob]; };
+  for (int cta = 0; cta < kTcCtas; ++cta) {
+    uint16_t* wi = &img[(size_t)cta * kTcWimgBytes / 2];
+    float* pr = &prm[(size_t)cta * kTcPrm];
+    if (cta < 32) {                                   // GRU-1: 16 units, columns gate*16 + i
+      for (int i = 0; i < 16; ++i) {
+        const int unit = 16 * cta + i, j = unit & 3;
+        const float* b = unit_blob(unit);
+        for (int gate = 0; gate < 3; ++gate) {
+          put(wi, 48, gate * 16 + i, b + pm.ohh1 + (size_t)(gate * 4 + j) * R);
+          pr[64 + gate * 16 + i] = b[pm.obhh1 + gate * 4 + j];
+        }
+        for (int kind = 0; kind < 4; ++kind) pr[kind * 16 + i] = b[pm.oAx + kind * 4 + j];
+      }
+    } else if (cta < 96) {                            // GRU-2: 8 units, W_ih2 image then W_hh2 image, columns gate*8 + i (24-31 zero)
+      const int ci = cta - 32;
+      for (int i = 0; i < 8; ++i) {
+        const int unit = 8 * ci + i, j = unit & 3;
+        const float* b = unit_blob(unit);
+        for (int gate = 0; gate < 3; ++gate) {
+          put(wi, 32, gate * 8 + i, b + pm.oih2 + (size_t)(gate * 4 + j) * R);
+          put(wi + 32768, 32, gate * 8 + i, b + pm.ohh2 + (size_t)(gate * 4 + j) * R);
+          pr[gate * 8 + i] = b[pm.obhh2 + gate * 4 + j];
+        }
+      }
+    } else if (cta < 112) {                           // fc1 / fc2: 64 units
+      const bool first = cta < 104;
+      const int ci = first ? cta - 96 : cta - 104;
+      for (int i = 0; i < 64; ++i) {
+        const int unit = 64 * ci + i, j = unit & 3;
+        const float* b = unit_blob(unit);
+        put(wi, 64, i, b + (first ? pm.ofc1 : pm.ofc2) + (size_t)j * R);
+      }
+    } else {                                          // fc3: 64 classes
+      const int ci = cta - 112;
+      for (int i = 0; i < 64; ++i) {
+        const int cls = 64 * ci + i;
+        const float* b = &pb[(size_t)(cls >> 3) * pm.blob];
+        put(wi, 64, i, b + pm.ofc3 + (size_t)(cls & 7) * F);
+        pr[i] = b[pm.obfc3 + (cls & 7)];
+      }
+    }
+  }
+  return true;
 }
 
 }  // namespace b200tts
