@@ -186,7 +186,7 @@ typedef struct {
   int32_t lstm_units;       /* 256  decoder_lstm_units (checkpoint kernels are [768+256,1024] and [512,1024]) */
   int32_t enc_dim;          /* 512  2 * encoder_lstm_units                      */
   int32_t attn_dim;         /* 128  attention_dim                               */
-  int32_t attn_filters;     /* 32   attention_filters                           */
+  int32_t attn_filters;     /* 32   attention_filters (at most 32: location features of 512 tokens x 32 fill the decoder's buffer) */
   int32_t attn_kernel;      /* 31   attention_kernel                            */
   float zoneout;            /* 0.1  tacotron_zoneout_rate                       */
 } b200tts_taco_cfg;
@@ -238,8 +238,10 @@ int b200tts_taco_decode_gta(b200tts_taco* ctx, const float* d_memory, const int3
  * variables):
  *   b200tts_taco_encode   <- embedding lookup + EncoderConvolutions + EncoderRNN   tacotron.py:44-57, modules.py:145-217
  *   b200tts_taco_postnet  <- clip + Postnet + postnet_projection + residual + clip  tacotron.py:111-129, modules.py:345-376
- * d_ids [B][Tx_max] symbol ids (tacotron/utils/text.py:18-31), d_memory [B][Tx_max][enc_dim];
- * d_frames [B][max_steps][num_mels] raw decoder outputs, d_nsteps [B], d_mel [B][max_steps][num_mels] (rows >= nsteps untouched). */
+ * d_ids [B][Tx_max] symbol ids (tacotron/utils/text.py:18-31; each id below its sentence's length must be < the vocabulary size),
+ * d_lengths [B], d_memory [B][Tx_max][enc_dim] (rows >= length are zero);
+ * d_frames [B][max_steps][num_mels] raw decoder outputs, d_nsteps [B], d_mel [B][max_steps][num_mels] (rows >= nsteps untouched).
+ * Like the decoders, both clamp each length to [0, Tx_max] / [0, max_steps]: a length <= 0 is an empty sentence. */
 int b200tts_taco_encode(b200tts_taco* ctx, const int32_t* d_ids, const int32_t* d_lengths, int B, int Tx_max, float* d_memory,
                         void* stream);
 int b200tts_taco_postnet(b200tts_taco* ctx, const float* d_frames, const int32_t* d_nsteps, int B, int max_steps, float* d_mel,

@@ -31,9 +31,10 @@ struct ConvArgs {
   float lo, hi;
 };
 
+// Rows t >= lengths[b] are neither read nor written; a length outside [0, Tmax] is clamped to it, as the decoders do.
 __global__ void taco_conv_bn_kernel(ConvArgs A) {
   extern __shared__ float xs[];                      // [(kConvTile + k - 1)][Cin]
-  const int b = blockIdx.y, t0 = blockIdx.x * kConvTile, len = A.lengths[b];
+  const int b = blockIdx.y, t0 = blockIdx.x * kConvTile, len = min(max(A.lengths[b], 0), A.Tmax);
   if (t0 >= len) return;
   const int half = (A.k - 1) / 2, rows = kConvTile + A.k - 1;
   for (int e = threadIdx.x; e < rows * A.Cin; e += blockDim.x) {
@@ -71,6 +72,7 @@ __global__ void taco_conv_bn_kernel(ConvArgs A) {
 }
 
 // One CTA per (sentence, direction): zoneout LSTM over the sentence, output = un-zoned new_h  -> memory[b][t][dir*U ..]
+// The sentence length is clamped to [0, Tmax] (a sentence of length 0 gives all-zero rows).
 __global__ void __launch_bounds__(kTacoThreads, 1) taco_bilstm_kernel(const float* __restrict__ x /*[B][Tmax][Cin]*/,
                                                                        const int* __restrict__ lengths, int Tmax, int Cin, int U,
                                                                        const float* __restrict__ Kfw, const float* __restrict__ bfw,
@@ -81,7 +83,7 @@ __global__ void __launch_bounds__(kTacoThreads, 1) taco_bilstm_kernel(const floa
   float* z = in + Cin + U;      // [4U]
   float* c = z + 4 * U;         // [U]
   float* part = c + U;          // [>= 4 * 4U]
-  const int b = blockIdx.x, dir = blockIdx.y, len = lengths[b], tid = threadIdx.x;
+  const int b = blockIdx.x, dir = blockIdx.y, len = min(max(lengths[b], 0), Tmax), tid = threadIdx.x;
   const float* K = dir ? Kbw : Kfw;
   const float* bias = dir ? bbw : bfw;
   for (int i = tid; i < U; i += kTacoThreads) { in[Cin + i] = 0.f; c[i] = 0.f; }

@@ -38,6 +38,17 @@ struct b200tts_taco {
   int sm_count = 0;
 };
 
+// Split-K partials of taco_decoder_kernel, in floats.  The matvecs and the context sum need at most 4096 of them; the attention
+// step keeps the location features f[Tx][NF] there, so b200tts_taco_create accepts only configs with kTacoMaxTx * NF <= this.
+constexpr int kTacoPartFloats = 16384;
+
+// dynamic shared memory of taco_decoder_kernel (its carve-up, plus the split-K partials)
+static size_t taco_decoder_smem_bytes(const TacoWeights& w) {
+  const size_t fl = 128 + w.P + (w.P + w.E + w.U) + 2 * w.U + 4 * w.U + 2 * w.U + (w.U + w.E) + w.A + 3 * kTacoMaxTx + 96 + 64 +
+                    (size_t)w.KW * w.NF + (size_t)w.NF * w.A + kTacoPartFloats;
+  return fl * sizeof(float);
+}
+
 extern "C" int b200tts_taco_create(b200tts_taco** out, int device, const b200tts_taco_cfg* cfg, const b200tts_tensor* weights,
                                    int n_weights) {
   API_BEGIN
@@ -48,6 +59,8 @@ extern "C" int b200tts_taco_create(b200tts_taco** out, int device, const b200tts
   REQUIRE(M % 4 == 0 && P % 4 == 0 && U % 4 == 0 && E % 4 == 0 && AD % 4 == 0, B200TTS_EINVAL, "dims must be multiples of 4");
   REQUIRE(M <= 96 && P == 256 && 4 * U == 1024 && E <= 1024 && AD <= 256 && KW % 2 == 1 && KW * NF <= 992 && NF * AD <= 4096,
           B200TTS_EINVAL, "decoder dims outside what taco_decoder_kernel is laid out for");
+  REQUIRE(kTacoMaxTx * NF <= kTacoPartFloats, B200TTS_EINVAL,
+          "attn_filters: the location features of a 512-token sentence must fit taco_decoder_kernel's partial buffer (NF <= 32)");
   check_device(device);
   DeviceGuard dg(device);
   TensorMap tm;
@@ -239,13 +252,6 @@ extern "C" void b200tts_taco_destroy(b200tts_taco* ctx) {
   if (!ctx) return;
   DeviceGuard dg(ctx->device, true);
   delete ctx;
-}
-
-// dynamic shared memory of taco_decoder_kernel (its carve-up, plus 16 K floats of split-K partials)
-static size_t taco_decoder_smem_bytes(const TacoWeights& w) {
-  const size_t fl = 128 + w.P + (w.P + w.E + w.U) + 2 * w.U + 4 * w.U + 2 * w.U + (w.U + w.E) + w.A + 3 * kTacoMaxTx + 96 + 64 +
-                    (size_t)w.KW * w.NF + (size_t)w.NF * w.A + 16384;
-  return fl * sizeof(float);
 }
 
 static int taco_decode_impl(b200tts_taco* ctx, const float* d_memory, const int32_t* d_lengths, int B, int Tx_max,

@@ -36,6 +36,8 @@ class TacoDecoderEngine:
         _lib.check(self.lib.b200tts_taco_create(C.byref(h), self.device, C.byref(c), arr, len(arr)))
         del keep
         self._h = h
+        emb = host.get('inputs_embedding')
+        self.vocab = int(emb.shape[0]) if emb is not None and emb.ndim == 2 else None
 
     def close(self):
         if getattr(self, '_h', None):
@@ -164,13 +166,21 @@ class TacoDecoderEngine:
                                np.asarray(st['cum'], np.float32), pad, np.asarray(st['alpha'], np.float32), pad])
 
     def encode(self, ids, lengths=None):
-        """ids int [B, Tx] (padded with anything beyond lengths) -> memory [B, Tx, enc_dim] (CUDA tensor)."""
+        """ids int [B, Tx] (padded with anything beyond lengths) -> memory [B, Tx, enc_dim] (CUDA tensor); lengths [B] in
+        [1, Tx] or None (= Tx).  Every id below its sentence's length must be in [0, vocab): checked before anything launches."""
         dev = self._dev()
-        i = torch.as_tensor(ids).to(device=dev, dtype=torch.int32).contiguous()
+        i = torch.as_tensor(ids).to(dtype=torch.int32)
         if i.dim() != 2:
             raise ValueError('ids must be [B, Tx]')
         B, Tx = i.shape
         ln = torch.full((B,), Tx, dtype=torch.int32) if lengths is None else torch.as_tensor(lengths, dtype=torch.int32)
+        if tuple(ln.shape) != (B,) or B < 1 or int(ln.max()) > Tx or int(ln.min()) < 1:
+            raise ValueError('lengths must be [B] in [1, Tx]')
+        if self.vocab is not None:                 # (without the encoder variables the library refuses the call itself)
+            valid = torch.arange(Tx, device=i.device)[None, :] < ln.to(i.device)[:, None]
+            if bool(((i < 0) | (i >= self.vocab))[valid].any()):
+                raise ValueError(f'ids below lengths must be in [0, {self.vocab})')
+        i = i.to(dev).contiguous()
         ln = ln.to(dev)
         with torch.cuda.device(self.device):
             mem = torch.zeros(B, Tx, self.cfg['enc_dim'], device=dev, dtype=torch.float32)
@@ -179,11 +189,16 @@ class TacoDecoderEngine:
         return mem
 
     def postnet(self, frames, nsteps):
-        """frames [B, max_steps, num_mels] raw decoder outputs + nsteps [B] -> mel [B, max_steps, num_mels] (clipped)."""
+        """frames [B, max_steps, num_mels] raw decoder outputs + nsteps [B] (<= max_steps; <= 0, e.g. the -1 of a failed decode,
+        is an empty row) -> mel [B, max_steps, num_mels] (clipped; rows at or beyond nsteps are zero)."""
         dev = self._dev()
         f = torch.as_tensor(frames).to(device=dev, dtype=torch.float32).contiguous()
-        n = torch.as_tensor(nsteps).to(device=dev, dtype=torch.int32).contiguous()
+        if f.dim() != 3 or f.shape[2] != self.cfg['num_mels']:
+            raise ValueError(f'frames must be [B, max_steps, {self.cfg["num_mels"]}]')
         B, ms, _ = f.shape
+        n = torch.as_tensor(nsteps).to(device=dev, dtype=torch.int32).contiguous()
+        if tuple(n.shape) != (B,) or B < 1 or int(n.max()) > ms:
+            raise ValueError('nsteps must be [B] with values <= max_steps')
         with torch.cuda.device(self.device):
             mel = torch.zeros_like(f)
             _lib.check(self.lib.b200tts_taco_postnet(self._h, _ptr(f), _ptr(n), B, ms, _ptr(mel), self._stream()))

@@ -274,3 +274,12 @@ def test_taco_error_codes_without_a_device():
     assert lib.b200tts_taco_decode(None, None, None, 1, 5, None, 10, 0, None, None, None, None, None) == -1
     assert lib.b200tts_taco_encode(None, None, None, 1, 5, None, None) == -1
     assert lib.b200tts_taco_postnet(None, None, None, 1, 10, None, None) == -1
+    # 64 location filters pass the per-step layout rules (15 x 64 taps <= 992, 64 x 64 <= 4096), but the location features of a
+    # 512-token sentence (512 x 64 floats) do not fit taco_decoder_kernel's 16384-float partial buffer: refused before any device call
+    from taco_common import synth_taco_weights
+    arr, keep = L.make_tensor_array(synth_taco_weights(7))
+    cfg = L.TacoCfg(num_mels=80, prenet_units=256, lstm_units=256, enc_dim=512, attn_dim=64, attn_filters=64, attn_kernel=15,
+                    zoneout=0.1)
+    assert lib.b200tts_taco_create(ctypes.byref(h), 0, ctypes.byref(cfg), arr, len(arr)) == -1 and not h.value
+    assert b'attn_filters' in lib.b200tts_last_error()
+    del keep
