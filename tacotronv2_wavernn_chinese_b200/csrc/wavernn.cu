@@ -2,6 +2,7 @@
 // choice of generation kernel.
 #include <cooperative_groups.h>
 #include <algorithm>
+#include <climits>
 #include <cmath>
 #include <cstdio>
 #include <cstdlib>
@@ -396,17 +397,21 @@ static void launch_utt(b200tts_wavernn* ctx, const GenArgs& a, cudaStream_t st) 
 }
 
 struct FoldGeom {           // fold_with_overlap geometry (fatchord_version.py:319-330)
-  int nfold, L, stride, total_len;
+  int nfold, L, stride;
 };
-static FoldGeom fold_geometry(int S, int target, int overlap) {
+// The geometry of an S-sample utterance, or a refusal.  The fold length target + 2 * overlap must fit an int: it is the step
+// count of every fold.
+static FoldGeom fold_geometry(long long S, int target, int overlap) {
+  REQUIRE(target >= 1 && overlap >= 2, B200TTS_EINVAL, "fold target/overlap out of range (target >= 1, overlap >= 2)");
+  REQUIRE(S > overlap, B200TTS_EINVAL, "utterance shorter than the fold overlap");
+  REQUIRE(S <= INT_MAX && (long long)target + 2LL * overlap <= INT_MAX, B200TTS_EINVAL,
+          "utterance or fold longer than 2^31 - 1 samples");
   FoldGeom g{};
   g.stride = target + overlap;
   g.L = target + 2 * overlap;
-  int num_folds = (S - overlap) / g.stride;
-  int extended = num_folds * g.stride + overlap;
-  if (S - extended != 0) num_folds += 1;
-  g.nfold = num_folds;
-  g.total_len = num_folds * g.stride + overlap;
+  const long long num_folds = (S - overlap) / g.stride;
+  const long long extended = num_folds * g.stride + overlap;
+  g.nfold = (int)(num_folds + (S - extended != 0 ? 1 : 0));
   return g;
 }
 
@@ -677,13 +682,12 @@ static void run_generate_rows(b200tts_wavernn* ctx, const float* d_mel, int B, i
     REQUIRE(wave_len >= fade_len, B200TTS_EINVAL,
             "T must be >= 21 frames: the reference's 20-hop fade-out (fatchord_version.py:256-258) fails below that");
   }
+  REQUIRE(o.fold_target >= 0, B200TTS_EINVAL, "fold target/overlap out of range (fold_target 0 turns folding off)");
   const bool folding = o.fold_target > 0;
   FoldGeom fg{};
   if (folding) {
     REQUIRE(B == 1, B200TTS_EINVAL, "fold-with-overlap generation takes exactly one utterance (the reference folds x[0] only)");
-    REQUIRE(o.fold_overlap >= 2 && o.fold_target >= 1, B200TTS_EINVAL, "fold target/overlap out of range");
     REQUIRE(steps == S, B200TTS_EINVAL, "max_steps is not supported together with folding");
-    REQUIRE(S > o.fold_overlap, B200TTS_EINVAL, "utterance shorter than the fold overlap");
     REQUIRE(!r.d_utterance_ids, B200TTS_EINVAL, "d_utterance_ids cannot be combined with fold-with-overlap generation");
     fg = fold_geometry(S, o.fold_target, o.fold_overlap);
     REQUIRE(fg.nfold >= 1 && fg.nfold <= 65535, B200TTS_EINVAL, "fold count out of range");
@@ -787,9 +791,8 @@ static void run_generate(b200tts_wavernn* ctx, const float* d_mel, int B, int T,
 
 extern "C" int b200tts_wavernn_fold_geometry(int T, int hop, int target, int overlap, int* n_folds, int* fold_len) {
   API_BEGIN
-  REQUIRE(T >= 1 && hop >= 1 && target >= 1 && overlap >= 2 && n_folds && fold_len, B200TTS_EINVAL, "bad argument");
-  REQUIRE(T * hop > overlap, B200TTS_EINVAL, "utterance shorter than the fold overlap");
-  FoldGeom g = fold_geometry(T * hop, target, overlap);
+  REQUIRE(T >= 1 && hop >= 1 && n_folds && fold_len, B200TTS_EINVAL, "bad argument");
+  FoldGeom g = fold_geometry((long long)T * hop, target, overlap);
   *n_folds = g.nfold;
   *fold_len = g.L;
   API_END

@@ -73,7 +73,9 @@ def test_upsample_vs_reference_golden(torch_cuda, name):
     assert np.array_equal(aux, np.repeat(aux[:, ::275], 275, axis=1))
 
 
-@pytest.mark.parametrize('B,T', [(1, 21), (3, 37), (2, 5)])
+# T on both sides of melresnet_kernel's 8-frame tile, and the long mel_fir_kernel grids of the fold tests' utterances
+@pytest.mark.parametrize('B,T', [(1, 21), (3, 37), (2, 5), (1, 1), (4, 7), (2, 8), (3, 9), (4, 16), (1, 17), (2, 255), (4, 256),
+                                 (3, 257)])
 def test_upsample_vs_oracle_shapes(torch_cuda, B, T):
     eng, p = engine_for('synth5')
     mels = synth.synth_mels(77 + T, B, T)
