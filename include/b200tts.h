@@ -12,6 +12,8 @@
  *   b200tts_wavernn_generate   <- WaveRNN.generate (unbatched branch)   wavernn/models/fatchord_version.py:169-264
  *                                 incl. decode_mu_law                   wavernn/utils/dsp.py:98-103
  *   b200tts_wavernn_generate_host  same, HOST buffers in/out (what wavernn_gen.py:41 sees end to end)
+ *   b200tts_wavernn_create_mol / _generate_mol  the same with voc_mode = 'MOL' (wavernn_hparams.py:35): fc3 gives a mixture
+ *                                 of 10 logistics, sampled by sample_from_discretized_mix_logistic  wavernn/utils/distribution.py:87-123
  *   gen_opts.fold_target/_overlap  <- fold_with_overlap + xfade_and_unfold  fatchord_version.py:293-405 (--batched)
  *   b200tts_griffin_lim        <- audio.inv_mel_spectrogram (Griffin-Lim) tacotron/datasets/audio.py:122-137, :176-210
  *   b200tts_resample           <- audio.load_wav at another rate (librosa 0.7.2 core.resample, resampy kaiser_best) :14-15
@@ -77,7 +79,8 @@ typedef struct {
  * argmax_i(logit_i - log q_i). */
 enum {
   B200TTS_RNG_PHILOX = 0,          /* q from Philox4x32-10 keyed by (seed, global utterance, step, class) */
-  B200TTS_RNG_EXT_EXPONENTIAL = 1  /* q read from d_q[S][B][n_classes] (tests: noise shared with the oracle) */
+  B200TTS_RNG_EXT_EXPONENTIAL = 1, /* q read from d_q[S][B][n_classes] (tests: noise shared with the oracle) */
+  B200TTS_RNG_EXT_UNIFORM = 2      /* MOL only: the 11 uniforms of each step read from d_q[S][B][11] (see _generate_mol) */
 };
 typedef struct {
   int32_t mode;
@@ -141,6 +144,30 @@ int b200tts_wavernn_upsample(b200tts_wavernn* ctx, const float* d_mel, int B, in
 int b200tts_wavernn_generate(b200tts_wavernn* ctx, const float* d_mel, int B, int T, const b200tts_rng* rng,
                              const b200tts_gen_opts* opts, int16_t* d_labels, double* d_wave, void* stream);
 
+/* Mixture-of-logistics models (voc_mode = 'MOL').  create_mol takes the same cfg and weights as create, except that cfg.bits
+ * is ignored and fc3 must be [30][fc_dims] (B200TTS_ESHAPE otherwise).  A MOL context is refused by _generate and
+ * _generate_host, and a RAW context by _generate_mol.
+ *
+ * generate_mol: per row and step, with p = fc3 output (p[0..9] mixture logits, p[10..19] means, p[20..29] log-scales) and
+ * uniforms u[0..10] in [1e-5, 1 - 1e-5], all in fp32 as the reference computes it:
+ *     k = argmax_j (p[j] - log(-log(u[j])))          (first maximum)
+ *     x = clamp(p[10+k] + exp(max(p[20+k], log(1e-14))) * (log(u[10]) - log(1 - u[10])), -1, 1)
+ * x is the sample and the next step's input.  Noise: PHILOX draws u from Philox4x32-10 keyed by (seed, global utterance, step,
+ * j = 0..2) (b200tts_philox_mol_uniform dumps it), EXT_UNIFORM reads d_q[S][B][11].
+ *   d_samples   [B][S] float32 (may be NULL), [n_folds][fold_len] when folding
+ *   d_teacher_x optional [B][S] (or folded): fed back instead of the sample
+ *   d_wave      [B][(T-1)*hop] float64 of the samples (no mu-law: the reference turns it off for MOL), truncated and faded like
+ *               RAW; the cross-faded wave when folding
+ * opts: mu_law is ignored, d_teacher must be NULL, d_logits is [S][B][30], packed rows and kernel = TC are refused.  Kernels as
+ * for RAW without the tensor cores: AUTO / GRID take the push kernel up to 32 rows and the wide grid above, UTTERANCE the
+ * utterance kernel.  max_steps, fold_target/_overlap, d_utt_frames and d_utterance_ids work as for
+ * RAW. */
+int b200tts_wavernn_create_mol(b200tts_wavernn** out, int device, const b200tts_wavernn_cfg* cfg,
+                               const b200tts_tensor* weights, int n_weights);
+int b200tts_wavernn_generate_mol(b200tts_wavernn* ctx, const float* d_mel, int B, int T, const b200tts_rng* rng,
+                                 const b200tts_gen_opts* opts, const float* d_teacher_x, float* d_samples, double* d_wave,
+                                 void* stream);
+
 /* n_folds and fold_len = target + 2*overlap of fold_with_overlap (fatchord_version.py:319-330) for a T-frame utterance. */
 int b200tts_wavernn_fold_geometry(int T, int hop, int target, int overlap, int* n_folds, int* fold_len);
 
@@ -152,6 +179,10 @@ int b200tts_wavernn_generate_host(b200tts_wavernn* ctx, const float* h_mel, int 
  * Lets a test hand the production noise stream to the oracle. */
 int b200tts_philox_exponential(int device, uint64_t seed, uint64_t utterance_offset, int B, int step0, int n_steps,
                                int n_classes, float* d_q, void* stream);
+
+/* The uniforms the PHILOX mode of b200tts_wavernn_generate_mol draws for (utterance, step): d_u[n_steps][B][11]. */
+int b200tts_philox_mol_uniform(int device, uint64_t seed, uint64_t utterance_offset, int B, int step0, int n_steps, float* d_u,
+                               void* stream);
 
 /* Number of kernel launches the library has issued on this context since creation (bench.py: gpu_launches). */
 int64_t b200tts_wavernn_launch_count(const b200tts_wavernn* ctx);

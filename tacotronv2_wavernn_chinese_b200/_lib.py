@@ -14,7 +14,7 @@ import numpy as np
 from .build import LIB
 
 OK = 0
-RNG_PHILOX, RNG_EXT_EXPONENTIAL = 0, 1
+RNG_PHILOX, RNG_EXT_EXPONENTIAL, RNG_EXT_UNIFORM = 0, 1, 2
 KERNEL_AUTO, KERNEL_UTTERANCE, KERNEL_GRID, KERNEL_TC = 0, 1, 2, 3
 KERNELS = {'auto': KERNEL_AUTO, 'utterance': KERNEL_UTTERANCE, 'grid': KERNEL_GRID, 'tc': KERNEL_TC}
 
@@ -90,6 +90,10 @@ SIGNATURES = {
                                            C.c_void_p]),
     'b200tts_wavernn_generate': (C.c_int, [C.c_void_p, C.c_void_p, C.c_int, C.c_int, C.POINTER(Rng), C.POINTER(GenOpts),
                                            C.c_void_p, C.c_void_p, C.c_void_p]),
+    'b200tts_wavernn_create_mol': (C.c_int, [C.POINTER(C.c_void_p), C.c_int, C.POINTER(WaveRNNCfg), C.POINTER(Tensor), C.c_int]),
+    'b200tts_wavernn_generate_mol': (C.c_int, [C.c_void_p, C.c_void_p, C.c_int, C.c_int, C.POINTER(Rng), C.POINTER(GenOpts),
+                                               C.c_void_p, C.c_void_p, C.c_void_p, C.c_void_p]),
+    'b200tts_philox_mol_uniform': (C.c_int, [C.c_int, C.c_uint64, C.c_uint64, C.c_int, C.c_int, C.c_int, C.c_void_p, C.c_void_p]),
     'b200tts_wavernn_fold_geometry': (C.c_int, [C.c_int, C.c_int, C.c_int, C.c_int, C.POINTER(C.c_int), C.POINTER(C.c_int)]),
     'b200tts_wavernn_generate_host': (C.c_int, [C.c_void_p, C.c_void_p, C.c_int, C.c_int, C.POINTER(Rng),
                                                 C.POINTER(GenOpts), C.c_void_p, C.c_void_p]),

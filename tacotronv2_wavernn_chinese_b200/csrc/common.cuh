@@ -61,6 +61,56 @@ __device__ __forceinline__ void philox_exp4(uint64_t seed, uint64_t utt, uint32_
 }
 
 // ---------------------------------------------------------------------------------------------
+// Mixture-of-logistics sampling (voc_mode = 'MOL'): sample_from_discretized_mix_logistic, reference
+// wavernn/utils/distribution.py:87-123, for one row.  fc3 gives p[0..29]: 10 mixture logits, 10 means, 10 log-scales.
+// ---------------------------------------------------------------------------------------------
+constexpr int kMolMix = 10, kMolParams = 3 * kMolMix, kMolU = kMolMix + 1;
+constexpr float kMolLogScaleMin = -32.23619079589844f;   // float(np.log(1e-14)) rounded to fp32, as torch.clamp takes it
+
+// uint32 -> uniform(1e-5, 1 - 1e-5) (the range of the reference's uniform_ calls): 24 random bits, exact in fp32
+__device__ __forceinline__ float mol_uniform_from_bits(uint32_t x) {
+  return __fmaf_rn((float)(x >> 8) * (1.0f / 16777216.0f), 1.0f - 2e-5f, 1e-5f);
+}
+
+// The 11 uniforms of one (utterance, step): counter (step, j, utt_lo, utt_hi), j = 0..2, gives 12 words; u[0..9] choose the
+// mixture, u[10] drives the logistic, the 12th word is unused.  b200tts_philox_mol_uniform dumps the same stream.
+__device__ __forceinline__ void philox_mol_u(uint64_t seed, uint64_t utt, uint32_t step, float (&u)[kMolU]) {
+#pragma unroll
+  for (int j = 0; j < 3; ++j) {
+    uint32_t c[4] = {step, (uint32_t)j, (uint32_t)utt, (uint32_t)(utt >> 32)};
+    philox4x32_10(c, seed);
+#pragma unroll
+    for (int i = 0; i < 4; ++i)
+      if (4 * j + i < kMolU) u[4 * j + i] = mol_uniform_from_bits(c[i]);
+  }
+}
+
+// The sample x in [-1, 1] for parameters p and uniforms u, each operation rounded as torch rounds it on fp32 tensors (no
+// contraction into FMAs, IEEE logf / expf):
+//   k = argmax_j (p[j] - log(-log(u[j])))   (first maximum, like torch .max)
+//   x = clamp(p[10+k] + exp(max(p[20+k], log(1e-14))) * (log(u[10]) - log(1 - u[10])), -1, 1)
+__device__ __forceinline__ float mol_sample(const float* p, const float (&u)[kMolU]) {
+  int k = 0;
+  float best = __fsub_rn(p[0], logf(-logf(u[0])));
+#pragma unroll
+  for (int j = 1; j < kMolMix; ++j) {
+    const float v = __fsub_rn(p[j], logf(-logf(u[j])));
+    if (v > best) { best = v; k = j; }
+  }
+  const float ls = fmaxf(p[2 * kMolMix + k], kMolLogScaleMin);
+  const float l = __fsub_rn(logf(u[kMolMix]), logf(__fsub_rn(1.0f, u[kMolMix])));
+  const float x = __fadd_rn(p[kMolMix + k], __fmul_rn(expf(ls), l));
+  return fminf(fmaxf(x, -1.0f), 1.0f);
+}
+
+// The MOL outputs of a step kernel: the sample of each step is a float, not a label.
+struct MolIO {
+  const float* teacher_x;     // [B][S] or null: fed back instead of the sample
+  float* samples;             // [B][S]
+  float* par;                 // wide grid only: [2][Bp][32] fc3 outputs of the last two steps, by step parity
+};
+
+// ---------------------------------------------------------------------------------------------
 // argmax packing: (ordered float bits << 32) | (0xFFFFFFFF - index)  -> max() picks the largest key and,
 // among equal keys, the SMALLEST index (torch.argmax returns the first maximum).
 // ---------------------------------------------------------------------------------------------

@@ -1,5 +1,5 @@
-// libb200tts.so -- WaveRNN vocoder (wavernn_*.cuh): b200tts_wavernn_*, b200tts_philox_exponential, weight packing and the
-// choice of generation kernel.
+// libb200tts.so -- WaveRNN vocoder (wavernn_*.cuh): b200tts_wavernn_*, b200tts_philox_exponential / _mol_uniform, weight
+// packing and the choice of generation kernel.
 #include <cooperative_groups.h>
 #include <algorithm>
 #include <climits>
@@ -19,13 +19,14 @@ using namespace b200tts;
 struct b200tts_wavernn {
   int device = 0;
   b200tts_wavernn_cfg cfg{};
-  int NC = 0, NT = 0, sm_count = 0;
+  bool mol = false;               // voc_mode = 'MOL' (b200tts_wavernn_create_mol): fc3 gives 30 mixture parameters
+  int NC = 0, NT = 0, sm_count = 0;   // NC: fc3 rows as packed (MOL: the 30 parameters padded to 32)
   DeviceBuf weights;          // original layouts, one blob (pack_original)
   StepWeights sw{};
   ResnetParams rp{};
   const float* d_fir = nullptr;   // [hop][NT]
   GridModel gm{};                 // per-CTA weight blobs of the grid kernel
-  DeviceBuf grid_blob, mels_T, aux_T, grid_sync, fold_mels, fold_aux;
+  DeviceBuf grid_blob, mels_T, aux_T, grid_sync, fold_mels, fold_aux, grid_mol_par;
   PushModel pm{};                 // small-batch push kernel (wavernn_push.cuh): per-CTA blobs + conditioning-projection weights
   PushCondW pcw{};
   DeviceBuf push_blob, push_condw, push_tab, push_vec, push_best;
@@ -124,7 +125,18 @@ static StepWeights pack_original(b200tts_wavernn* ctx, const TensorMap& tm, Pack
   size_t o_bih2 = copy("rnn2.bias_ih_l0", {3 * R}), o_bhh2 = copy("rnn2.bias_hh_l0", {3 * R});
   size_t o_fc1 = copy("fc1.weight", {F, R + AUX}), o_fc1b = copy("fc1.bias", {F});
   size_t o_fc2 = copy("fc2.weight", {F, F + AUX}), o_fc2b = copy("fc2.bias", {F});
-  size_t o_fc3 = copy("fc3.weight", {NC, F}), o_fc3b = copy("fc3.bias", {NC});
+  size_t o_fc3, o_fc3b;
+  if (ctx->mol) {               // 30 rows padded with zero rows to NC = 32: the step kernels dot whole quads of rows
+    const float* w = need(tm, "fc3.weight", {kMolParams, F})->data;
+    const float* b = need(tm, "fc3.bias", {kMolParams})->data;
+    o_fc3 = pk.add((size_t)NC * F);
+    o_fc3b = pk.add((size_t)NC);
+    std::memcpy(&pk.h[o_fc3], w, sizeof(float) * kMolParams * F);
+    std::memcpy(&pk.h[o_fc3b], b, sizeof(float) * kMolParams);
+  } else {
+    o_fc3 = copy("fc3.weight", {NC, F});
+    o_fc3b = copy("fc3.bias", {NC});
+  }
 
   // ---- MelResNet, transposed to [in][out]; BatchNorm (eval, eps 1e-5) folded to scale/shift in double ----
   const float* cin = need(tm, "upsample.resnet.conv_in.weight", {C, FEAT, K})->data;
@@ -206,8 +218,8 @@ static void upload(DeviceBuf& d, const V& h) {
   B200_CUDA(cudaMemcpy(d.p, h.data(), h.size() * sizeof(h[0]), cudaMemcpyHostToDevice));
 }
 
-extern "C" int b200tts_wavernn_create(b200tts_wavernn** out, int device, const b200tts_wavernn_cfg* cfg,
-                                      const b200tts_tensor* weights, int n_weights) {
+static int create_context(b200tts_wavernn** out, int device, const b200tts_wavernn_cfg* cfg, const b200tts_tensor* weights,
+                          int n_weights, bool mol) {
   API_BEGIN
   REQUIRE(out && cfg && weights && n_weights > 0, B200TTS_EINVAL, "null argument");
   *out = nullptr;
@@ -221,7 +233,7 @@ extern "C" int b200tts_wavernn_create(b200tts_wavernn** out, int device, const b
   REQUIRE(prod == c.hop_length, B200TTS_EINVAL, "prod(upsample_factors) != hop_length (wavernn_train.py:67 asserts the same)");
   REQUIRE(c.res_out_dims % 4 == 0, B200TTS_EINVAL, "res_out_dims must be divisible by 4");
   REQUIRE(c.rnn_dims % 128 == 0 && c.fc_dims % 128 == 0, B200TTS_EINVAL, "rnn_dims / fc_dims must be multiples of 128");
-  REQUIRE(c.bits >= 2 && c.bits <= 15, B200TTS_EINVAL, "bits must be 2..15 (labels are int16)");
+  REQUIRE(mol || (c.bits >= 2 && c.bits <= 15), B200TTS_EINVAL, "bits must be 2..15 (labels are int16)");
   REQUIRE(c.compute_dims <= 1024 && c.res_out_dims <= 1024, B200TTS_EINVAL, "compute/res_out dims too large");
   const int AUX = c.res_out_dims / 4, FEAT = c.feat_dims;
   REQUIRE(AUX % 4 == 0, B200TTS_EINVAL, "aux dims (res_out_dims/4) must be a multiple of 4");
@@ -235,7 +247,8 @@ extern "C" int b200tts_wavernn_create(b200tts_wavernn** out, int device, const b
   std::unique_ptr<b200tts_wavernn> ctx(new b200tts_wavernn());
   ctx->device = device;
   ctx->cfg = c;
-  ctx->NC = 1 << c.bits;
+  ctx->mol = mol;
+  ctx->NC = mol ? round4(kMolParams) : 1 << c.bits;
   int coop = 0;
   B200_CUDA(cudaDeviceGetAttribute(&ctx->sm_count, cudaDevAttrMultiProcessorCount, device));
   B200_CUDA(cudaDeviceGetAttribute(&coop, cudaDevAttrCooperativeLaunch, device));
@@ -243,23 +256,39 @@ extern "C" int b200tts_wavernn_create(b200tts_wavernn** out, int device, const b
   // Each kernel's weights are cut from the host blobs of the one before it (grid -> push -> tensor cores), so each capability
   // implies the previous one.
   Packer pk;
-  const StepWeights hw = pack_original(ctx.get(), tm, pk);
-  const std::vector<float> gb = pack_grid_model(hw, ctx->sm_count, coop != 0, ctx->gm);
-  upload(ctx->grid_blob, gb);
-  std::vector<float> cw;
-  const std::vector<float> pb = pack_push_model(ctx->gm, gb, c.hop_length, ctx->NT, ctx->pm, cw);
-  upload(ctx->push_blob, pb);
-  upload(ctx->push_condw, cw);
-  if (ctx->pm.ok) {
-    const int n = ctx->pm.ncta;
-    const float* cwd = ctx->push_condw.as<float>();
-    ctx->pcw = PushCondW{cwd, cwd + (size_t)n * 16 * FEAT, cwd + (size_t)n * (16 * FEAT + 36 * AUX), n, FEAT, AUX};
+  StepWeights hw = pack_original(ctx.get(), tm, pk);
+  std::vector<float> mol_w3, mol_b3;
+  if (mol) {                    // the grid and push kernels take fc3 as 2R classes, 8 per CTA: parameter j becomes class 8j
+    mol_w3.assign((size_t)2 * c.rnn_dims * c.fc_dims, 0.f);
+    mol_b3.assign((size_t)2 * c.rnn_dims, 0.f);
+    for (int j = 0; j < kMolParams; ++j) {
+      std::memcpy(&mol_w3[(size_t)kCPC * j * c.fc_dims], hw.fc3_w + (size_t)j * c.fc_dims, sizeof(float) * c.fc_dims);
+      mol_b3[(size_t)kCPC * j] = hw.fc3_b[j];
+    }
+    hw.fc3_w = mol_w3.data();
+    hw.fc3_b = mol_b3.data();
+    hw.NC = 2 * c.rnn_dims;
   }
-  std::vector<uint16_t> img;
-  std::vector<float> prm;
-  ctx->tc_ok = pack_tc_images(ctx->pm, pb, ctx->sm_count, c.hop_length * ctx->NT, img, prm);
-  upload(ctx->tc_wimg, img);
-  upload(ctx->tc_prm, prm);
+  {
+    const std::vector<float> gb = pack_grid_model(hw, ctx->sm_count, coop != 0, ctx->gm);
+    upload(ctx->grid_blob, gb);
+    std::vector<float> cw;
+    const std::vector<float> pb = pack_push_model(ctx->gm, gb, c.hop_length, ctx->NT, ctx->pm, cw);
+    upload(ctx->push_blob, pb);
+    upload(ctx->push_condw, cw);
+    if (ctx->pm.ok) {
+      const int n = ctx->pm.ncta;
+      const float* cwd = ctx->push_condw.as<float>();
+      ctx->pcw = PushCondW{cwd, cwd + (size_t)n * 16 * FEAT, cwd + (size_t)n * (16 * FEAT + 36 * AUX), n, FEAT, AUX};
+    }
+    if (!mol) {                 // MOL models do not run on the tensor cores (choose_kernel)
+      std::vector<uint16_t> img;
+      std::vector<float> prm;
+      ctx->tc_ok = pack_tc_images(ctx->pm, pb, ctx->sm_count, c.hop_length * ctx->NT, img, prm);
+      upload(ctx->tc_wimg, img);
+      upload(ctx->tc_prm, prm);
+    }
+  }
 
   ctx->error.ensure(sizeof(int));
   B200_CUDA(cudaMemset(ctx->error.p, 0, sizeof(int)));
@@ -267,6 +296,16 @@ extern "C" int b200tts_wavernn_create(b200tts_wavernn** out, int device, const b
   B200_CUDA(cudaEventCreate(&ctx->ev1));
   *out = ctx.release();
   API_END
+}
+
+extern "C" int b200tts_wavernn_create(b200tts_wavernn** out, int device, const b200tts_wavernn_cfg* cfg,
+                                      const b200tts_tensor* weights, int n_weights) {
+  return create_context(out, device, cfg, weights, n_weights, false);
+}
+
+extern "C" int b200tts_wavernn_create_mol(b200tts_wavernn** out, int device, const b200tts_wavernn_cfg* cfg,
+                                          const b200tts_tensor* weights, int n_weights) {
+  return create_context(out, device, cfg, weights, n_weights, true);
 }
 
 extern "C" void b200tts_wavernn_destroy(b200tts_wavernn* ctx) {
@@ -382,15 +421,21 @@ static void coop_launch(b200tts_wavernn* ctx, const void* kern, const char* what
 }
 
 template <int G>
-static void launch_utt(b200tts_wavernn* ctx, const GenArgs& a, cudaStream_t st) {
+static void launch_utt(b200tts_wavernn* ctx, const GenArgs& a, const MolIO* mol, cudaStream_t st) {
   const StepWeights& w = ctx->sw;
   size_t fl = (size_t)G * (w.ldI + w.R + 4 * w.R + 2 * (w.R + w.aux) + (w.F + w.aux) + w.F + w.NC);
   size_t smem = fl * sizeof(float);
   REQUIRE(smem <= 227 * 1024, B200TTS_EINVAL, "model too large for the utterance kernel's shared memory");
-  B200_CUDA(cudaFuncSetAttribute(wavernn_utt_kernel<G>, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)smem));
   int grid = (a.B + G - 1) / G;
-  B200_CUDA(cudaEventRecord(ctx->ev0, st));
-  wavernn_utt_kernel<G><<<grid, kUttThreads, smem, st>>>(w, a);
+  if (mol) {
+    B200_CUDA(cudaFuncSetAttribute(wavernn_utt_mol_kernel<G>, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)smem));
+    B200_CUDA(cudaEventRecord(ctx->ev0, st));
+    wavernn_utt_mol_kernel<G><<<grid, kUttThreads, smem, st>>>(w, a, *mol);
+  } else {
+    B200_CUDA(cudaFuncSetAttribute(wavernn_utt_kernel<G>, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)smem));
+    B200_CUDA(cudaEventRecord(ctx->ev0, st));
+    wavernn_utt_kernel<G><<<grid, kUttThreads, smem, st>>>(w, a);
+  }
   B200_CUDA(cudaGetLastError());
   ctx->launches++;
   B200_CUDA(cudaEventRecord(ctx->ev1, st));
@@ -417,7 +462,8 @@ static FoldGeom fold_geometry(long long S, int target, int overlap) {
 
 // `fold` != null: `a` describes the folded problem (B = nfold, S = T = L, hop = 1); the conditioning of the single source utterance
 // of S0 samples, in ctx->mels_up [S0][feat] / ctx->aux_frames [T0][O], is cut into the per-fold rows this kernel reads first.
-static void launch_utterance(b200tts_wavernn* ctx, GenArgs a, cudaStream_t st, const FoldGeom* fold, int S0) {
+// `mol` != null: a MOL context's generation, with its sample buffers.
+static void launch_utterance(b200tts_wavernn* ctx, GenArgs a, const MolIO* mol, cudaStream_t st, const FoldGeom* fold, int S0) {
   const b200tts_wavernn_cfg& c = ctx->cfg;
   if (fold) {
     const int O = c.res_out_dims;
@@ -434,19 +480,23 @@ static void launch_utterance(b200tts_wavernn* ctx, GenArgs a, cudaStream_t st, c
   }
   // utterances per CTA: enough CTAs to cover the SMs first, then amortise the L2 weight stream over more rows
   int per = (a.B + ctx->sm_count - 1) / ctx->sm_count;
-  if (per <= 1) launch_utt<1>(ctx, a, st);
-  else if (per <= 2) launch_utt<2>(ctx, a, st);
-  else if (per <= 4) launch_utt<4>(ctx, a, st);
-  else launch_utt<8>(ctx, a, st);
+  if (per <= 1) launch_utt<1>(ctx, a, mol, st);
+  else if (per <= 2) launch_utt<2>(ctx, a, mol, st);
+  else if (per <= 4) launch_utt<4>(ctx, a, mol, st);
+  else launch_utt<8>(ctx, a, mol, st);
 }
 
 template <int U, int UW, int GROUPS>
-static void launch_grid_t(b200tts_wavernn* ctx, GridArgs& a, cudaStream_t st) {
+static void launch_grid_t(b200tts_wavernn* ctx, GridArgs& a, const MolIO* mol, cudaStream_t st) {
   using MT = MapTraits<U, UW, GROUPS>;
   GridModel gm = ctx->gm;
   size_t smem = ((size_t)gm.blob + (size_t)MT::kScratchFloats) * sizeof(float);
-  void* args[] = {(void*)&gm, (void*)&a};
-  coop_launch(ctx, (const void*)wavernn_grid_kernel<U, UW, GROUPS>, "grid kernel", gm.ncta, MT::NW * 32, smem, args, st);
+  MolIO io = mol ? *mol : MolIO{};
+  void* args[] = {(void*)&gm, (void*)&a, (void*)&io};
+  if (mol)
+    coop_launch(ctx, (const void*)wavernn_grid_mol_kernel<U, UW, GROUPS>, "grid kernel", gm.ncta, MT::NW * 32, smem, args, st);
+  else
+    coop_launch(ctx, (const void*)wavernn_grid_kernel<U, UW, GROUPS>, "grid kernel", gm.ncta, MT::NW * 32, smem, args, st);
 }
 
 // Mapping for B utterances: returns the padded batch; variant = index into the dispatch table below.
@@ -463,7 +513,7 @@ static int grid_variant(int B, int* variant) {
 
 // `fold` != null: `ua` already describes the folded problem (B = nfold, S = T = L, hop = 1) and the conditioning of the
 // single source utterance is in ctx->mels_up [S0][feat] / ctx->aux_frames [T0][O].
-static void launch_grid(b200tts_wavernn* ctx, const float* d_mel, const GenArgs& ua, bool prof, cudaStream_t st,
+static void launch_grid(b200tts_wavernn* ctx, const float* d_mel, const GenArgs& ua, const MolIO* mol, bool prof, cudaStream_t st,
                         const FoldGeom* fold, int S0) {
   const b200tts_wavernn_cfg& c = ctx->cfg;
   const GridModel& g = ctx->gm;
@@ -513,12 +563,19 @@ static void launch_grid(b200tts_wavernn* ctx, const float* d_mel, const GenArgs&
   a.B = B; a.Bp = Bp; a.S = S; a.T = T; a.hop = ua.hop; a.steps = ua.steps;
   copy_gen_fields(a, ua);
   a.prof = phase_counters(ctx, prof, g.ncta, st);
+  MolIO io{};
+  if (mol) {                    // the fc3 outputs of the last two steps, [2][Bp][32]
+    io = *mol;
+    ctx->grid_mol_par.ensure((size_t)2 * Bp * 32 * sizeof(float));
+    io.par = ctx->grid_mol_par.as<float>();
+  }
+  const MolIO* iop = mol ? &io : nullptr;
   switch (variant) {
-    case GV_N4: launch_grid_t<0, 4, 1>(ctx, a, st); break;
-    case GV_W1: launch_grid_t<1, 1, 1>(ctx, a, st); break;
-    case GV_W2: launch_grid_t<2, 1, 1>(ctx, a, st); break;
-    case GV_W4: launch_grid_t<4, 1, 1>(ctx, a, st); break;
-    case GV_W4x2: launch_grid_t<4, 1, 2>(ctx, a, st); break;
+    case GV_N4: launch_grid_t<0, 4, 1>(ctx, a, iop, st); break;
+    case GV_W1: launch_grid_t<1, 1, 1>(ctx, a, iop, st); break;
+    case GV_W2: launch_grid_t<2, 1, 1>(ctx, a, iop, st); break;
+    case GV_W4: launch_grid_t<4, 1, 1>(ctx, a, iop, st); break;
+    case GV_W4x2: launch_grid_t<4, 1, 2>(ctx, a, iop, st); break;
     default: REQUIRE(false, B200TTS_EINVAL, "internal: unknown grid variant");
   }
 }
@@ -540,11 +597,13 @@ static const float* launch_cond_table(b200tts_wavernn* ctx, const float* d_mel, 
 
 // ---- small-batch push kernel (wavernn_push.cuh) --------------------------------------------------------------------------
 template <int G>
-static void launch_push_t(b200tts_wavernn* ctx, PushArgs& a, cudaStream_t st) {
+static void launch_push_t(b200tts_wavernn* ctx, PushArgs& a, const MolIO* mol, cudaStream_t st) {
   PushModel pm = ctx->pm;
   size_t smem = ((size_t)pm.blob + (size_t)PushTraits<G>::scratch_floats(a.hop, a.NT)) * sizeof(float);
-  void* args[] = {(void*)&pm, (void*)&a};
-  coop_launch(ctx, (const void*)wavernn_push_kernel<G>, "push kernel", pm.ncta, kPushThreads, smem, args, st);
+  MolIO io = mol ? *mol : MolIO{};
+  void* args[] = {(void*)&pm, (void*)&a, (void*)&io};
+  if (mol) coop_launch(ctx, (const void*)wavernn_push_mol_kernel<G>, "push kernel", pm.ncta, kPushThreads, smem, args, st);
+  else coop_launch(ctx, (const void*)wavernn_push_kernel<G>, "push kernel", pm.ncta, kPushThreads, smem, args, st);
 }
 
 // rows of the push kernel variant: up to 8 rows run the 8-row variant (on the previous GPU a 4-row variant was slower, its
@@ -558,7 +617,7 @@ struct PackInfo {            // gen_opts.d_pack_*: kernel rows run queues of utt
   const int* start;
   int rows, segs, steps, n_utt;
 };
-static void launch_push(b200tts_wavernn* ctx, const float* d_mel, const GenArgs& ua, bool prof, cudaStream_t st,
+static void launch_push(b200tts_wavernn* ctx, const float* d_mel, const GenArgs& ua, const MolIO* mol, bool prof, cudaStream_t st,
                         const FoldGeom* fold, int T0, const PackInfo* pack) {
   const PushModel& pm = ctx->pm;
   const int rows = pack ? pack->rows : ua.B;
@@ -585,9 +644,9 @@ static void launch_push(b200tts_wavernn* ctx, const float* d_mel, const GenArgs&
   copy_gen_fields(a, ua);
   a.prof = phase_counters(ctx, prof, pm.ncta, st);
   switch (G) {
-    case 8: launch_push_t<8>(ctx, a, st); break;
-    case 16: launch_push_t<16>(ctx, a, st); break;
-    default: launch_push_t<32>(ctx, a, st); break;
+    case 8: launch_push_t<8>(ctx, a, mol, st); break;
+    case 16: launch_push_t<16>(ctx, a, mol, st); break;
+    default: launch_push_t<32>(ctx, a, mol, st); break;
   }
 }
 
@@ -636,6 +695,9 @@ constexpr int kTcMinRows = 129;
 // create time, so a refused call has launched nothing.
 static StepKernel choose_kernel(b200tts_wavernn* ctx, int rows, const b200tts_gen_opts& o) {
   const bool packing = o.d_pack_utt != nullptr;
+  if (ctx->mol)                 // never on the tensor cores: MOL takes the push kernel up to 32 rows and the wide grid above
+    REQUIRE(o.kernel != B200TTS_KERNEL_TC, B200TTS_EINVAL,
+            "kernel=tc is RAW only: a MOL model runs on kernel=auto (push / wide grid), grid or utterance");
   // tc_ok implies pm.ok implies gm.ok (pack_tc_images, pack_push_model)
   const bool tc = ctx->tc_ok && o.fold_target == 0 && !packing && rows <= kTcRows * kTcMaxGroups;
   const bool push = ctx->pm.ok && (packing ? o.pack_rows : rows) <= kPushMaxRows;
@@ -667,12 +729,22 @@ static StepKernel choose_kernel(b200tts_wavernn* ctx, int rows, const b200tts_ge
   return SK_GRID;
 }
 
+// RAW contexts write labels to d_labels; MOL contexts write float samples to d_samples and take d_teacher_x.
 static void run_generate_rows(b200tts_wavernn* ctx, const float* d_mel, int B, int T, const b200tts_rng& r,
-                              const b200tts_gen_opts& o, bool prof, int16_t* d_labels, double* d_wave, cudaStream_t st) {
+                              const b200tts_gen_opts& o, bool prof, int16_t* d_labels, double* d_wave, float* d_samples,
+                              const float* d_teacher_x, cudaStream_t st) {
   const b200tts_wavernn_cfg& c = ctx->cfg;
   const int hop = c.hop_length, S = T * hop, O = c.res_out_dims;
-  REQUIRE(r.mode == B200TTS_RNG_PHILOX || r.mode == B200TTS_RNG_EXT_EXPONENTIAL, B200TTS_EINVAL, "unknown rng mode");
-  REQUIRE(r.mode != B200TTS_RNG_EXT_EXPONENTIAL || r.d_q, B200TTS_EINVAL, "EXT_EXPONENTIAL needs d_q");
+  if (ctx->mol) {
+    REQUIRE(r.mode == B200TTS_RNG_PHILOX || r.mode == B200TTS_RNG_EXT_UNIFORM, B200TTS_EINVAL,
+            "MOL generation takes PHILOX or EXT_UNIFORM noise");
+    REQUIRE(r.mode != B200TTS_RNG_EXT_UNIFORM || r.d_q, B200TTS_EINVAL, "EXT_UNIFORM needs d_q");
+    REQUIRE(!o.d_teacher, B200TTS_EINVAL, "MOL generation is teacher-forced through d_teacher_x (float samples), not d_teacher");
+    REQUIRE(!o.d_pack_utt, B200TTS_EINVAL, "packed rows are not built for MOL models: generate the utterances in plain batches");
+  } else {
+    REQUIRE(r.mode == B200TTS_RNG_PHILOX || r.mode == B200TTS_RNG_EXT_EXPONENTIAL, B200TTS_EINVAL, "unknown rng mode");
+    REQUIRE(r.mode != B200TTS_RNG_EXT_EXPONENTIAL || r.d_q, B200TTS_EINVAL, "EXT_EXPONENTIAL needs d_q");
+  }
   REQUIRE(o.max_steps >= 0 && o.max_steps <= S, B200TTS_EINVAL, "max_steps out of range");
   const int steps = o.max_steps ? o.max_steps : S;
   const int fade_len = 20 * hop;                      // fatchord_version.py:256
@@ -706,7 +778,12 @@ static void run_generate_rows(b200tts_wavernn* ctx, const float* d_mel, int B, i
   ctx->prof_ncta = 0;
   ctx->aux_frames.ensure((size_t)B * T * O * sizeof(float));
   int16_t* labels = d_labels;
-  if (!labels) {
+  float* samples = d_samples;
+  if (ctx->mol && !samples) {
+    ctx->labels.ensure((size_t)GB * GS * sizeof(float));
+    samples = ctx->labels.as<float>();
+  }
+  if (!ctx->mol && !labels) {
     ctx->labels.ensure((size_t)GB * GS * sizeof(int16_t));
     labels = ctx->labels.as<int16_t>();
   }
@@ -727,14 +804,25 @@ static void run_generate_rows(b200tts_wavernn* ctx, const float* d_mel, int B, i
 
   const FoldGeom* fold = folding ? &fg : nullptr;
   const PackInfo pi{o.d_pack_utt, o.d_pack_start, o.pack_rows, o.pack_segs, o.pack_steps, B};
+  const MolIO mol{d_teacher_x, samples};
   switch (kernel) {
-    case SK_UTTERANCE: launch_utterance(ctx, a, st, fold, S); break;
-    case SK_GRID: launch_grid(ctx, d_mel, a, prof, st, fold, S); break;
-    case SK_PUSH: launch_push(ctx, d_mel, a, prof, st, fold, T, packing ? &pi : nullptr); break;
+    case SK_UTTERANCE: launch_utterance(ctx, a, ctx->mol ? &mol : nullptr, st, fold, S); break;
+    case SK_GRID: launch_grid(ctx, d_mel, a, ctx->mol ? &mol : nullptr, prof, st, fold, S); break;
+    case SK_PUSH: launch_push(ctx, d_mel, a, ctx->mol ? &mol : nullptr, prof, st, fold, T, packing ? &pi : nullptr); break;
     case SK_TC: launch_tc(ctx, d_mel, a, prof, st); break;
   }
   ctx->ev_valid = true;
-  if (d_wave) {
+  if (d_wave && ctx->mol) {
+    if (folding) {
+      xfade_unfold_mol_kernel<<<(wave_len + 255) / 256, 256, 0, st>>>(samples, fg.nfold, fg.L, o.fold_target, o.fold_overlap,
+                                                                      wave_len, fade_len, ctx->error.as<int>(), d_wave);
+    } else {
+      dim3 grid((wave_len + 255) / 256, B);
+      finish_wave_mol_kernel<<<grid, 256, 0, st>>>(samples, S, wave_len, fade_len, o.d_utt_frames, hop, ctx->error.as<int>(), d_wave);
+    }
+    B200_CUDA(cudaGetLastError());
+    ctx->launches++;
+  } else if (d_wave) {
     if (folding) {
       xfade_unfold_kernel<<<(wave_len + 255) / 256, 256, 0, st>>>(labels, fg.nfold, fg.L, o.fold_target, o.fold_overlap, wave_len,
                                                                   fade_len, ctx->NC, o.mu_law, ctx->error.as<int>(), d_wave);
@@ -753,7 +841,8 @@ static void run_generate_rows(b200tts_wavernn* ctx, const float* d_mel, int B, i
 // under a budget (default 8 GB, env B200TTS_MAX_COND_BYTES); the noise is keyed by the global row, so the result is unchanged.
 // (Not for the debug modes whose buffers are indexed [step][row]: external noise, logits.)
 static void run_generate(b200tts_wavernn* ctx, const float* d_mel, int B, int T, const b200tts_rng* rng,
-                         const b200tts_gen_opts* opts, int16_t* d_labels, double* d_wave, cudaStream_t st) {
+                         const b200tts_gen_opts* opts, int16_t* d_labels, double* d_wave, float* d_samples,
+                         const float* d_teacher_x, cudaStream_t st) {
   b200tts_rng r{};
   if (rng) r = *rng;
   b200tts_gen_opts o{};
@@ -764,13 +853,14 @@ static void run_generate(b200tts_wavernn* ctx, const float* d_mel, int B, int T,
   const double budget = getenv("B200TTS_MAX_COND_BYTES") ? atof(getenv("B200TTS_MAX_COND_BYTES")) : 8e9;   // read per call
   const b200tts_wavernn_cfg& c = ctx->cfg;
   const double per_row = (double)T * c.hop_length * c.feat_dims * sizeof(float);
-  const bool whole = r.mode == B200TTS_RNG_EXT_EXPONENTIAL || o.d_logits || o.fold_target > 0 || o.d_pack_utt || !d_labels;
+  const bool whole = r.mode == B200TTS_RNG_EXT_EXPONENTIAL || r.mode == B200TTS_RNG_EXT_UNIFORM || o.d_logits || o.fold_target > 0 ||
+                     o.d_pack_utt || !(d_labels || d_samples);
   // kernel=auto and more than 256 rows: launches of 256 rows through the tensor-core pipeline (66 us per lock-step each on an H100)
   // beat the wide mapping on the whole batch (91 us per 256 rows); the noise is keyed by the global row, so the result does not change
   constexpr int kTcSlice = kTcRows * kTcMaxGroups;
   const bool tc_slices = !whole && B > kTcSlice && o.kernel == B200TTS_KERNEL_AUTO && choose_kernel(ctx, kTcSlice, o) == SK_TC;
   if (whole || (!tc_slices && per_row * ((B + 255) / 256 * 256) <= budget)) {
-    run_generate_rows(ctx, d_mel, B, T, r, o, prof, d_labels, d_wave, st);
+    run_generate_rows(ctx, d_mel, B, T, r, o, prof, d_labels, d_wave, d_samples, d_teacher_x, st);
     return;
   }
   int rows = tc_slices ? kTcSlice : (int)(budget / per_row);
@@ -784,8 +874,9 @@ static void run_generate(b200tts_wavernn* ctx, const float* d_mel, int B, int T,
     b200tts_gen_opts os = o;
     if (os.d_teacher) os.d_teacher += (size_t)r0 * S;
     if (os.d_utt_frames) os.d_utt_frames += r0;
-    run_generate_rows(ctx, d_mel + (size_t)r0 * c.feat_dims * T, nb, T, rs, os, prof, d_labels + (size_t)r0 * S,
-                      d_wave ? d_wave + (size_t)r0 * wave_len : nullptr, st);
+    run_generate_rows(ctx, d_mel + (size_t)r0 * c.feat_dims * T, nb, T, rs, os, prof, d_labels ? d_labels + (size_t)r0 * S : nullptr,
+                      d_wave ? d_wave + (size_t)r0 * wave_len : nullptr, d_samples ? d_samples + (size_t)r0 * S : nullptr,
+                      d_teacher_x ? d_teacher_x + (size_t)r0 * S : nullptr, st);
   }
 }
 
@@ -803,8 +894,21 @@ extern "C" int b200tts_wavernn_generate(b200tts_wavernn* ctx, const float* d_mel
   API_BEGIN
   REQUIRE(ctx && d_mel, B200TTS_EINVAL, "null argument");
   REQUIRE(B >= 1 && T >= 1 && B <= 65535, B200TTS_EINVAL, "B must be 1..65535 and T positive");
+  REQUIRE(!ctx->mol, B200TTS_EINVAL, "this context holds a MOL model: generate with b200tts_wavernn_generate_mol");
   DeviceGuard dg(ctx->device);
-  run_generate(ctx, d_mel, B, T, rng, opts, d_labels, d_wave, (cudaStream_t)stream);
+  run_generate(ctx, d_mel, B, T, rng, opts, d_labels, d_wave, nullptr, nullptr, (cudaStream_t)stream);
+  API_END
+}
+
+extern "C" int b200tts_wavernn_generate_mol(b200tts_wavernn* ctx, const float* d_mel, int B, int T, const b200tts_rng* rng,
+                                            const b200tts_gen_opts* opts, const float* d_teacher_x, float* d_samples,
+                                            double* d_wave, void* stream) {
+  API_BEGIN
+  REQUIRE(ctx && d_mel, B200TTS_EINVAL, "null argument");
+  REQUIRE(B >= 1 && T >= 1 && B <= 65535, B200TTS_EINVAL, "B must be 1..65535 and T positive");
+  REQUIRE(ctx->mol, B200TTS_EINVAL, "this context holds a RAW model: generate with b200tts_wavernn_generate");
+  DeviceGuard dg(ctx->device);
+  run_generate(ctx, d_mel, B, T, rng, opts, nullptr, d_wave, d_samples, d_teacher_x, (cudaStream_t)stream);
   API_END
 }
 
@@ -813,6 +917,7 @@ extern "C" int b200tts_wavernn_generate_host(b200tts_wavernn* ctx, const float* 
   API_BEGIN
   REQUIRE(ctx && h_mel, B200TTS_EINVAL, "null argument");
   REQUIRE(B >= 1 && T >= 1 && B <= 65535, B200TTS_EINVAL, "B must be 1..65535 and T positive");
+  REQUIRE(!ctx->mol, B200TTS_EINVAL, "the host entry point is RAW only: generate a MOL model with b200tts_wavernn_generate_mol");
   REQUIRE(!opts || (!opts->d_teacher && !opts->d_logits), B200TTS_EINVAL, "device-side debug buffers need the device entry point");
   REQUIRE(!rng || rng->mode == B200TTS_RNG_PHILOX, B200TTS_EINVAL, "the host entry point only takes the PHILOX mode");
   REQUIRE(!opts || opts->fold_target == 0 || !h_labels, B200TTS_EINVAL, "folded generation returns only the wave through the host entry point");
@@ -832,7 +937,7 @@ extern "C" int b200tts_wavernn_generate_host(b200tts_wavernn* ctx, const float* 
     ctx->wave.ensure(wav_bytes);
     d_wave = ctx->wave.as<double>();
   }
-  run_generate(ctx, ctx->mel_in.as<float>(), B, T, rng, opts, ctx->labels.as<int16_t>(), d_wave, st);
+  run_generate(ctx, ctx->mel_in.as<float>(), B, T, rng, opts, ctx->labels.as<int16_t>(), d_wave, nullptr, nullptr, st);
   if (h_labels) {
     B200_CUDA(cudaMemcpyAsync(ctx->h_stage.p, ctx->labels.p, lab_bytes, cudaMemcpyDeviceToHost, st));
     B200_CUDA(cudaStreamSynchronize(st));
@@ -912,6 +1017,30 @@ extern "C" int b200tts_philox_exponential(int device, uint64_t seed, uint64_t ut
   size_t total = (size_t)n_steps * B * (n_classes / 4);
   unsigned grid = (unsigned)std::min<size_t>((total + 255) / 256, 132 * 16);
   philox_dump_kernel<<<grid, 256, 0, (cudaStream_t)stream>>>(seed, utterance_offset, B, step0, n_steps, n_classes, d_q);
+  B200_CUDA(cudaGetLastError());
+  API_END
+}
+
+__global__ void philox_mol_dump_kernel(unsigned long long seed, unsigned long long utt0, int B, int step0, int n_steps,
+                                       float* __restrict__ u) {
+  const size_t total = (size_t)n_steps * B;
+  for (size_t e = (size_t)blockIdx.x * blockDim.x + threadIdx.x; e < total; e += (size_t)gridDim.x * blockDim.x) {
+    const int b = (int)(e % B), s = (int)(e / B);
+    float v[kMolU];
+    philox_mol_u(seed, utt0 + (unsigned long long)b, (uint32_t)(step0 + s), v);
+#pragma unroll
+    for (int j = 0; j < kMolU; ++j) u[e * kMolU + j] = v[j];
+  }
+}
+
+extern "C" int b200tts_philox_mol_uniform(int device, uint64_t seed, uint64_t utterance_offset, int B, int step0, int n_steps,
+                                          float* d_u, void* stream) {
+  API_BEGIN
+  REQUIRE(d_u && B >= 1 && n_steps >= 1 && step0 >= 0, B200TTS_EINVAL, "bad argument");
+  DeviceGuard dg(device);
+  const size_t total = (size_t)n_steps * B;
+  unsigned grid = (unsigned)std::min<size_t>((total + 255) / 256, 132 * 16);
+  philox_mol_dump_kernel<<<grid, 256, 0, (cudaStream_t)stream>>>(seed, utterance_offset, B, step0, n_steps, d_u);
   B200_CUDA(cudaGetLastError());
   API_END
 }

@@ -244,4 +244,55 @@ __global__ void finish_wave_kernel(const int16_t* __restrict__ labels /*[B][S]*/
   }
 }
 
+// The same two epilogues for MOL samples: float samples in, no decode (generate() forces mu_law off for MOL, :174).
+__global__ void xfade_unfold_mol_kernel(const float* __restrict__ samples /*[nfold][L]*/, int nfold, int L, int target, int overlap,
+                                        int wave_len, int fade_len, const int* __restrict__ gen_error,
+                                        double* __restrict__ wave /*[wave_len]*/) {
+  const bool poisoned = gen_error && *gen_error;
+  const int stride = target + overlap;
+  const int silence = overlap / 2, flen = overlap - silence;
+  const double lin_step = -1.0 / (double)(fade_len - 1);
+  for (int n = blockIdx.x * blockDim.x + threadIdx.x; n < wave_len; n += gridDim.x * blockDim.x) {
+    double acc = 0.0;
+    int u_hi = n / stride;
+    if (u_hi >= nfold) u_hi = nfold - 1;
+    for (int u = u_hi; u >= 0 && u >= u_hi - 1; --u) {
+      const int t = n - u * stride;
+      if (t < 0 || t >= L) continue;
+      double y = (double)samples[(size_t)u * L + t];
+      if (t < overlap) {
+        double g = 0.0;
+        if (t >= silence) { const int k = t - silence; const double tt = xfade_t(k, flen); g = sqrt(0.5 * (1.0 + tt)); }
+        y *= g;
+      }
+      if (t >= L - overlap) {
+        const int k2 = t - (L - overlap);
+        double g = 1.0;
+        if (k2 >= silence) { const int k = k2 - silence; const double tt = xfade_t(k, flen); g = sqrt(0.5 * (1.0 - tt)); }
+        y *= g;
+      }
+      acc += y;
+    }
+    const int k = n - (wave_len - fade_len);
+    if (k >= 0) acc *= (k == fade_len - 1) ? 0.0 : (1.0 + (double)k * lin_step);
+    wave[n] = poisoned ? nan("") : acc;
+  }
+}
+
+__global__ void finish_wave_mol_kernel(const float* __restrict__ samples /*[B][S]*/, int S, int wave_len_max, int fade_len,
+                                       const int* __restrict__ utt_frames, int hop, const int* __restrict__ gen_error,
+                                       double* __restrict__ wave /*[B][wave_len_max]*/) {
+  const int b = blockIdx.y;
+  const bool poisoned = gen_error && *gen_error;
+  const double step = -1.0 / (double)(fade_len - 1);
+  const int wave_len = utt_frames ? min(wave_len_max, max(0, (utt_frames[b] - 1) * hop)) : wave_len_max;
+  for (int i = blockIdx.x * blockDim.x + threadIdx.x; i < wave_len_max; i += gridDim.x * blockDim.x) {
+    if (i >= wave_len) { wave[(size_t)b * wave_len_max + i] = 0.0; continue; }
+    double y = (double)samples[(size_t)b * S + i];
+    int k = i - (wave_len - fade_len);
+    if (k >= 0) y *= (k == fade_len - 1) ? 0.0 : (1.0 + (double)k * step);
+    wave[(size_t)b * wave_len_max + i] = poisoned ? nan("") : y;
+  }
+}
+
 }  // namespace b200tts

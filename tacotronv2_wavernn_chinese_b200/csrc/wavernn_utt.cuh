@@ -4,7 +4,7 @@
 // Replaces the hot loop of WaveRNN.generate, reference wavernn/models/fatchord_version.py:201-237:
 //   I (:208-209) -> GRUCell rnn1 (:210) -> +res (:212) -> GRUCell rnn2 (:213-214) -> +res (:216)
 //   -> relu fc1 (:217-218) -> relu fc2 (:220-221) -> fc3 (:223) -> softmax + Categorical.sample (:232-235)
-//   -> x = 2*label/1023 - 1 (:235-237).
+//   -> x = 2*label/1023 - 1 (:235-237); or, for MOL models, sample_from_discretized_mix_logistic (:225-229).
 // This kernel keeps the reference's operation structure one to one (no algebraic folding), takes the debug
 // options (teacher forcing, logits dump) and serves as the on-device cross-check of the grid kernel.
 #pragma once
@@ -40,7 +40,7 @@ struct GenArgs {
   int rng_mode;
   unsigned long long seed, utt_offset;
   const unsigned long long* utt_ids;   // optional [B]: global utterance index of every row (overrides utt_offset + row)
-  const float* q;             // [S][B][NC] (EXT_EXPONENTIAL)
+  const float* q;             // [S][B][NC] (EXT_EXPONENTIAL); [S][B][11] uniforms (EXT_UNIFORM, MOL)
   const int16_t* teacher;     // [B][S] or null
   float* logits_out;          // [S][B][NC] or null
   int16_t* labels;            // [B][S]
@@ -79,8 +79,9 @@ __device__ __forceinline__ void warp_rows_dot(const float* __restrict__ W, int l
     for (int g = 0; g < G; ++g) out[r][g] = warp_sum(acc[r][g]);
 }
 
-template <int G>
-__global__ void __launch_bounds__(kUttThreads, 1) wavernn_utt_kernel(StepWeights W, GenArgs A) {
+// The whole loop; MOL selects the sampler (fc3 then has NC = 32 rows, the 30 parameters padded to whole quads).
+template <int G, bool MOL>
+__device__ __forceinline__ void utt_run(StepWeights W, GenArgs A, MolIO M) {
   extern __shared__ __align__(16) float sm[];
   const int R = W.R, F = W.F, AUX = W.aux, NC = W.NC, ldI = W.ldI;
   const int KX = R + AUX;                       // 544
@@ -220,45 +221,65 @@ __global__ void __launch_bounds__(kUttThreads, 1) wavernn_utt_kernel(StepWeights
       }
     }
     __syncthreads();
-    // ---- sample: argmax_c (logit_c - log q_c), q ~ Exp(1)  == Categorical(softmax(logits)).sample() ----
+    if constexpr (MOL) {
+      // ---- sample_from_discretized_mix_logistic, one thread per row (distribution.py:87-123, fatchord_version.py:225-229) ----
+      if (tid < G && b0 + tid < A.B) {
+        const int g = tid, b = b0 + g;
+        float u[kMolU];
+        if (A.rng_mode == 0) {
+          philox_mol_u(A.seed, A.utt_ids ? A.utt_ids[b] : A.utt_offset + (unsigned long long)b, (uint32_t)i, u);
+        } else {
 #pragma unroll
-    for (int g = 0; g < G; ++g) {
-      const int b = b0 + g;
-      unsigned long long best = 0ull;
-      if (b < A.B) {
-        for (int c4 = tid; c4 < NC / 4; c4 += kUttThreads) {
-          float q[4];
-          if (A.rng_mode == 0) {
-            philox_exp4(A.seed, A.utt_ids ? A.utt_ids[b] : A.utt_offset + (unsigned long long)b, (uint32_t)i, (uint32_t)c4, q);
-          } else {
-            float4 qv = *reinterpret_cast<const float4*>(A.q + ((size_t)i * A.B + b) * NC + c4 * 4);
-            q[0] = qv.x; q[1] = qv.y; q[2] = qv.z; q[3] = qv.w;
-          }
-#pragma unroll
-          for (int u = 0; u < 4; ++u) {
-            float l = lg[g * NC + c4 * 4 + u];
-            if (A.logits_out) A.logits_out[((size_t)i * A.B + b) * NC + c4 * 4 + u] = l;
-            unsigned long long p = pack_key(l - logf(q[u]), (uint32_t)(c4 * 4 + u));
-            best = p > best ? p : best;
-          }
+          for (int j = 0; j < kMolU; ++j) u[j] = A.q[((size_t)i * A.B + b) * kMolU + j];
         }
+        const float* p = lg + g * NC;
+        if (A.logits_out)
+          for (int j = 0; j < kMolParams; ++j) A.logits_out[((size_t)i * A.B + b) * kMolParams + j] = p[j];
+        const float x = mol_sample(p, u);
+        M.samples[(size_t)b * A.S + i] = x;
+        xin[g * ldI] = M.teacher_x ? M.teacher_x[(size_t)b * A.S + i] : x;
       }
-      best = warp_max_u64(best);
-      if (lane == 0) red[g][warp] = best;
-    }
-    __syncthreads();
-    if (warp == 0) {
+    } else {
+      // ---- sample: argmax_c (logit_c - log q_c), q ~ Exp(1)  == Categorical(softmax(logits)).sample() ----
 #pragma unroll
       for (int g = 0; g < G; ++g) {
-        unsigned long long v = lane < NW ? red[g][lane] : 0ull;
-        v = warp_max_u64(v);
-        if (lane == 0) {
-          const int b = b0 + g;
-          int label = (int)unpack_idx(v);
-          if (b < A.B) {
-            A.labels[(size_t)b * A.S + i] = (int16_t)label;
-            int fb = A.teacher ? (int)A.teacher[(size_t)b * A.S + i] : label;
-            xin[g * ldI] = label_to_float(fb, ncls_m1);
+        const int b = b0 + g;
+        unsigned long long best = 0ull;
+        if (b < A.B) {
+          for (int c4 = tid; c4 < NC / 4; c4 += kUttThreads) {
+            float q[4];
+            if (A.rng_mode == 0) {
+              philox_exp4(A.seed, A.utt_ids ? A.utt_ids[b] : A.utt_offset + (unsigned long long)b, (uint32_t)i, (uint32_t)c4, q);
+            } else {
+              float4 qv = *reinterpret_cast<const float4*>(A.q + ((size_t)i * A.B + b) * NC + c4 * 4);
+              q[0] = qv.x; q[1] = qv.y; q[2] = qv.z; q[3] = qv.w;
+            }
+#pragma unroll
+            for (int u = 0; u < 4; ++u) {
+              float l = lg[g * NC + c4 * 4 + u];
+              if (A.logits_out) A.logits_out[((size_t)i * A.B + b) * NC + c4 * 4 + u] = l;
+              unsigned long long p = pack_key(l - logf(q[u]), (uint32_t)(c4 * 4 + u));
+              best = p > best ? p : best;
+            }
+          }
+        }
+        best = warp_max_u64(best);
+        if (lane == 0) red[g][warp] = best;
+      }
+      __syncthreads();
+      if (warp == 0) {
+#pragma unroll
+        for (int g = 0; g < G; ++g) {
+          unsigned long long v = lane < NW ? red[g][lane] : 0ull;
+          v = warp_max_u64(v);
+          if (lane == 0) {
+            const int b = b0 + g;
+            int label = (int)unpack_idx(v);
+            if (b < A.B) {
+              A.labels[(size_t)b * A.S + i] = (int16_t)label;
+              int fb = A.teacher ? (int)A.teacher[(size_t)b * A.S + i] : label;
+              xin[g * ldI] = label_to_float(fb, ncls_m1);
+            }
           }
         }
       }
@@ -266,6 +287,16 @@ __global__ void __launch_bounds__(kUttThreads, 1) wavernn_utt_kernel(StepWeights
     cur ^= 1;
     __syncthreads();
   }
+}
+
+template <int G>
+__global__ void __launch_bounds__(kUttThreads, 1) wavernn_utt_kernel(StepWeights W, GenArgs A) {
+  utt_run<G, false>(W, A, MolIO{});
+}
+
+template <int G>
+__global__ void __launch_bounds__(kUttThreads, 1) wavernn_utt_mol_kernel(StepWeights W, GenArgs A, MolIO M) {
+  utt_run<G, true>(W, A, M);
 }
 
 }  // namespace b200tts

@@ -39,7 +39,9 @@ def all_gather_rows(local: torch.Tensor, n_items: int, group=None) -> torch.Tens
 
 def generate_sharded(generate_fn, mels, seed: int, group=None, **kw):
     """Runs `generate_fn(mels[lo:hi], seed=seed, utterance_offset=lo, **kw)` on this rank's slice of the GLOBAL batch
-    `mels [B, feat, T]` and all-gathers the int16 labels.  `generate_fn` is `WaveRNNEngine.generate`."""
+    `mels [B, feat, T]` and all-gathers the int16 labels.  `generate_fn` is `WaveRNNEngine.generate` of a RAW engine."""
+    if getattr(getattr(generate_fn, '__self__', None), 'mode', 'RAW') == 'MOL':
+        raise ValueError('sharded generation gathers int16 labels and is RAW only; run a MOL engine per GPU without sharding')
     world = dist.get_world_size(group) if dist.is_initialized() else 1
     rank = dist.get_rank(group) if dist.is_initialized() else 0
     n = mels.shape[0]

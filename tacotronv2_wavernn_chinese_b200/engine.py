@@ -33,8 +33,12 @@ def _ptr(t):
     return C.c_void_p(t.data_ptr()) if t is not None else C.c_void_p(0)
 
 
+MOL_PARAMS, MOL_U = 30, 11          # fc3 outputs and uniforms per step of a mixture-of-logistics model (voc_mode = 'MOL')
+
+
 class WaveRNNEngine:
-    """Owns the packed weights of one model on one device."""
+    """Owns the packed weights of one model on one device.  `dims['mode']` is the reference's voc_mode: 'RAW' (default)
+    or 'MOL'."""
 
     def __init__(self, state_dict: dict, dims: dict, device: int | None = None):
         if not torch.cuda.is_available():
@@ -42,10 +46,13 @@ class WaveRNNEngine:
         self.lib = _lib.load()
         self.device = torch.cuda.current_device() if device is None else int(device)
         self.dims = dict(dims)
+        self.mode = dims.get('mode', 'RAW')
+        if self.mode not in ('RAW', 'MOL'):
+            raise ValueError(f"unknown voc_mode {self.mode!r} (expected 'RAW' or 'MOL')")
         self.hop = int(dims['hop_length'])
         self.feat = int(dims['feat_dims'])
         self.res_out = int(dims['res_out_dims'])
-        self.n_classes = 1 << int(dims['bits'])
+        self.n_classes = MOL_PARAMS if self.mode == 'MOL' else 1 << int(dims['bits'])
         host = {}
         for k, v in state_dict.items():
             if hasattr(v, 'detach'):
@@ -56,7 +63,8 @@ class WaveRNNEngine:
         arr, keep = _lib.make_tensor_array(host)
         cfg = _cfg_from_dims(dims)
         h = C.c_void_p()
-        _lib.check(self.lib.b200tts_wavernn_create(C.byref(h), self.device, C.byref(cfg), arr, len(arr)))
+        create = self.lib.b200tts_wavernn_create_mol if self.mode == 'MOL' else self.lib.b200tts_wavernn_create
+        _lib.check(create(C.byref(h), self.device, C.byref(cfg), arr, len(arr)))
         del keep
         self._h = h
 
@@ -99,14 +107,28 @@ class WaveRNNEngine:
 
     def generate(self, mels, *, seed: int = 0, utterance_offset: int = 0, utterance_ids=None, q=None, teacher=None,
                  return_logits: bool = False, want_wave: bool = True, mu_law: bool = True, kernel: str = 'auto',
-                 max_steps: int = 0, fold=None, utt_frames=None, pack=None):
+                 max_steps: int = 0, fold=None, utt_frames=None, pack=None, u=None):
         """Runs the generation loop on the device.
 
         Returns dict(labels int16 [B,S] cuda, wave float64 [B,wave_len] cuda or None, logits [S,B,NC] or None).
         q: optional Exp(1) noise [S,B,NC] (torch/numpy) -> EXT_EXPONENTIAL mode; otherwise PHILOX(seed).
         pack: optional packed-row schedule dict(rows, utt int32 [rows, segs], start int32 [rows, segs+1], steps) from
         pipeline.pack_schedule: `rows` kernel rows run queues of the B utterances back to back (gen_opts.d_pack_*).
+
+        A MOL engine returns dict(samples float32 [B,S] cuda, wave, logits [S,B,30] or None) instead: it takes `u`, the
+        uniforms [S,B,11] of every step (EXT_UNIFORM mode), in place of `q`, `teacher` as float samples [B,S], and ignores
+        mu_law (the reference turns it off for MOL).  Folding changes [B,S] to [n_folds, fold_len] as for RAW.
         """
+        if self.mode == 'MOL':
+            if q is not None:
+                raise ValueError('a MOL engine takes uniforms u [S, B, 11], not the Exp(1) race noise q')
+            if pack is not None:
+                raise ValueError('packed rows are not built for MOL models: generate the utterances in plain batches')
+            return self._generate_mol(mels, seed=seed, utterance_offset=utterance_offset, utterance_ids=utterance_ids, u=u,
+                                      teacher=teacher, return_logits=return_logits, want_wave=want_wave, kernel=kernel,
+                                      max_steps=max_steps, fold=fold, utt_frames=utt_frames)
+        if u is not None:
+            raise ValueError('u (uniforms) is the noise of a MOL engine; a RAW engine takes q')
         m = self._mel(mels)
         B, _, T = m.shape
         S = T * self.hop
@@ -179,6 +201,69 @@ class WaveRNNEngine:
                     t.record_stream(torch.cuda.current_stream(self.device))
         return dict(labels=labels, wave=wave, logits=logits, steps=steps)
 
+    def _generate_mol(self, mels, *, seed, utterance_offset, utterance_ids, u, teacher, return_logits, want_wave, kernel,
+                      max_steps, fold, utt_frames):
+        m = self._mel(mels)
+        B, _, T = m.shape
+        S = T * self.hop
+        GB, GS = B, S
+        if fold is not None:
+            if B != 1:
+                raise ValueError('fold-with-overlap generation takes exactly one utterance')
+            GB, GS = self.fold_geometry(T, int(fold[0]), int(fold[1]))
+        steps = max_steps if max_steps else GS
+        dev = self._dev()
+        with torch.cuda.device(self.device):
+            samples = torch.zeros(GB, GS, device=dev, dtype=torch.float32)
+            wave = None
+            if want_wave and steps == GS:
+                wave = torch.empty(B, (T - 1) * self.hop, device=dev, dtype=torch.float64)
+            rng = Rng()
+            rng.seed = int(seed) & 0xFFFFFFFFFFFFFFFF
+            rng.utterance_offset = int(utterance_offset)
+            keep = []
+            if utterance_ids is not None:
+                ids = torch.as_tensor(np.asarray(utterance_ids, dtype=np.int64)).to(dev).contiguous()
+                if tuple(ids.shape) != (B,) or fold is not None:
+                    raise ValueError('utterance_ids must be [B] (and cannot be combined with fold)')
+                rng.d_utterance_ids = ids.data_ptr()
+                keep.append(ids)
+            if u is not None:
+                ud = torch.as_tensor(u).to(device=dev, dtype=torch.float32).contiguous()
+                if ud.dim() != 3 or tuple(ud.shape[1:]) != (GB, MOL_U) or ud.shape[0] < steps:
+                    raise ValueError(f'u must be [>= {steps}, {GB}, {MOL_U}], got {tuple(ud.shape)}')
+                rng.mode = _lib.RNG_EXT_UNIFORM
+                rng.d_q = ud.data_ptr()
+                keep.append(ud)
+            else:
+                rng.mode = _lib.RNG_PHILOX
+            opts = GenOpts()
+            opts.kernel = _lib.KERNELS[kernel]
+            opts.max_steps = int(max_steps)
+            if fold is not None:
+                opts.fold_target, opts.fold_overlap = int(fold[0]), int(fold[1])
+            if utt_frames is not None:
+                uf = torch.as_tensor(utt_frames).to(device=dev, dtype=torch.int32).contiguous()
+                if tuple(uf.shape) != (B,):
+                    raise ValueError('utt_frames must be [B]')
+                opts.d_utt_frames = uf.data_ptr()
+                keep.append(uf)
+            td = None
+            if teacher is not None:
+                td = torch.as_tensor(teacher).to(device=dev, dtype=torch.float32).contiguous()
+                if tuple(td.shape) != (GB, GS):
+                    raise ValueError('teacher must be [B, S] ([n_folds, fold_len] when folding)')
+                keep.append(td)
+            logits = None
+            if return_logits:
+                logits = torch.empty(steps, GB, MOL_PARAMS, device=dev, dtype=torch.float32)
+                opts.d_logits = logits.data_ptr()
+            _lib.check(self.lib.b200tts_wavernn_generate_mol(self._h, _ptr(m), B, T, C.byref(rng), C.byref(opts), _ptr(td),
+                                                             _ptr(samples), _ptr(wave), self._stream()))
+            for t in [m] + keep:
+                t.record_stream(torch.cuda.current_stream(self.device))
+        return dict(samples=samples, wave=wave, logits=logits, steps=steps)
+
     def fold_geometry(self, T: int, target: int, overlap: int):
         """(n_folds, fold_len) of fold_with_overlap for a T-frame utterance."""
         nf, fl = C.c_int(), C.c_int()
@@ -215,6 +300,14 @@ class WaveRNNEngine:
             _lib.check(self.lib.b200tts_philox_exponential(self.device, int(seed) & 0xFFFFFFFFFFFFFFFF, int(utterance_offset),
                                                            B, step0, n_steps, self.n_classes, _ptr(q), self._stream()))
         return q
+
+    def philox_mol_uniform(self, seed: int, utterance_offset: int, B: int, step0: int, n_steps: int):
+        """The uniforms the PHILOX mode of a MOL engine draws, [n_steps, B, 11] on the device (for parity tests)."""
+        with torch.cuda.device(self.device):
+            u = torch.empty(n_steps, B, MOL_U, device=self._dev(), dtype=torch.float32)
+            _lib.check(self.lib.b200tts_philox_mol_uniform(self.device, int(seed) & 0xFFFFFFFFFFFFFFFF, int(utterance_offset),
+                                                           B, step0, n_steps, _ptr(u), self._stream()))
+        return u
 
     def debug_phase_cycles(self):
         """[6][2] mean cycles (compute, barrier) per phase of the last grid launch; needs B200TTS_GRID_PROF=1.  After a

@@ -101,6 +101,7 @@ def vocode_ragged(voc, mels, ids, seed=0, max_rows=32, kernel='auto', allow_pack
     if n == 0:
         return []
     frames = [int(m.shape[0]) for m in mels]
+    allow_pack = allow_pack and getattr(voc, 'mode', 'RAW') == 'RAW'      # packed rows are not built for MOL models
     kind, plan = plan_ragged(frames, max_rows, voc.hop) if allow_pack else ('chunks', plan_chunks(frames, max_rows))
     if kind == 'pack':
         # ONE launch: `rows` kernel rows run queues of utterances back to back (state reset at every utterance start)

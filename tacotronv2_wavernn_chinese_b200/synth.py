@@ -24,11 +24,16 @@ def _uniform(rs, shape, bound):
     return rs.uniform(-bound, bound, size=shape).astype(np.float32)
 
 
-def synth_state_dict(seed: int = 0, dims: dict | None = None, logit_gain: float = 60.0) -> dict:
+def synth_state_dict(seed: int = 0, dims: dict | None = None, logit_gain: float = 60.0, mode: str = 'RAW',
+                     mol_clamp: bool = False) -> dict:
     """Deterministic numpy state_dict with the reference's key names.
 
     `logit_gain` scales fc3 so the softmax is peaky like the trained model's
     (trained |logit| reaches ~450, SURVEY.md section 4); gain 1 is torch-default init.
+    mode='MOL' gives the mixture-of-logistics head (voc_mode = 'MOL'): fc3 has 30 rows (10 mixture logits, 10 means,
+    10 log-scales) and its log-scale biases sit near -5, so that samples stay mostly inside [-1, 1].  `mol_clamp` moves
+    half the means beyond +-1 and half the log-scales below the sampler's floor log(1e-14), so both clamps fire often.
+    Every other tensor is the same as in RAW mode with the same seed.
     """
     d = dict(DEFAULT_DIMS)
     if dims:
@@ -75,9 +80,29 @@ def synth_state_dict(seed: int = 0, dims: dict | None = None, logit_gain: float 
     sd['fc1.bias'] = _uniform(rs, (F,), 1.0 / np.sqrt(R + aux))
     sd['fc2.weight'] = _uniform(rs, (F, F + aux), 1.0 / np.sqrt(F + aux))
     sd['fc2.bias'] = _uniform(rs, (F,), 1.0 / np.sqrt(F + aux))
+    if mode == 'MOL':
+        w = _uniform(rs, (30, F), 1.0 / np.sqrt(F))
+        w[:10] *= 4.0                                             # mixture logits: a few units apart
+        w[10:20] *= 0.5                                           # means
+        b = np.concatenate([_uniform(rs, (10,), 1.0), _uniform(rs, (10,), 0.5), -5.0 + _uniform(rs, (10,), 1.0)])
+        if mol_clamp:
+            b[10:20:2] += np.float32(1.5) * np.sign(b[10:20:2] + np.float32(1e-3))
+            b[21:30:2] = np.float32(-40.0)
+        sd['fc3.weight'] = w.astype(np.float32)
+        sd['fc3.bias'] = b.astype(np.float32)
+        return sd
+    if mode != 'RAW':
+        raise ValueError(f"unknown voc_mode {mode!r}")
     sd['fc3.weight'] = (logit_gain * _uniform(rs, (ncls, F), 1.0 / np.sqrt(F))).astype(np.float32)
     sd['fc3.bias'] = _uniform(rs, (ncls,), 1.0 / np.sqrt(F))
     return sd
+
+
+def synth_mol_uniform(seed: int, steps: int, batch: int) -> np.ndarray:
+    """The 11 uniforms of every step, u[S, B, 11] in [1e-5, 1 - 1e-5] (the range of the reference's uniform_ calls,
+    wavernn/utils/distribution.py:106,117), for the EXT_UNIFORM mode of MOL generation."""
+    rs = np.random.RandomState(seed)
+    return rs.uniform(1e-5, 1.0 - 1e-5, size=(steps, batch, 11)).astype(np.float32)
 
 
 def synth_mels(seed: int, batch: int, frames: int, feat_dims: int = 80) -> np.ndarray:

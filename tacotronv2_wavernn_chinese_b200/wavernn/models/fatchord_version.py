@@ -99,7 +99,7 @@ class WaveRNN(nn.Module):
         self.sample_rate = sample_rate
         self._dims = dict(rnn_dims=rnn_dims, fc_dims=fc_dims, bits=bits, pad=pad,
                           upsample_factors=tuple(upsample_factors), feat_dims=feat_dims, compute_dims=compute_dims,
-                          res_out_dims=res_out_dims, res_blocks=res_blocks, hop_length=hop_length)
+                          res_out_dims=res_out_dims, res_blocks=res_blocks, hop_length=hop_length, mode=mode)
 
         self.upsample = UpsampleNetwork(feat_dims, upsample_factors, compute_dims, res_blocks, res_out_dims, pad)
         self.I = nn.Linear(feat_dims + self.aux_dims + 1, rnn_dims)
@@ -124,8 +124,6 @@ class WaveRNN(nn.Module):
 
     def _engine_for_current_weights(self, device=None) -> WaveRNNEngine:
         """(Re)packs the weights into a libb200tts context when they changed since the last call."""
-        if self.mode != 'RAW':
-            raise NotImplementedError("only voc_mode='RAW' is on the GPU path (the shipped model, wavernn_hparams.py:35)")
         p = next(self.parameters())
         dev = device if device is not None else (p.device.index if p.is_cuda else torch.cuda.current_device()
                                                  if torch.cuda.is_available() else None)
@@ -170,7 +168,10 @@ class WaveRNN(nn.Module):
         out = eng.generate(m, seed=seed, mu_law=bool(mu_law), kernel=kernel, fold=(target, overlap) if batched else None)
         wave = out['wave'].cpu().numpy()                       # [B, wave_len] float64 (synchronises)
         eng.check()                                            # a timed-out persistent kernel must not yield audio
-        self.last_labels = out['labels']
+        if self.mode == 'MOL':
+            self.last_samples = out['samples']
+        else:
+            self.last_labels = out['labels']
         self.last_gen_seconds = time.time() - start
         b_size, seq_len = m.shape[0], T * self.hop_length
         self.gen_display(seq_len - 1, seq_len, b_size, start)
