@@ -777,15 +777,13 @@ static void run_generate_rows(b200tts_wavernn* ctx, const float* d_mel, int B, i
   ctx->last_kernel = kernel;
   ctx->prof_ncta = 0;
   ctx->aux_frames.ensure((size_t)B * T * O * sizeof(float));
+  // the rows' output, RAW labels or MOL samples: the context's scratch when the caller passed no buffer
   int16_t* labels = d_labels;
   float* samples = d_samples;
-  if (ctx->mol && !samples) {
-    ctx->labels.ensure((size_t)GB * GS * sizeof(float));
-    samples = ctx->labels.as<float>();
-  }
-  if (!ctx->mol && !labels) {
-    ctx->labels.ensure((size_t)GB * GS * sizeof(int16_t));
-    labels = ctx->labels.as<int16_t>();
+  if (ctx->mol ? !samples : !labels) {
+    ctx->labels.ensure((size_t)GB * GS * (ctx->mol ? sizeof(float) : sizeof(int16_t)));
+    if (ctx->mol) samples = ctx->labels.as<float>();
+    else labels = ctx->labels.as<int16_t>();
   }
   float* mels_up = nullptr;
   if (kernel == SK_UTTERANCE || (folding && kernel == SK_GRID)) {
@@ -812,24 +810,22 @@ static void run_generate_rows(b200tts_wavernn* ctx, const float* d_mel, int B, i
     case SK_TC: launch_tc(ctx, d_mel, a, prof, st); break;
   }
   ctx->ev_valid = true;
-  if (d_wave && ctx->mol) {
+  if (d_wave) {
+    const int* err = ctx->error.as<int>();
     if (folding) {
-      xfade_unfold_mol_kernel<<<(wave_len + 255) / 256, 256, 0, st>>>(samples, fg.nfold, fg.L, o.fold_target, o.fold_overlap,
-                                                                      wave_len, fade_len, ctx->error.as<int>(), d_wave);
+      const int blocks = (wave_len + 255) / 256;
+      if (ctx->mol)
+        xfade_unfold_mol_kernel<<<blocks, 256, 0, st>>>(samples, fg.nfold, fg.L, o.fold_target, o.fold_overlap, wave_len, fade_len,
+                                                        err, d_wave);
+      else
+        xfade_unfold_kernel<<<blocks, 256, 0, st>>>(labels, fg.nfold, fg.L, o.fold_target, o.fold_overlap, wave_len, fade_len,
+                                                    ctx->NC, o.mu_law, err, d_wave);
     } else {
       dim3 grid((wave_len + 255) / 256, B);
-      finish_wave_mol_kernel<<<grid, 256, 0, st>>>(samples, S, wave_len, fade_len, o.d_utt_frames, hop, ctx->error.as<int>(), d_wave);
-    }
-    B200_CUDA(cudaGetLastError());
-    ctx->launches++;
-  } else if (d_wave) {
-    if (folding) {
-      xfade_unfold_kernel<<<(wave_len + 255) / 256, 256, 0, st>>>(labels, fg.nfold, fg.L, o.fold_target, o.fold_overlap, wave_len,
-                                                                  fade_len, ctx->NC, o.mu_law, ctx->error.as<int>(), d_wave);
-    } else {
-      dim3 grid((wave_len + 255) / 256, B);
-      finish_wave_kernel<<<grid, 256, 0, st>>>(labels, S, wave_len, fade_len, ctx->NC, o.mu_law, o.d_utt_frames, hop,
-                                               ctx->error.as<int>(), d_wave);
+      if (ctx->mol)
+        finish_wave_mol_kernel<<<grid, 256, 0, st>>>(samples, S, wave_len, fade_len, o.d_utt_frames, hop, err, d_wave);
+      else
+        finish_wave_kernel<<<grid, 256, 0, st>>>(labels, S, wave_len, fade_len, ctx->NC, o.mu_law, o.d_utt_frames, hop, err, d_wave);
     }
     B200_CUDA(cudaGetLastError());
     ctx->launches++;

@@ -174,13 +174,36 @@ __device__ __forceinline__ double xfade_t(int k, int flen) {
   return (k == flen - 1) ? 1.0 : (-1.0 + k * (2.0 / (flen - 1)));
 }
 
+// The two wave epilogues below read RAW labels and MOL samples through one of these readers, which return stored sample i as
+// the float64 the wave is built from, so that the fade, overlap-add, truncation and NaN poisoning are written once for both.
+// A RAW label is decoded and, with mu_law, expanded (dsp.py:98-103); a MOL sample is used as is (generate() forces mu_law
+// off for MOL, :174).  The kernel sets `mu` once: computing it per sample inside the reader changes the RAW kernels' code.
+struct LabelSamples {
+  const int16_t* __restrict__ labels;
+  double mu;
+  int ncls, mu_law;
+  __device__ __forceinline__ double operator()(size_t i) const {
+    float yf = label_to_float((int)labels[i], (float)(ncls - 1));
+    double y = (double)yf;
+    if (mu_law) {
+      const double a = fabs(y), sgn = (y > 0.0) - (y < 0.0);
+      y = sgn / mu * (pow(1.0 + mu, a) - 1.0);
+    }
+    return y;
+  }
+};
+struct FloatSamples {
+  const float* __restrict__ samples;
+  __device__ __forceinline__ double operator()(size_t i) const { return (double)samples[i]; }
+};
+
 // xfade_and_unfold (fatchord_version.py:342-405) + the generate() epilogue (:247-258), fp64:
-// decode every fold's labels, apply the equal-power fade-in/out over `overlap` (first half of the fade-in is silence),
+// read every fold's samples, apply the equal-power fade-in/out over `overlap` (first half of the fade-in is silence),
 // overlap-add at stride target+overlap, truncate to wave_len, 20-hop linear fade-out.
-__global__ void xfade_unfold_kernel(const int16_t* __restrict__ labels /*[nfold][L]*/, int nfold, int L, int target, int overlap,
-                                    int wave_len, int fade_len, int ncls, int mu_law, const int* __restrict__ gen_error,
-                                    double* __restrict__ wave /*[wave_len]*/) {
-  const double mu = (double)(ncls - 1);
+template <class Samples>
+__device__ __forceinline__ void xfade_unfold(const Samples& sample /*[nfold][L]*/, int nfold, int L, int target, int overlap,
+                                             int wave_len, int fade_len, const int* __restrict__ gen_error,
+                                             double* __restrict__ wave /*[wave_len]*/) {
   const bool poisoned = gen_error && *gen_error;    // the generation kernel timed out: never hand back plausible-looking audio
   const int stride = target + overlap;
   const int silence = overlap / 2, flen = overlap - silence;
@@ -192,12 +215,7 @@ __global__ void xfade_unfold_kernel(const int16_t* __restrict__ labels /*[nfold]
     for (int u = u_hi; u >= 0 && u >= u_hi - 1; --u) {
       const int t = n - u * stride;
       if (t < 0 || t >= L) continue;
-      float yf = label_to_float((int)labels[(size_t)u * L + t], (float)(ncls - 1));
-      double y = (double)yf;
-      if (mu_law) {
-        const double a = fabs(y), sgn = (y > 0.0) - (y < 0.0);
-        y = sgn / mu * (pow(1.0 + mu, a) - 1.0);
-      }
+      double y = sample((size_t)u * L + t);
       // np.linspace(-1, 1, flen)[k] = -1 + k * 2/(flen-1)
       if (t < overlap) {
         double g = 0.0;
@@ -218,81 +236,48 @@ __global__ void xfade_unfold_kernel(const int16_t* __restrict__ labels /*[nfold]
   }
 }
 
-// generate() epilogue (fatchord_version.py:243-258): float64, decode_mu_law (dsp.py:98-103), truncate, 20-hop fade.
+// generate() epilogue (fatchord_version.py:243-258): float64, truncate, 20-hop fade.
 // `utt_frames` (optional, [B]): true frame count of each row of a zero-padded ragged batch -> that row is truncated / faded at
 // ITS OWN (T_b - 1) * hop like a batch-1 run of the reference, and zero beyond.
-__global__ void finish_wave_kernel(const int16_t* __restrict__ labels /*[B][S]*/, int S, int wave_len_max, int fade_len,
-                                   int ncls, int mu_law, const int* __restrict__ utt_frames, int hop,
-                                   const int* __restrict__ gen_error, double* __restrict__ wave /*[B][wave_len_max]*/) {
+template <class Samples>
+__device__ __forceinline__ void finish_wave(const Samples& sample /*[B][S]*/, int S, int wave_len_max, int fade_len,
+                                            const int* __restrict__ utt_frames, int hop, const int* __restrict__ gen_error,
+                                            double* __restrict__ wave /*[B][wave_len_max]*/) {
   const int b = blockIdx.y;
   const bool poisoned = gen_error && *gen_error;    // the generation kernel timed out: never hand back plausible-looking audio
-  const double mu = (double)(ncls - 1);
   const double step = -1.0 / (double)(fade_len - 1);   // np.linspace(1, 0, fade_len)
   const int wave_len = utt_frames ? min(wave_len_max, max(0, (utt_frames[b] - 1) * hop)) : wave_len_max;
   for (int i = blockIdx.x * blockDim.x + threadIdx.x; i < wave_len_max; i += gridDim.x * blockDim.x) {
     if (i >= wave_len) { wave[(size_t)b * wave_len_max + i] = 0.0; continue; }
-    float yf = label_to_float((int)labels[(size_t)b * S + i], (float)(ncls - 1));
-    double y = (double)yf;
-    if (mu_law) {
-      double a = fabs(y);
-      double sgn = (y > 0.0) - (y < 0.0);
-      y = sgn / mu * (pow(1.0 + mu, a) - 1.0);
-    }
+    double y = sample((size_t)b * S + i);
     int k = i - (wave_len - fade_len);
     if (k >= 0) y *= (k == fade_len - 1) ? 0.0 : (1.0 + (double)k * step);
     wave[(size_t)b * wave_len_max + i] = poisoned ? nan("") : y;
   }
 }
 
-// The same two epilogues for MOL samples: float samples in, no decode (generate() forces mu_law off for MOL, :174).
+__global__ void xfade_unfold_kernel(const int16_t* __restrict__ labels /*[nfold][L]*/, int nfold, int L, int target, int overlap,
+                                    int wave_len, int fade_len, int ncls, int mu_law, const int* __restrict__ gen_error,
+                                    double* __restrict__ wave /*[wave_len]*/) {
+  xfade_unfold(LabelSamples{labels, (double)(ncls - 1), ncls, mu_law}, nfold, L, target, overlap, wave_len, fade_len, gen_error, wave);
+}
+
+__global__ void finish_wave_kernel(const int16_t* __restrict__ labels /*[B][S]*/, int S, int wave_len_max, int fade_len,
+                                   int ncls, int mu_law, const int* __restrict__ utt_frames, int hop,
+                                   const int* __restrict__ gen_error, double* __restrict__ wave /*[B][wave_len_max]*/) {
+  finish_wave(LabelSamples{labels, (double)(ncls - 1), ncls, mu_law}, S, wave_len_max, fade_len, utt_frames, hop, gen_error, wave);
+}
+
 __global__ void xfade_unfold_mol_kernel(const float* __restrict__ samples /*[nfold][L]*/, int nfold, int L, int target, int overlap,
                                         int wave_len, int fade_len, const int* __restrict__ gen_error,
                                         double* __restrict__ wave /*[wave_len]*/) {
-  const bool poisoned = gen_error && *gen_error;
-  const int stride = target + overlap;
-  const int silence = overlap / 2, flen = overlap - silence;
-  const double lin_step = -1.0 / (double)(fade_len - 1);
-  for (int n = blockIdx.x * blockDim.x + threadIdx.x; n < wave_len; n += gridDim.x * blockDim.x) {
-    double acc = 0.0;
-    int u_hi = n / stride;
-    if (u_hi >= nfold) u_hi = nfold - 1;
-    for (int u = u_hi; u >= 0 && u >= u_hi - 1; --u) {
-      const int t = n - u * stride;
-      if (t < 0 || t >= L) continue;
-      double y = (double)samples[(size_t)u * L + t];
-      if (t < overlap) {
-        double g = 0.0;
-        if (t >= silence) { const int k = t - silence; const double tt = xfade_t(k, flen); g = sqrt(0.5 * (1.0 + tt)); }
-        y *= g;
-      }
-      if (t >= L - overlap) {
-        const int k2 = t - (L - overlap);
-        double g = 1.0;
-        if (k2 >= silence) { const int k = k2 - silence; const double tt = xfade_t(k, flen); g = sqrt(0.5 * (1.0 - tt)); }
-        y *= g;
-      }
-      acc += y;
-    }
-    const int k = n - (wave_len - fade_len);
-    if (k >= 0) acc *= (k == fade_len - 1) ? 0.0 : (1.0 + (double)k * lin_step);
-    wave[n] = poisoned ? nan("") : acc;
-  }
+  xfade_unfold(FloatSamples{samples}, nfold, L, target, overlap, wave_len, fade_len, gen_error, wave);
 }
 
 __global__ void finish_wave_mol_kernel(const float* __restrict__ samples /*[B][S]*/, int S, int wave_len_max, int fade_len,
                                        const int* __restrict__ utt_frames, int hop, const int* __restrict__ gen_error,
                                        double* __restrict__ wave /*[B][wave_len_max]*/) {
-  const int b = blockIdx.y;
-  const bool poisoned = gen_error && *gen_error;
-  const double step = -1.0 / (double)(fade_len - 1);
-  const int wave_len = utt_frames ? min(wave_len_max, max(0, (utt_frames[b] - 1) * hop)) : wave_len_max;
-  for (int i = blockIdx.x * blockDim.x + threadIdx.x; i < wave_len_max; i += gridDim.x * blockDim.x) {
-    if (i >= wave_len) { wave[(size_t)b * wave_len_max + i] = 0.0; continue; }
-    double y = (double)samples[(size_t)b * S + i];
-    int k = i - (wave_len - fade_len);
-    if (k >= 0) y *= (k == fade_len - 1) ? 0.0 : (1.0 + (double)k * step);
-    wave[(size_t)b * wave_len_max + i] = poisoned ? nan("") : y;
-  }
+  finish_wave(FloatSamples{samples}, S, wave_len_max, fade_len, utt_frames, hop, gen_error, wave);
 }
 
 }  // namespace b200tts

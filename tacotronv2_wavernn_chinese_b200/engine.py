@@ -119,16 +119,17 @@ class WaveRNNEngine:
         uniforms [S,B,11] of every step (EXT_UNIFORM mode), in place of `q`, `teacher` as float samples [B,S], and ignores
         mu_law (the reference turns it off for MOL).  Folding changes [B,S] to [n_folds, fold_len] as for RAW.
         """
-        if self.mode == 'MOL':
+        mol = self.mode == 'MOL'
+        if mol:
             if q is not None:
                 raise ValueError('a MOL engine takes uniforms u [S, B, 11], not the Exp(1) race noise q')
             if pack is not None:
                 raise ValueError('packed rows are not built for MOL models: generate the utterances in plain batches')
-            return self._generate_mol(mels, seed=seed, utterance_offset=utterance_offset, utterance_ids=utterance_ids, u=u,
-                                      teacher=teacher, return_logits=return_logits, want_wave=want_wave, kernel=kernel,
-                                      max_steps=max_steps, fold=fold, utt_frames=utt_frames)
-        if u is not None:
-            raise ValueError('u (uniforms) is the noise of a MOL engine; a RAW engine takes q')
+            noise, noise_name, noise_width, noise_mode = u, 'u', MOL_U, _lib.RNG_EXT_UNIFORM
+        else:
+            if u is not None:
+                raise ValueError('u (uniforms) is the noise of a MOL engine; a RAW engine takes q')
+            noise, noise_name, noise_width, noise_mode = q, 'q', self.n_classes, _lib.RNG_EXT_EXPONENTIAL
         m = self._mel(mels)
         B, _, T = m.shape
         S = T * self.hop
@@ -140,35 +141,36 @@ class WaveRNNEngine:
         steps = max_steps if max_steps else GS
         dev = self._dev()
         with torch.cuda.device(self.device):
-            labels = torch.zeros(GB, GS, device=dev, dtype=torch.int16)
+            # labels (RAW) or samples (MOL); a teacher is fed back in their place, so it takes their dtype
+            out = torch.zeros(GB, GS, device=dev, dtype=torch.float32 if mol else torch.int16)
             wave = None
             if want_wave and steps == GS:
                 wave = torch.empty(B, (T - 1) * self.hop, device=dev, dtype=torch.float64)
+            keep = [m]                          # inputs the stream reads after this call returns
             rng = Rng()
             rng.seed = int(seed) & 0xFFFFFFFFFFFFFFFF
             rng.utterance_offset = int(utterance_offset)
-            ids = None
             if utterance_ids is not None:       # rows that are NOT consecutive utterances (length-sorted chunks): per-row global index
                 ids = torch.as_tensor(np.asarray(utterance_ids, dtype=np.int64)).to(dev).contiguous()
                 if tuple(ids.shape) != (B,) or fold is not None:
                     raise ValueError('utterance_ids must be [B] (and cannot be combined with fold)')
                 rng.d_utterance_ids = ids.data_ptr()
-            qd = None
-            if q is not None:
-                qd = torch.as_tensor(q).to(device=dev, dtype=torch.float32).contiguous()
-                if qd.dim() != 3 or tuple(qd.shape[1:]) != (GB, self.n_classes) or qd.shape[0] < steps:
-                    raise ValueError(f'q must be [>= {steps}, {GB}, {self.n_classes}], got {tuple(qd.shape)}')
-                rng.mode = _lib.RNG_EXT_EXPONENTIAL
-                rng.d_q = qd.data_ptr()
+                keep.append(ids)
+            if noise is not None:
+                nd = torch.as_tensor(noise).to(device=dev, dtype=torch.float32).contiguous()
+                if nd.dim() != 3 or tuple(nd.shape[1:]) != (GB, noise_width) or nd.shape[0] < steps:
+                    raise ValueError(f'{noise_name} must be [>= {steps}, {GB}, {noise_width}], got {tuple(nd.shape)}')
+                rng.mode = noise_mode
+                rng.d_q = nd.data_ptr()
+                keep.append(nd)
             else:
                 rng.mode = _lib.RNG_PHILOX
             opts = GenOpts()
             opts.kernel = _lib.KERNELS[kernel]
-            opts.mu_law = 1 if mu_law else 0
+            opts.mu_law = 1 if mu_law and not mol else 0
             opts.max_steps = int(max_steps)
             if fold is not None:
                 opts.fold_target, opts.fold_overlap = int(fold[0]), int(fold[1])
-            pk_u = pk_s = None
             if pack is not None:
                 pk_u = torch.as_tensor(np.ascontiguousarray(pack['utt'], dtype=np.int32)).to(dev)
                 pk_s = torch.as_tensor(np.ascontiguousarray(pack['start'], dtype=np.int32)).to(dev)
@@ -177,71 +179,7 @@ class WaveRNNEngine:
                     raise ValueError('pack: utt must be [rows, segs], start [rows, segs + 1]')
                 opts.d_pack_utt, opts.d_pack_start = pk_u.data_ptr(), pk_s.data_ptr()
                 opts.pack_rows, opts.pack_segs, opts.pack_steps = rows, segs, int(pack['steps'])
-            uf = None
-            if utt_frames is not None:
-                uf = torch.as_tensor(utt_frames).to(device=dev, dtype=torch.int32).contiguous()
-                if tuple(uf.shape) != (B,):
-                    raise ValueError('utt_frames must be [B]')
-                opts.d_utt_frames = uf.data_ptr()
-            td = None
-            if teacher is not None:
-                td = torch.as_tensor(teacher).to(device=dev, dtype=torch.int16).contiguous()
-                if tuple(td.shape) != (GB, GS):
-                    raise ValueError('teacher must be [B, S] ([n_folds, fold_len] when folding)')
-                opts.d_teacher = td.data_ptr()
-            logits = None
-            if return_logits:
-                logits = torch.empty(steps, GB, self.n_classes, device=dev, dtype=torch.float32)
-                opts.d_logits = logits.data_ptr()
-            _lib.check(self.lib.b200tts_wavernn_generate(self._h, _ptr(m), B, T, C.byref(rng), C.byref(opts),
-                                                         _ptr(labels), _ptr(wave), self._stream()))
-            # keep inputs alive until the stream has consumed them
-            for t in (m, qd, td, uf, ids, pk_u, pk_s):
-                if t is not None:
-                    t.record_stream(torch.cuda.current_stream(self.device))
-        return dict(labels=labels, wave=wave, logits=logits, steps=steps)
-
-    def _generate_mol(self, mels, *, seed, utterance_offset, utterance_ids, u, teacher, return_logits, want_wave, kernel,
-                      max_steps, fold, utt_frames):
-        m = self._mel(mels)
-        B, _, T = m.shape
-        S = T * self.hop
-        GB, GS = B, S
-        if fold is not None:
-            if B != 1:
-                raise ValueError('fold-with-overlap generation takes exactly one utterance')
-            GB, GS = self.fold_geometry(T, int(fold[0]), int(fold[1]))
-        steps = max_steps if max_steps else GS
-        dev = self._dev()
-        with torch.cuda.device(self.device):
-            samples = torch.zeros(GB, GS, device=dev, dtype=torch.float32)
-            wave = None
-            if want_wave and steps == GS:
-                wave = torch.empty(B, (T - 1) * self.hop, device=dev, dtype=torch.float64)
-            rng = Rng()
-            rng.seed = int(seed) & 0xFFFFFFFFFFFFFFFF
-            rng.utterance_offset = int(utterance_offset)
-            keep = []
-            if utterance_ids is not None:
-                ids = torch.as_tensor(np.asarray(utterance_ids, dtype=np.int64)).to(dev).contiguous()
-                if tuple(ids.shape) != (B,) or fold is not None:
-                    raise ValueError('utterance_ids must be [B] (and cannot be combined with fold)')
-                rng.d_utterance_ids = ids.data_ptr()
-                keep.append(ids)
-            if u is not None:
-                ud = torch.as_tensor(u).to(device=dev, dtype=torch.float32).contiguous()
-                if ud.dim() != 3 or tuple(ud.shape[1:]) != (GB, MOL_U) or ud.shape[0] < steps:
-                    raise ValueError(f'u must be [>= {steps}, {GB}, {MOL_U}], got {tuple(ud.shape)}')
-                rng.mode = _lib.RNG_EXT_UNIFORM
-                rng.d_q = ud.data_ptr()
-                keep.append(ud)
-            else:
-                rng.mode = _lib.RNG_PHILOX
-            opts = GenOpts()
-            opts.kernel = _lib.KERNELS[kernel]
-            opts.max_steps = int(max_steps)
-            if fold is not None:
-                opts.fold_target, opts.fold_overlap = int(fold[0]), int(fold[1])
+                keep += [pk_u, pk_s]
             if utt_frames is not None:
                 uf = torch.as_tensor(utt_frames).to(device=dev, dtype=torch.int32).contiguous()
                 if tuple(uf.shape) != (B,):
@@ -250,19 +188,25 @@ class WaveRNNEngine:
                 keep.append(uf)
             td = None
             if teacher is not None:
-                td = torch.as_tensor(teacher).to(device=dev, dtype=torch.float32).contiguous()
+                td = torch.as_tensor(teacher).to(device=dev, dtype=out.dtype).contiguous()
                 if tuple(td.shape) != (GB, GS):
                     raise ValueError('teacher must be [B, S] ([n_folds, fold_len] when folding)')
+                if not mol:
+                    opts.d_teacher = td.data_ptr()
                 keep.append(td)
             logits = None
             if return_logits:
-                logits = torch.empty(steps, GB, MOL_PARAMS, device=dev, dtype=torch.float32)
+                logits = torch.empty(steps, GB, self.n_classes, device=dev, dtype=torch.float32)
                 opts.d_logits = logits.data_ptr()
-            _lib.check(self.lib.b200tts_wavernn_generate_mol(self._h, _ptr(m), B, T, C.byref(rng), C.byref(opts), _ptr(td),
-                                                             _ptr(samples), _ptr(wave), self._stream()))
-            for t in [m] + keep:
+            if mol:
+                _lib.check(self.lib.b200tts_wavernn_generate_mol(self._h, _ptr(m), B, T, C.byref(rng), C.byref(opts), _ptr(td),
+                                                                 _ptr(out), _ptr(wave), self._stream()))
+            else:
+                _lib.check(self.lib.b200tts_wavernn_generate(self._h, _ptr(m), B, T, C.byref(rng), C.byref(opts),
+                                                             _ptr(out), _ptr(wave), self._stream()))
+            for t in keep:
                 t.record_stream(torch.cuda.current_stream(self.device))
-        return dict(samples=samples, wave=wave, logits=logits, steps=steps)
+        return {'samples' if mol else 'labels': out, 'wave': wave, 'logits': logits, 'steps': steps}
 
     def fold_geometry(self, T: int, target: int, overlap: int):
         """(n_folds, fold_len) of fold_with_overlap for a T-frame utterance."""
