@@ -6,6 +6,7 @@
 #include <cmath>
 #include <cstdio>
 #include <cstdlib>
+#include <set>
 
 #include "api.h"
 #include "wavernn_upsample.cuh"
@@ -15,6 +16,16 @@
 #include "wavernn_tc.cuh"
 
 using namespace b200tts;
+
+// One RAW utterance generated in pieces on the push kernel (b200tts_wavernn_session_*): its conditioning tables, computed once
+// at open, and the state its last run saved (SessRow).  Owned by its context, which frees the sessions still open.
+struct b200tts_wavernn_session {
+  b200tts_wavernn* ctx = nullptr;
+  int T = 0, mu_law = 1;
+  int64_t pos = 0, S = 0, wave_len = 0;     // next step; steps of the utterance; samples of its wave
+  uint64_t seed = 0, id = 0;
+  DeviceBuf tab, state;
+};
 
 struct b200tts_wavernn {
   int device = 0;
@@ -44,7 +55,10 @@ struct b200tts_wavernn {
   bool ev_valid = false;
   int64_t launches = 0;
   bool warned_fallback = false;
+  std::set<b200tts_wavernn_session*> sessions;   // open sessions, freed with the context
+  DeviceBuf sess_labels;                         // labels of a session run whose caller passed none
   ~b200tts_wavernn() {
+    for (b200tts_wavernn_session* s : sessions) delete s;
     if (ev0) cudaEventDestroy(ev0);
     if (ev1) cudaEventDestroy(ev1);
   }
@@ -388,7 +402,7 @@ extern "C" int b200tts_wavernn_upsample(b200tts_wavernn* ctx, const float* d_mel
 
 // ---- generation -----------------------------------------------------------------------------------
 // The step kernel a launch runs; the values are those b200tts_wavernn_last_kernel reports.
-enum StepKernel { SK_UTTERANCE = 1, SK_GRID = 2, SK_PUSH = 3, SK_TC = 5 };
+enum StepKernel { SK_UTTERANCE = 1, SK_GRID = 2, SK_PUSH = 3, SK_TC = 5, SK_SESSION = 6 };
 
 // The fields every step kernel's arguments take from GenArgs as they are: noise, debug buffers, labels.
 template <class Args>
@@ -582,17 +596,21 @@ static void launch_grid(b200tts_wavernn* ctx, const float* d_mel, const GenArgs&
 
 // Conditioning tables [tab_rows][T+1][ncta][52] of the push and tensor-core kernels from the first `src_rows` utterances of the
 // mels / frame-rate aux; table rows past them are zero.
+// `dst` (optional): the tables go there instead of the context's scratch ctx->push_tab.
 static const float* launch_cond_table(b200tts_wavernn* ctx, const float* d_mel, const float* aux_frames, int src_rows, int tab_rows,
-                                      int T, cudaStream_t st) {
+                                      int T, cudaStream_t st, float* dst = nullptr) {
   const b200tts_wavernn_cfg& c = ctx->cfg;
   constexpr int FT = 8;
-  ctx->push_tab.ensure((size_t)tab_rows * (T + 1) * ctx->pm.ncta * kPushCondRows * sizeof(float));
+  if (!dst) {
+    ctx->push_tab.ensure((size_t)tab_rows * (T + 1) * ctx->pm.ncta * kPushCondRows * sizeof(float));
+    dst = ctx->push_tab.as<float>();
+  }
   dim3 grid((T + 1 + FT - 1) / FT, tab_rows);
   size_t smem = (size_t)(c.feat_dims + c.res_out_dims) * FT * sizeof(float);
-  push_cond_table_kernel<FT><<<grid, 256, smem, st>>>(ctx->pcw, d_mel, aux_frames, src_rows, T, ctx->push_tab.as<float>());
+  push_cond_table_kernel<FT><<<grid, 256, smem, st>>>(ctx->pcw, d_mel, aux_frames, src_rows, T, dst);
   B200_CUDA(cudaGetLastError());
   ctx->launches++;
-  return ctx->push_tab.as<float>();
+  return dst;
 }
 
 // ---- small-batch push kernel (wavernn_push.cuh) --------------------------------------------------------------------------
@@ -988,6 +1006,142 @@ extern "C" int b200tts_wavernn_debug_phase_cycles(b200tts_wavernn* ctx, double* 
     for (int c = 0; c < n; ++c) s += (double)h[(size_t)c * 12 + i];
     out12[i] = s / n;
   }
+  API_END
+}
+
+// ---- generation sessions: one RAW utterance in pieces on the push kernel (wavernn_push_session_kernel) ---------------------
+// Every refusal below comes before the first CUDA call, so a refused call has launched and allocated nothing.
+static void require_session_model(const b200tts_wavernn* ctx) {
+  REQUIRE(!ctx->mol, B200TTS_EINVAL, "generation sessions are RAW only: this context holds a MOL model");
+  REQUIRE(ctx->pm.ok, B200TTS_EINVAL, "generation sessions need the push kernel (rnn_dims = fc_dims = 512 on >= 128 SMs)");
+}
+
+extern "C" int b200tts_wavernn_session_open(b200tts_wavernn* ctx, const float* d_mel, int T, const b200tts_rng* rng, int mu_law,
+                                            b200tts_wavernn_session** out, void* stream) {
+  API_BEGIN
+  REQUIRE(ctx && d_mel && rng && out, B200TTS_EINVAL, "null argument");
+  *out = nullptr;
+  require_session_model(ctx);
+  REQUIRE(rng->mode == B200TTS_RNG_PHILOX && !rng->d_utterance_ids, B200TTS_EINVAL,
+          "a session takes PHILOX noise keyed by (seed, rng->utterance_offset as the utterance id); d_utterance_ids must be NULL");
+  const int hop = ctx->cfg.hop_length;
+  REQUIRE(T >= 21, B200TTS_EINVAL, "T must be >= 21 frames: the reference's 20-hop fade-out (fatchord_version.py:256-258) fails below that");
+  REQUIRE((long long)T * hop <= INT_MAX, B200TTS_EINVAL, "utterance longer than 2^31 - 1 samples");
+  DeviceGuard dg(ctx->device);
+  const cudaStream_t st = (cudaStream_t)stream;
+  std::unique_ptr<b200tts_wavernn_session> s(new b200tts_wavernn_session());
+  s->ctx = ctx;
+  s->T = T;
+  s->mu_law = mu_law ? 1 : 0;
+  s->S = (int64_t)T * hop;
+  s->wave_len = (int64_t)(T - 1) * hop;
+  s->seed = rng->seed;
+  s->id = rng->utterance_offset;
+  s->tab.ensure((size_t)(T + 1) * ctx->pm.ncta * kPushCondRows * sizeof(float));
+  s->state.ensure((size_t)kSessStateFloats * sizeof(float));
+  // the conditioning of a one-shot run of this mel, once: MelResNet into the context's scratch, consumed in stream order by the
+  // tables, which the session owns (the next generate overwrites every scratch buffer)
+  ctx->aux_frames.ensure((size_t)T * ctx->cfg.res_out_dims * sizeof(float));
+  run_upsample(ctx, d_mel, 1, T, nullptr, ctx->aux_frames.as<float>(), nullptr, st);
+  launch_cond_table(ctx, d_mel, ctx->aux_frames.as<float>(), 1, 1, T, st, s->tab.as<float>());
+  ctx->sessions.insert(s.get());
+  *out = s.release();
+  API_END
+}
+
+// cudaFree waits for the work queued on the device, so no run still in flight reads the memory freed here.
+extern "C" void b200tts_wavernn_session_destroy(b200tts_wavernn_session* s) {
+  if (!s) return;
+  DeviceGuard dg(s->ctx->device, true);
+  s->ctx->sessions.erase(s);
+  delete s;
+}
+
+extern "C" int b200tts_wavernn_session_info(const b200tts_wavernn_session* s, int64_t* pos, int64_t* steps, int64_t* wave_len) {
+  API_BEGIN
+  REQUIRE(s, B200TTS_EINVAL, "null argument");
+  if (pos) *pos = s->pos;
+  if (steps) *steps = s->S;
+  if (wave_len) *wave_len = s->wave_len;
+  API_END
+}
+
+template <int G>
+static void launch_session_t(b200tts_wavernn* ctx, PushArgs& a, SessIO& io, cudaStream_t st) {
+  PushModel pm = ctx->pm;
+  const size_t smem = ((size_t)pm.blob + (size_t)PushTraits<G>::scratch_floats(a.hop, a.NT)) * sizeof(float);
+  void* args[] = {(void*)&pm, (void*)&a, (void*)&io};
+  coop_launch(ctx, (const void*)wavernn_push_session_kernel<G>, "push session kernel", pm.ncta, kPushThreads, smem, args, st);
+}
+
+extern "C" int b200tts_wavernn_session_run(b200tts_wavernn* ctx, b200tts_wavernn_session* const* s, int n, int max_steps,
+                                           int16_t* d_labels, double* d_wave, void* stream) {
+  API_BEGIN
+  REQUIRE(ctx && s, B200TTS_EINVAL, "null argument");
+  require_session_model(ctx);
+  REQUIRE(n >= 1 && n <= kPushMaxRows, B200TTS_EINVAL, "a session run takes 1..32 sessions");
+  REQUIRE(max_steps >= 1, B200TTS_EINVAL, "max_steps must be >= 1");
+  for (int i = 0; i < n; ++i) {
+    REQUIRE(s[i], B200TTS_EINVAL, "null session");
+    REQUIRE(s[i]->ctx == ctx, B200TTS_EINVAL, "the session belongs to another context");
+    for (int j = 0; j < i; ++j) REQUIRE(s[j] != s[i], B200TTS_EINVAL, "the same session appears twice in one run");
+  }
+  DeviceGuard dg(ctx->device);
+  const cudaStream_t st = (cudaStream_t)stream;
+  SessIO io{};
+  int steps = 0;
+  for (int i = 0; i < n; ++i) {
+    SessRow& r = io.row[i];
+    r.tab = s[i]->tab.as<float>();
+    r.state = s[i]->state.as<float>();
+    r.seed = s[i]->seed;
+    r.id = s[i]->id;
+    r.T = s[i]->T;
+    r.pos = (int)s[i]->pos;
+    r.n = (int)std::min<int64_t>(max_steps, s[i]->S - s[i]->pos);
+    r.mu_law = s[i]->mu_law;
+    steps = std::max(steps, r.n);
+  }
+  io.ld = max_steps;
+  io.labels = d_labels;
+  if (!io.labels) {
+    ctx->sess_labels.ensure((size_t)n * max_steps * sizeof(int16_t));
+    io.labels = ctx->sess_labels.as<int16_t>();
+  }
+  B200_CUDA(cudaMemsetAsync(ctx->error.p, 0, sizeof(int), st));     // b200tts_wavernn_check reports this run
+  if (steps > 0) {
+    const PushModel& pm = ctx->pm;
+    const int G = push_rows(n);
+    const size_t nvec = (size_t)kPushVecs * 2 * pm.ncta * G * 4, nbest = (size_t)pm.ncta * G;
+    ctx->push_vec.ensure(nvec * sizeof(float));
+    ctx->push_best.ensure(nbest * sizeof(unsigned long long));
+    launch_push_init(ctx->push_vec.as<uint32_t>(), nvec, ctx->push_best.as<unsigned long long>(), nbest, nullptr, ctx->sm_count, st);
+    ctx->launches++;
+    PushArgs a{};
+    a.wblob = ctx->push_blob.as<float>();
+    a.vec = ctx->push_vec.as<float>();
+    a.best = ctx->push_best.as<unsigned long long>();
+    a.error = ctx->error.as<int>();
+    a.fir = ctx->d_fir;
+    a.NT = ctx->NT;
+    a.B = n; a.hop = ctx->cfg.hop_length; a.steps = steps;
+    a.rng_mode = B200TTS_RNG_PHILOX;
+    switch (G) {
+      case 8: launch_session_t<8>(ctx, a, io, st); break;
+      case 16: launch_session_t<16>(ctx, a, io, st); break;
+      default: launch_session_t<32>(ctx, a, io, st); break;
+    }
+    ctx->last_kernel = SK_SESSION;
+    ctx->prof_ncta = 0;
+    ctx->ev_valid = true;
+  }
+  if (d_wave) {
+    dim3 grid((max_steps + 255) / 256, n);
+    session_wave_kernel<<<grid, 256, 0, st>>>(io, ctx->cfg.hop_length, 20 * ctx->cfg.hop_length, ctx->NC, ctx->error.as<int>(), d_wave);
+    B200_CUDA(cudaGetLastError());
+    ctx->launches++;
+  }
+  for (int i = 0; i < n; ++i) s[i]->pos += io.row[i].n;     // at enqueue: the counts are known without a synchronisation
   API_END
 }
 

@@ -88,6 +88,26 @@ struct PushArgs {
   int pack_segs, pack_rows;      // kernel rows >= pack_rows are idle
 };
 
+// GENERATION SESSIONS (b200tts_wavernn_session_*, wavernn_push_session_kernel): row u of a launch resumes session u at its
+// position `pos` and runs `n` steps, a segment from lock-step 0 to n whose step within the utterance is pos + t; then it is idle.
+// At the end of its run a row saves what makes its next step exactly the one-shot run's next step: both GRU states, the two
+// recurrent projections W_hh . h as this CTA reduced them for the next step (12 rows per CTA) and the last label (the next x).
+// Saving the reduced projections instead of recomputing them keeps the summation order, hence the bits.  Needs R = 512 and
+// 128 CTAs (pm.ok).
+constexpr int kSessH1 = 0, kSessH2 = 512, kSessGh1 = 1024, kSessGh2 = kSessGh1 + 128 * 12, kSessLabel = kSessGh2 + 128 * 12;
+constexpr int kSessStateFloats = kSessLabel + 4;
+struct SessRow {
+  const float* tab;                 // [T+1][ncta][52] the session's conditioning tables
+  float* state;                     // [kSessStateFloats]; the label is stored as an int
+  unsigned long long seed, id;      // Philox key of the one-shot run: (seed, utterance id, step within the utterance)
+  int T, pos, n, mu_law;            // frames; first step of this run; steps of this run (0: idle row); wave decoding
+};
+struct SessIO {                     // passed by value, next to PushArgs (whose field offsets are left alone)
+  SessRow row[kPushMaxRows];
+  int16_t* labels;                  // [rows][ld]: the label of step pos + i of row u at labels[u * ld + i]
+  int ld;
+};
+
 struct PushRowState {            // per-row bookkeeping in shared memory (normal mode: row u == utterance u from step 0, forever)
   // current segment: utterance (-1 idle), first step, first step of the NEXT segment, index
   int utt[kPushMaxRows], t0[kPushMaxRows], end[kPushMaxRows], k[kPushMaxRows];
@@ -241,9 +261,10 @@ __device__ __forceinline__ float push_part_sum(const float* part, int r, int u) 
 // loads of an item in flight at once.  Rows 16-35 (GRU-2 12, fc1 4, fc2 4: aux projection + bias) are constant within a
 // frame -> push_cond20, refreshed only when the next step starts a new frame (every step in fold mode, where rows sit at
 // different phases).
-template <int G>
-__device__ __forceinline__ void push_cond16(const PushArgs& A, const PushRowState& R, const float* fir_s, float* cdst, int c, int ncta, int t,
-                                            int tid) {
+// SESS: the tables and frame count of row u are those of session u (SessIO).
+template <int G, bool SESS>
+__device__ __forceinline__ void push_cond16(const PushArgs& A, const PushRowState& R, const SessIO& sio, const float* fir_s, float* cdst,
+                                            int c, int ncta, int t, int tid) {
   const size_t fstride = (size_t)ncta * kPushCondRows;
   const int fr0 = t / A.hop, ph0 = t - fr0 * A.hop;                   // plain batch: every row is at the same frame / phase
   // items start at thread 4G: the gate threads (0 ... 4G-1) are busy with the fc2 gate, the re-arm and its fence at this point
@@ -257,20 +278,22 @@ __device__ __forceinline__ void push_cond16(const PushArgs& A, const PushRowStat
       beyond = n >= A.S_src;                                           // past the source utterance: zero mel and aux -> bias only
       fr = beyond ? A.T : (int)(n / A.hop);
       ph = beyond ? 0 : (int)(n - (long long)fr * A.hop);
-    } else if (A.pack_utt) {
+    } else if (SESS || A.pack_utt) {
       int n;
       push_row_next(A, R, u, t, src, n);
       if (src < 0) { cdst[r * G + u] = 0.f; continue; }                // idle row
       fr = n / A.hop;
       ph = n - fr * A.hop;
     }
-    const float* row = A.tab + (((size_t)src * (A.T + 1) + fr) * ncta + c) * kPushCondRows;
+    const int T = SESS ? sio.row[src].T : A.T;
+    const float* row = SESS ? sio.row[src].tab + ((size_t)fr * ncta + c) * kPushCondRows
+                            : A.tab + (((size_t)src * (A.T + 1) + fr) * ncta + c) * kPushCondRows;
     float v = __ldg(row + 16 + r);
     float pm[kMaxTaps];
 #pragma unroll
     for (int j = 0; j < kMaxTaps; ++j) {
       const int f = fr + j - A.NT / 2;
-      pm[j] = (!beyond && j < A.NT && f >= 0 && f < A.T) ? __ldg(row + ((ptrdiff_t)(f - fr)) * (ptrdiff_t)fstride + r) : 0.f;
+      pm[j] = (!beyond && j < A.NT && f >= 0 && f < T) ? __ldg(row + ((ptrdiff_t)(f - fr)) * (ptrdiff_t)fstride + r) : 0.f;
     }
 #pragma unroll
     for (int j = 0; j < kMaxTaps; ++j)
@@ -278,8 +301,9 @@ __device__ __forceinline__ void push_cond16(const PushArgs& A, const PushRowStat
     cdst[r * G + u] = v;
   }
 }
-template <int G>
-__device__ __forceinline__ void push_cond20(const PushArgs& A, const PushRowState& R, float* cdst, int c, int ncta, int t, int tid) {
+template <int G, bool SESS>
+__device__ __forceinline__ void push_cond20(const PushArgs& A, const PushRowState& R, const SessIO& sio, float* cdst, int c, int ncta, int t,
+                                            int tid) {
   const int fr0 = t / A.hop;
   for (int it = tid; it < 20 * G; it += kPushThreads) {
     const int u = it / 20, r = it - u * 20;
@@ -288,13 +312,14 @@ __device__ __forceinline__ void push_cond20(const PushArgs& A, const PushRowStat
       const long long n = (long long)u * A.row_stride + t;
       src = 0;
       fr = n >= A.S_src ? A.T : (int)(n / A.hop);
-    } else if (A.pack_utt) {
+    } else if (SESS || A.pack_utt) {
       int n;
       push_row_next(A, R, u, t, src, n);
       if (src < 0) { cdst[r * G + u] = 0.f; continue; }
       fr = n / A.hop;
     }
-    cdst[r * G + u] = __ldg(A.tab + (((size_t)src * (A.T + 1) + fr) * ncta + c) * kPushCondRows + 32 + r);
+    cdst[r * G + u] = SESS ? __ldg(sio.row[src].tab + ((size_t)fr * ncta + c) * kPushCondRows + 32 + r)
+                           : __ldg(A.tab + (((size_t)src * (A.T + 1) + fr) * ncta + c) * kPushCondRows + 32 + r);
   }
 }
 
@@ -303,15 +328,36 @@ __device__ __forceinline__ void push_cond20(const PushArgs& A, const PushRowStat
 // tag alone.  The words and the exchange protocol are RAW's; P01 gathers the 30 parameters instead of reducing the winners.
 template <int G>
 __global__ void __launch_bounds__(kPushThreads, 1) wavernn_push_kernel(PushModel M, PushArgs A) {
-  constexpr bool MOL = false;
+  constexpr bool MOL = false, SESS = false;
   [[maybe_unused]] const MolIO io{};
+  [[maybe_unused]] const SessIO sio{};
 #include "wavernn_push_step.cuh"
 }
 
 template <int G>
 __global__ void __launch_bounds__(kPushThreads, 1) wavernn_push_mol_kernel(PushModel M, PushArgs A, MolIO io) {
-  constexpr bool MOL = true;
+  constexpr bool MOL = true, SESS = false;
+  [[maybe_unused]] const SessIO sio{};
 #include "wavernn_push_step.cuh"
+}
+
+// RAW generation sessions: row u resumes session u of `sio` (see SessRow); A carries the shared buffers and B = rows.
+template <int G>
+__global__ void __launch_bounds__(kPushThreads, 1) wavernn_push_session_kernel(PushModel M, PushArgs A, SessIO sio) {
+  constexpr bool MOL = false, SESS = true;
+  [[maybe_unused]] const MolIO io{};
+#include "wavernn_push_step.cuh"
+}
+
+// The wave of one run of each session: samples [pos, pos + n) of its one-shot wave (finish_wave_kernel), i.e. mu-law decoded,
+// zero from (T-1)*hop on and faded over the 20 hops before; entries past n are zero.  wave [rows][ld].
+__global__ void session_wave_kernel(SessIO sio, int hop, int fade_len, int ncls, const int* __restrict__ gen_error,
+                                    double* __restrict__ wave) {
+  const int b = blockIdx.y;
+  const SessRow& r = sio.row[b];
+  const LabelSamples sample{sio.labels + (size_t)b * sio.ld, (double)(ncls - 1), ncls, r.mu_law};
+  const int wave_len = (r.T - 1) * hop;
+  finish_wave_range(sample, r.pos, r.n, wave_len, fade_len, gen_error, sio.ld, wave + (size_t)b * sio.ld);
 }
 
 // ---- conditioning tables: tab[u][f][c][52] for f in [0, T]; frame T carries the bias only (zero conditioning) ------------

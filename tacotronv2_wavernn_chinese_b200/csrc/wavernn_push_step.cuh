@@ -1,6 +1,7 @@
-// The body of wavernn_push_kernel<G> and wavernn_push_mol_kernel<G> (wavernn_push.cuh): included inside both kernels, with `MOL` (constexpr bool) and
-// `io` (MolIO) declared by the includer.  Each kernel is thus compiled from its own copy of the text, so the RAW kernel's code
-// is exactly what it was before MOL existed; `if constexpr (MOL)` selects the sampler.  Not a standalone header.
+// The body of wavernn_push_kernel<G>, wavernn_push_mol_kernel<G> and wavernn_push_session_kernel<G> (wavernn_push.cuh): included
+// inside each kernel, with `MOL`, `SESS` (constexpr bool), `io` (MolIO) and `sio` (SessIO) declared by the includer.  Each kernel
+// is thus compiled from its own copy of the text, so the RAW kernel's code is exactly what it was before MOL and sessions
+// existed; `if constexpr (MOL)` selects the sampler, `SESS` the per-session rows, state and addressing.  Not a standalone header.
   using PT = PushTraits<G>;
   constexpr int NU = PT::NU;
   extern __shared__ __align__(16) float smem[];
@@ -47,12 +48,28 @@
     if (!A.pack_utt) {                                     // plain batch / folds: row u is utterance u from step 0 to the end
       R.k[tid] = 0; R.utt[tid] = tid < A.B ? tid : -1; R.end[tid] = 0x7fffffff;
     }
+    if constexpr (SESS) {                                  // row u: session u from step pos (t0 = -pos) for n lock-steps
+      const bool live = tid < A.B && sio.row[tid].n > 0;
+      R.utt[tid] = live ? tid : -1;
+      R.t0[tid] = live ? -sio.row[tid].pos : 0;
+      R.end[tid] = live ? sio.row[tid].n : 0x7fffffff;
+      R.rst[tid] = (!live || sio.row[tid].pos == 0) ? 1 : 0;  // position 0 starts from the zero state, as a one-shot run
+    }
   }
   __syncthreads();
+  if constexpr (SESS) {                                    // a resumed row: the projections its previous run saved
+    for (int i = tid; i < 12 * G; i += kPushThreads) {
+      const int u = i % G;
+      if (R.utt[u] >= 0 && !R.rst[u]) {
+        gh1[i] = sio.row[u].state[kSessGh1 + c * 12 + i / G];
+        gh2[i] = sio.row[u].state[kSessGh2 + c * 12 + i / G];
+      }
+    }
+  }
   float* cond16 = cond;                       // [2][16][G]  rows 0-15 of step t (parity buffers, written one step ahead)
   float* cond20 = cond + 2 * 16 * G;          // [20][G]     rows 16-35 of the current frame
-  push_cond16<G>(A, R, fir_s, cond16, c, ncta, 0, tid);
-  push_cond20<G>(A, R, cond20, c, ncta, 0, tid);
+  push_cond16<G, SESS>(A, R, sio, fir_s, cond16, c, ncta, 0, tid);
+  push_cond20<G, SESS>(A, R, sio, cond20, c, ncta, 0, tid);
   __syncthreads();
   if (A.pack_utt && tid < G) {                             // enter segment 0 (kernel rows beyond the schedule stay idle)
     const bool live = tid < A.pack_rows && A.pack_segs > 0;
@@ -65,6 +82,15 @@
 
   PollGuard pg{A.error, 0, 0, false};
   float h1own = 0.f, h2own = 0.f;                          // gate threads: state of unit 4c+gj, row gu
+  [[maybe_unused]] float x_resume = 0.f;                   // SESS: x of a resumed row's first step (its last label)
+  if constexpr (SESS) {
+    if (gate && R.utt[gu] >= 0 && !R.rst[gu]) {
+      const float* st = sio.row[gu].state;
+      h1own = st[kSessH1 + 4 * c + gj];
+      h2own = st[kSessH2 + 4 * c + gj];
+      x_resume = label_to_float(reinterpret_cast<const int*>(st)[kSessLabel], ncls_m1);
+    }
+  }
   __shared__ long long s_pf[12];                           // optional per-phase cycle counters of thread 0 (debug)
   __shared__ long long s_tmark;
   if (tid == 0) {
@@ -86,6 +112,9 @@
     const int par = t & 1;
     // ================= P01: winners of step t-1 -> label -> GRU 1 =================
     float x = 0.f;
+    if constexpr (SESS) {
+      if (t == 0) x = x_resume;
+    }
     if (t > 0) {
       const unsigned long long want = (unsigned long long)((uint32_t)t & 0x3FFFFFu);
       unsigned long long rec[NREC];
@@ -143,7 +172,14 @@
         const int label = (int)push_cls(b);
         const int putt = R.putt[gu], pn = R.pn[gu];         // where this row was at step t-1
         if (putt >= 0) {
-          if (c == 0 && gj == 0) A.labels[(size_t)putt * A.S + pn] = (int16_t)label;
+          if (c == 0 && gj == 0) {
+            if constexpr (SESS) {
+              sio.labels[(size_t)putt * sio.ld + (pn - sio.row[putt].pos)] = (int16_t)label;
+              reinterpret_cast<int*>(sio.row[putt].state)[kSessLabel] = label;
+            } else {
+              A.labels[(size_t)putt * A.S + pn] = (int16_t)label;
+            }
+          }
           const int fb = A.teacher ? (int)A.teacher[(size_t)putt * A.S + pn] : label;
           x = label_to_float(fb, ncls_m1);
         }
@@ -199,6 +235,12 @@
                                  push_part_sum<G, 16>(partX, 8 + gj, gu) + cd[(8 + gj) * G + gu], g2r + bhh[gj], g2z + bhh[4 + gj],
                                  g2n + bhh[8 + gj], h2own);
       h2own = h;
+      if constexpr (SESS) {
+        if (R.utt[gu] >= 0 && t + 1 == R.end[gu]) {      // the row's last step of this run: save its state
+          sio.row[gu].state[kSessH1 + 4 * c + gj] = h1own;
+          sio.row[gu].state[kSessH2 + 4 * c + gj] = h2own;
+        }
+      }
       f1x = push_part_sum<G, 16>(partX, 12 + gj, gu);
       st_relaxed_f32(vecp(PV_H2, par) + ((size_t)c * G + gu) * 4 + gj, h);
     }
@@ -226,7 +268,16 @@
       push_mma<G, 12>(Wb + M.ohh2, a, partY, ul, kq, warp, lane);
     }
     if (__syncthreads_or(pg.aborted ? 1 : 0)) return;
-    for (int i = tid; i < 12 * G; i += kPushThreads) gh2[i] = push_part_sum<G, 12>(partY, i / G, i % G);
+    for (int i = tid; i < 12 * G; i += kPushThreads) {
+      gh2[i] = push_part_sum<G, 12>(partY, i / G, i % G);
+      if constexpr (SESS) {                                   // this thread also wrote gh1[i] above (same mapping)
+        const int u = i % G;
+        if (R.utt[u] >= 0 && t + 1 == R.end[u]) {
+          sio.row[u].state[kSessGh1 + c * 12 + i / G] = gh1[i];
+          sio.row[u].state[kSessGh2 + c * 12 + i / G] = gh2[i];
+        }
+      }
+    }
     PUSH_MARK(6);
 
     // ================= P4: fc2 + relu on f1(t) =================
@@ -252,8 +303,8 @@
     __syncwarp();
     // shadow: conditioning of step t+1 (rows 0-15 into the other parity buffer; rows 16-35 only when a new frame starts)
     if (t + 1 < A.steps) {
-      push_cond16<G>(A, R, fir_s, cond16 + (par ^ 1) * 16 * G, c, ncta, t + 1, tid);
-      if (A.row_stride || A.pack_utt || (t + 1) % A.hop == 0) push_cond20<G>(A, R, cond20, c, ncta, t + 1, tid);
+      push_cond16<G, SESS>(A, R, sio, fir_s, cond16 + (par ^ 1) * 16 * G, c, ncta, t + 1, tid);
+      if (SESS || A.row_stride || A.pack_utt || (t + 1) % A.hop == 0) push_cond20<G, SESS>(A, R, sio, cond20, c, ncta, t + 1, tid);
     }
     PUSH_MARK(8);
 
@@ -277,7 +328,11 @@
       float qv = 1.0f;
       const int utt = R.utt[u], n = t - R.t0[u];               // plain batch: utt == u, n == t
       if (utt >= 0) {
-        if (A.rng_mode == 0) {
+        if (SESS) {                                              // the session's key; n is the step within the utterance
+          float q4[4];
+          philox_exp4(sio.row[utt].seed, sio.row[utt].id, (uint32_t)n, (uint32_t)(cls >> 2), q4);
+          qv = q4[cls & 3];
+        } else if (A.rng_mode == 0) {
           float q4[4];
           philox_exp4(A.seed, A.utt_ids ? A.utt_ids[utt] : A.utt_offset + (unsigned long long)utt, (uint32_t)n, (uint32_t)(cls >> 2), q4);
           qv = q4[cls & 3];

@@ -236,6 +236,14 @@ __device__ __forceinline__ void xfade_unfold(const Samples& sample /*[nfold][L]*
   }
 }
 
+// Sample i < wave_len of the wave after the 20-hop linear fade-out over its last fade_len samples (fatchord_version.py:256-258);
+// step = -1 / (fade_len - 1), np.linspace(1, 0, fade_len).  Elementwise in i, so a piece of the wave is faded like the whole.
+__device__ __forceinline__ double fade_tail(double y, int i, int wave_len, int fade_len, double step) {
+  int k = i - (wave_len - fade_len);
+  if (k >= 0) y *= (k == fade_len - 1) ? 0.0 : (1.0 + (double)k * step);
+  return y;
+}
+
 // generate() epilogue (fatchord_version.py:243-258): float64, truncate, 20-hop fade.
 // `utt_frames` (optional, [B]): true frame count of each row of a zero-padded ragged batch -> that row is truncated / faded at
 // ITS OWN (T_b - 1) * hop like a batch-1 run of the reference, and zero beyond.
@@ -249,10 +257,22 @@ __device__ __forceinline__ void finish_wave(const Samples& sample /*[B][S]*/, in
   const int wave_len = utt_frames ? min(wave_len_max, max(0, (utt_frames[b] - 1) * hop)) : wave_len_max;
   for (int i = blockIdx.x * blockDim.x + threadIdx.x; i < wave_len_max; i += gridDim.x * blockDim.x) {
     if (i >= wave_len) { wave[(size_t)b * wave_len_max + i] = 0.0; continue; }
-    double y = sample((size_t)b * S + i);
-    int k = i - (wave_len - fade_len);
-    if (k >= 0) y *= (k == fade_len - 1) ? 0.0 : (1.0 + (double)k * step);
+    const double y = fade_tail(sample((size_t)b * S + i), i, wave_len, fade_len, step);
     wave[(size_t)b * wave_len_max + i] = poisoned ? nan("") : y;
+  }
+}
+
+// The same epilogue over samples [first, first + n) of one utterance whose stored samples are sample(0 ... n-1): wave[i] is
+// sample first + i of the whole wave, zero from wave_len on and for i >= n (up to ld).
+template <class Samples>
+__device__ __forceinline__ void finish_wave_range(const Samples& sample, int first, int n, int wave_len, int fade_len,
+                                                  const int* __restrict__ gen_error, int ld, double* __restrict__ wave /*[ld]*/) {
+  const bool poisoned = gen_error && *gen_error;
+  const double step = -1.0 / (double)(fade_len - 1);
+  for (int i = blockIdx.x * blockDim.x + threadIdx.x; i < ld; i += gridDim.x * blockDim.x) {
+    if (i >= n || first + i >= wave_len) { wave[i] = 0.0; continue; }     // (first + i < first + n <= S: no overflow)
+    const double y = fade_tail(sample((size_t)i), first + i, wave_len, fade_len, step);
+    wave[i] = poisoned ? nan("") : y;
   }
 }
 

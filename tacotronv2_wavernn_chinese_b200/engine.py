@@ -6,6 +6,7 @@ csrc/ through the C ABI.  Tensors in, tensors out.
 from __future__ import annotations
 
 import ctypes as C
+import weakref
 
 import numpy as np
 import torch
@@ -67,9 +68,12 @@ class WaveRNNEngine:
         _lib.check(create(C.byref(h), self.device, C.byref(cfg), arr, len(arr)))
         del keep
         self._h = h
+        self._sessions = weakref.WeakSet()
 
     def close(self):
         if getattr(self, '_h', None):
+            for s in list(self._sessions):      # the context frees its open sessions
+                s._h = None
             self.lib.b200tts_wavernn_destroy(self._h)
             self._h = None
 
@@ -208,6 +212,51 @@ class WaveRNNEngine:
                 t.record_stream(torch.cuda.current_stream(self.device))
         return {'samples' if mol else 'labels': out, 'wave': wave, 'logits': logits, 'steps': steps}
 
+    def open_session(self, mel, *, seed: int = 0, utterance_id: int = 0, mu_law: bool = True) -> 'WaveRNNSession':
+        """A generation session of one RAW utterance: mel [feat, T] (T >= 21) in [0, 1].  Its sample loop then runs in pieces
+        (`advance`), and the pieces, concatenated, are bit for bit `generate(mel[None], seed=seed, utterance_ids=[utterance_id])`.
+        The conditioning is computed here, once, on the current stream."""
+        m = torch.as_tensor(mel)
+        if m.dim() != 2 or m.shape[0] != self.feat:
+            raise ValueError(f'mel must be [{self.feat}, T], got {tuple(m.shape)}')
+        with torch.cuda.device(self.device):
+            m = m.to(device=self._dev(), dtype=torch.float32).contiguous()
+            rng = Rng()
+            rng.mode = _lib.RNG_PHILOX
+            rng.seed = int(seed) & 0xFFFFFFFFFFFFFFFF
+            rng.utterance_offset = int(utterance_id) & 0xFFFFFFFFFFFFFFFF
+            h = C.c_void_p()
+            _lib.check(self.lib.b200tts_wavernn_session_open(self._h, _ptr(m), int(m.shape[1]), C.byref(rng), 1 if mu_law else 0,
+                                                             C.byref(h), self._stream()))
+            m.record_stream(torch.cuda.current_stream(self.device))
+        s = WaveRNNSession(self, h)
+        self._sessions.add(s)
+        return s
+
+    def advance(self, sessions, max_steps: int):
+        """Runs up to `max_steps` more steps of each session (1..32 distinct open sessions of this engine) in one launch.
+        Returns, for each session, (labels int16 [n], wave float64 [w]) cuda tensors: its n = min(max_steps, steps - position)
+        labels from its old position, and the w samples of its wave among them (none past wave_len)."""
+        sessions = list(sessions)
+        if any(s._h is None for s in sessions):
+            raise ValueError('a session is closed')
+        max_steps = int(max_steps)
+        n = len(sessions)
+        info = [(s.position, s.steps, s.wave_len) for s in sessions]
+        dev = self._dev()
+        with torch.cuda.device(self.device):
+            rows = max(n, 1)
+            labels = torch.empty(rows, max(max_steps, 1), device=dev, dtype=torch.int16)
+            wave = torch.empty(rows, max(max_steps, 1), device=dev, dtype=torch.float64)
+            handles = (C.c_void_p * rows)(*[s._h.value for s in sessions])
+            _lib.check(self.lib.b200tts_wavernn_session_run(self._h, handles, n, max_steps, _ptr(labels), _ptr(wave), self._stream()))
+        out = []
+        for i, (pos, steps, wave_len) in enumerate(info):
+            k = min(max_steps, steps - pos)
+            w = max(0, min(pos + k, wave_len) - pos)
+            out.append((labels[i, :k], wave[i, :w]))
+        return out
+
     def fold_geometry(self, T: int, target: int, overlap: int):
         """(n_folds, fold_len) of fold_with_overlap for a T-frame utterance."""
         nf, fl = C.c_int(), C.c_int()
@@ -275,7 +324,8 @@ class WaveRNNEngine:
     def launch_count(self) -> int:
         return int(self.lib.b200tts_wavernn_launch_count(self._h))
 
-    KERNEL_NAMES = {0: None, 1: 'wavernn_utt_kernel', 2: 'wavernn_grid_kernel', 3: 'wavernn_push_kernel', 5: 'wavernn_tc_kernel'}
+    KERNEL_NAMES = {0: None, 1: 'wavernn_utt_kernel', 2: 'wavernn_grid_kernel', 3: 'wavernn_push_kernel', 5: 'wavernn_tc_kernel',
+                    6: 'wavernn_push_session_kernel'}
 
     def last_kernel(self):
         """Name of the step kernel the last generate call ran."""
@@ -286,3 +336,57 @@ class WaveRNNEngine:
         if ms < 0:
             raise _lib.B200TTSError(-1, self.lib.b200tts_last_error().decode())
         return ms
+
+
+class WaveRNNSession:
+    """One RAW utterance whose sample loop runs in pieces (WaveRNNEngine.open_session / advance).  A context manager; close()
+    frees its device memory (closing the engine frees it too)."""
+
+    def __init__(self, engine: WaveRNNEngine, handle):
+        self.engine = engine
+        self._h = handle
+
+    def _info(self):
+        if self._h is None:
+            raise ValueError('the session is closed')
+        pos, steps, wave_len = C.c_int64(), C.c_int64(), C.c_int64()
+        _lib.check(self.engine.lib.b200tts_wavernn_session_info(self._h, C.byref(pos), C.byref(steps), C.byref(wave_len)))
+        return pos.value, steps.value, wave_len.value
+
+    @property
+    def position(self) -> int:
+        """Steps generated so far (counted when a run is enqueued)."""
+        return self._info()[0]
+
+    @property
+    def steps(self) -> int:
+        """Steps of the utterance, T * hop."""
+        return self._info()[1]
+
+    @property
+    def wave_len(self) -> int:
+        """Samples of its wave, (T - 1) * hop."""
+        return self._info()[2]
+
+    @property
+    def done(self) -> bool:
+        pos, steps, _ = self._info()
+        return pos >= steps
+
+    def close(self):
+        if self._h is not None:
+            self.engine.lib.b200tts_wavernn_session_destroy(self._h)
+            self._h = None
+            self.engine._sessions.discard(self)
+
+    def __enter__(self):
+        return self
+
+    def __exit__(self, *exc):
+        self.close()
+
+    def __del__(self):
+        try:
+            self.close()
+        except Exception:
+            pass

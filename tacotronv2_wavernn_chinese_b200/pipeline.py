@@ -16,10 +16,16 @@ and below ~32 rows it barely depends on the row count at all, so
     length profile and the makespan is the longest sentence's;
   * the sampling noise and the prenet dropout are keyed by the GLOBAL sentence index (`rng.d_utterance_ids`), so a
     sentence's audio depends neither on the chunking nor on the number of ranks.
+For a service, where the time to the first audio matters more than the makespan, StreamingVocoder runs generation SESSIONS
+(engine.open_session / advance): every utterance advances by `chunk_steps` samples per launch, its piece of wave is handed out
+after each launch, finished utterances leave and queued ones take their rows between launches (continuous batching).  The
+pieces of an utterance concatenate to exactly the wave vocode_ragged gives it.
 Tacotron itself is replicated on every rank: one thread block decodes one sentence, all sentences of a set decode
 concurrently (<= 132 per GPU), so sharding it would not shorten anything -- and it removes the mel exchange.
 """
 from __future__ import annotations
+
+import collections
 
 import numpy as np
 import torch
@@ -175,3 +181,81 @@ def synthesize_sharded(synth, wavernn_engine, texts, seed=0, group=None, kernel=
         for k, i in enumerate(share):
             out[i] = host[k, :lens[i]].copy()
     return out, list(mels)
+
+
+def _host(x):
+    return x.cpu().numpy() if hasattr(x, 'cpu') else np.asarray(x)
+
+
+class StreamingVocoder:
+    """Continuous batching of vocoder sessions on one engine.  `submit` queues requests; every `step` admits queued requests
+    first come first served into free rows (at most `max_rows` <= 32 sessions per launch), advances every session by up to
+    `chunk_steps` samples in one launch and returns [(key, wave piece float64 numpy, finished)].  A key's pieces concatenate to
+    the wave vocode_ragged gives its mel with the same seed and id; mels shorter than MIN_FRAMES are zero-padded to it, as there."""
+
+    def __init__(self, engine, seed=0, chunk_steps=2750, max_rows=32):
+        if not 1 <= int(max_rows) <= 32:
+            raise ValueError('max_rows must be 1..32 (the push kernel runs at most 32 sessions per launch)')
+        if int(chunk_steps) < 1:
+            raise ValueError('chunk_steps must be >= 1')
+        self.engine, self.seed = engine, int(seed)
+        self.chunk_steps, self.max_rows = int(chunk_steps), int(max_rows)
+        self._queue = collections.deque()       # (key, mel [T, feat], utterance id)
+        self._active = []                       # (key, session) in admission order
+
+    def submit(self, key, mel, utterance_id):
+        """Queues mel [T, feat] in [0, 1]; the sampling noise is keyed by (seed, utterance_id) like a one-shot run."""
+        m = np.asarray(mel, dtype=np.float32)
+        if m.ndim != 2:
+            raise ValueError(f'mel must be [T, feat], got {m.shape}')
+        self._queue.append((key, m, int(utterance_id)))
+
+    @property
+    def pending(self) -> int:
+        return len(self._queue)
+
+    @property
+    def active(self) -> int:
+        return len(self._active)
+
+    def idle(self) -> bool:
+        return not self._queue and not self._active
+
+    def step(self):
+        while self._queue and len(self._active) < self.max_rows:
+            key, m, uid = self._queue.popleft()
+            T = max(m.shape[0], MIN_FRAMES)
+            padded = np.zeros((m.shape[1], T), dtype=np.float32)         # zero frames past the end, as vocode_ragged pads
+            padded[:, :m.shape[0]] = m.T
+            self._active.append((key, self.engine.open_session(padded, seed=self.seed, utterance_id=uid)))
+        if not self._active:
+            return []
+        pieces = self.engine.advance([s for _, s in self._active], self.chunk_steps)
+        out, still = [], []
+        for (key, s), (_labels, wave) in zip(self._active, pieces):
+            finished = s.done
+            out.append((key, _host(wave), finished))
+            if finished:
+                s.close()
+            else:
+                still.append((key, s))
+        self._active = still
+        check = getattr(self.engine, 'check', None)
+        if check is not None:
+            check()                              # a timed-out run raises here instead of handing out NaN audio
+        return out
+
+
+def synthesize_stream(synth, wavernn_engine, text, seed=0, utterance_id=0, chunk_steps=2750):
+    """One sentence as a stream: yields its Tacotron mel [T, 80] first, then its wave pieces (float64 numpy) as the vocoder
+    makes them.  The pieces concatenate to synthesize_batch's wave of the sentence with utterance_offset = utterance_id."""
+    mels, _ = synth.mels([text], seed=seed, utterance_offset=utterance_id)
+    mel = mels[0]
+    yield mel
+    sv = StreamingVocoder(wavernn_engine, seed=seed, chunk_steps=chunk_steps, max_rows=1)
+    sv.submit(0, mel, utterance_id)
+    while True:
+        for _key, piece, finished in sv.step():
+            yield piece
+            if finished:
+                return
