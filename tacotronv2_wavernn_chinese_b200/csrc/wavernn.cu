@@ -332,6 +332,13 @@ extern "C" int64_t b200tts_wavernn_launch_count(const b200tts_wavernn* ctx) { re
 
 extern "C" int b200tts_wavernn_last_kernel(const b200tts_wavernn* ctx) { return ctx ? ctx->last_kernel : 0; }
 
+// After the stream has been synchronised: did a kernel of the last generate call or session run give up waiting for a peer CTA?
+static void check_call_error(b200tts_wavernn* ctx) {
+  int flag = 0;
+  B200_CUDA(cudaMemcpy(&flag, ctx->error.p, sizeof(int), cudaMemcpyDeviceToHost));
+  REQUIRE(flag == 0, B200TTS_ECUDA, "grid kernel: a grid-barrier wait timed out (co-resident CTA missing); results are invalid");
+}
+
 extern "C" double b200tts_wavernn_last_kernel_ms(b200tts_wavernn* ctx) {
   if (!ctx || !ctx->ev_valid) {
     g_err = "no generate call has been timed on this context";
@@ -344,9 +351,10 @@ extern "C" double b200tts_wavernn_last_kernel_ms(b200tts_wavernn* ctx) {
     g_err = std::string("cudaEventElapsedTime: ") + cudaGetErrorString(e);
     return -1.0;
   }
-  int flag = 0;
-  if (cudaMemcpy(&flag, ctx->error.p, sizeof(int), cudaMemcpyDeviceToHost) == cudaSuccess && flag) {
-    g_err = "grid kernel: a grid-barrier wait timed out (co-resident CTA missing); results are invalid";
+  try {
+    check_call_error(ctx);
+  } catch (const Error& err) {
+    g_err = err.what();
     return -1.0;
   }
   return (double)ms;
@@ -411,48 +419,46 @@ static void copy_gen_fields(Args& a, const GenArgs& g) {
   a.teacher = g.teacher; a.logits_out = g.logits_out; a.labels = g.labels;
 }
 
-// Zeroed phase counters [ncta][12] for the launch when `prof`, else null; records what the launch will leave in ctx->prof.
+// Zeroed phase counters [ncta][12] for the launch when `prof`, else null.
 static long long* phase_counters(b200tts_wavernn* ctx, bool prof, int ncta, cudaStream_t st) {
   if (!prof) return nullptr;
   const size_t bytes = (size_t)ncta * 12 * sizeof(long long);
   ctx->prof.ensure(bytes);
   B200_CUDA(cudaMemsetAsync(ctx->prof.p, 0, bytes, st));
-  ctx->prof_ncta = ncta;
   return ctx->prof.as<long long>();
 }
 
-// Cooperative launch of a persistent step kernel whose `ncta` CTAs must all be resident at once, timed by ev0 / ev1.
-static void coop_launch(b200tts_wavernn* ctx, const void* kern, const char* what, int ncta, int threads, size_t smem, void** args,
-                        cudaStream_t st) {
+// Launches `kern`, step kernel `sk` of a generate call or session run, on `grid` CTAs, timed by ev0 / ev1 (`prof`: it fills
+// the phase counters), and records what b200tts_wavernn_last_kernel, _last_kernel_ms and _debug_phase_cycles report.  The
+// kernel is recorded before the checks here, so a call they refuse reports the kernel it chose; nothing between a call's
+// choice of kernel and this launch refuses.  Every step kernel but the utterance kernel keeps all its CTAs resident at once
+// and is launched cooperatively.  `args` may hold more arguments than the kernel takes.
+static void launch_step(b200tts_wavernn* ctx, StepKernel sk, const void* kern, const char* what, int grid, int threads, size_t smem,
+                        void** args, bool prof, cudaStream_t st) {
+  ctx->last_kernel = sk;
+  ctx->prof_ncta = prof ? grid : 0;
+  const bool coop = sk != SK_UTTERANCE;
+  REQUIRE(coop || smem <= 227 * 1024, B200TTS_EINVAL, "model too large for the utterance kernel's shared memory");
   B200_CUDA(cudaFuncSetAttribute(kern, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)smem));
   int per_sm = 0;
-  B200_CUDA(cudaOccupancyMaxActiveBlocksPerMultiprocessor(&per_sm, kern, threads, smem));
-  REQUIRE(per_sm * ctx->sm_count >= ncta, B200TTS_EINVAL, std::string(what) + " cannot be made co-resident on this device");
+  if (coop) B200_CUDA(cudaOccupancyMaxActiveBlocksPerMultiprocessor(&per_sm, kern, threads, smem));
+  REQUIRE(!coop || per_sm * ctx->sm_count >= grid, B200TTS_EINVAL, std::string(what) + " cannot be made co-resident on this device");
   B200_CUDA(cudaEventRecord(ctx->ev0, st));
-  B200_CUDA(cudaLaunchCooperativeKernel(kern, dim3(ncta), dim3(threads), args, smem, st));
+  if (coop) B200_CUDA(cudaLaunchCooperativeKernel(kern, dim3(grid), dim3(threads), args, smem, st));
+  else B200_CUDA(cudaLaunchKernel(kern, dim3(grid), dim3(threads), args, smem, st));
   ctx->launches++;
   B200_CUDA(cudaEventRecord(ctx->ev1, st));
+  ctx->ev_valid = true;
 }
 
 template <int G>
-static void launch_utt(b200tts_wavernn* ctx, const GenArgs& a, const MolIO* mol, cudaStream_t st) {
-  const StepWeights& w = ctx->sw;
-  size_t fl = (size_t)G * (w.ldI + w.R + 4 * w.R + 2 * (w.R + w.aux) + (w.F + w.aux) + w.F + w.NC);
-  size_t smem = fl * sizeof(float);
-  REQUIRE(smem <= 227 * 1024, B200TTS_EINVAL, "model too large for the utterance kernel's shared memory");
-  int grid = (a.B + G - 1) / G;
-  if (mol) {
-    B200_CUDA(cudaFuncSetAttribute(wavernn_utt_mol_kernel<G>, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)smem));
-    B200_CUDA(cudaEventRecord(ctx->ev0, st));
-    wavernn_utt_mol_kernel<G><<<grid, kUttThreads, smem, st>>>(w, a, *mol);
-  } else {
-    B200_CUDA(cudaFuncSetAttribute(wavernn_utt_kernel<G>, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)smem));
-    B200_CUDA(cudaEventRecord(ctx->ev0, st));
-    wavernn_utt_kernel<G><<<grid, kUttThreads, smem, st>>>(w, a);
-  }
-  B200_CUDA(cudaGetLastError());
-  ctx->launches++;
-  B200_CUDA(cudaEventRecord(ctx->ev1, st));
+static void launch_utt(b200tts_wavernn* ctx, GenArgs& a, const MolIO* mol, cudaStream_t st) {
+  StepWeights w = ctx->sw;
+  MolIO io = mol ? *mol : MolIO{};
+  void* args[] = {(void*)&w, (void*)&a, (void*)&io};
+  const void* kern = mol ? (const void*)wavernn_utt_mol_kernel<G> : (const void*)wavernn_utt_kernel<G>;
+  launch_step(ctx, SK_UTTERANCE, kern, "utterance kernel", (a.B + G - 1) / G, kUttThreads, utt_smem_floats(w, G) * sizeof(float),
+              args, false, st);
 }
 
 struct FoldGeom {           // fold_with_overlap geometry (fatchord_version.py:319-330)
@@ -507,10 +513,8 @@ static void launch_grid_t(b200tts_wavernn* ctx, GridArgs& a, const MolIO* mol, c
   size_t smem = ((size_t)gm.blob + (size_t)MT::kScratchFloats) * sizeof(float);
   MolIO io = mol ? *mol : MolIO{};
   void* args[] = {(void*)&gm, (void*)&a, (void*)&io};
-  if (mol)
-    coop_launch(ctx, (const void*)wavernn_grid_mol_kernel<U, UW, GROUPS>, "grid kernel", gm.ncta, MT::NW * 32, smem, args, st);
-  else
-    coop_launch(ctx, (const void*)wavernn_grid_kernel<U, UW, GROUPS>, "grid kernel", gm.ncta, MT::NW * 32, smem, args, st);
+  const void* kern = mol ? (const void*)wavernn_grid_mol_kernel<U, UW, GROUPS> : (const void*)wavernn_grid_kernel<U, UW, GROUPS>;
+  launch_step(ctx, SK_GRID, kern, "grid kernel", gm.ncta, MT::NW * 32, smem, args, a.prof != nullptr, st);
 }
 
 // Mapping for B utterances: returns the padded batch; variant = index into the dispatch table below.
@@ -595,55 +599,42 @@ static void launch_grid(b200tts_wavernn* ctx, const float* d_mel, const GenArgs&
 }
 
 // Conditioning tables [tab_rows][T+1][ncta][52] of the push and tensor-core kernels from the first `src_rows` utterances of the
-// mels / frame-rate aux; table rows past them are zero.
-// `dst` (optional): the tables go there instead of the context's scratch ctx->push_tab.
+// mels / frame-rate aux, into `dst`, which is sized to hold them; table rows past the utterances are zero.
 static const float* launch_cond_table(b200tts_wavernn* ctx, const float* d_mel, const float* aux_frames, int src_rows, int tab_rows,
-                                      int T, cudaStream_t st, float* dst = nullptr) {
+                                      int T, DeviceBuf& dst, cudaStream_t st) {
   const b200tts_wavernn_cfg& c = ctx->cfg;
   constexpr int FT = 8;
-  if (!dst) {
-    ctx->push_tab.ensure((size_t)tab_rows * (T + 1) * ctx->pm.ncta * kPushCondRows * sizeof(float));
-    dst = ctx->push_tab.as<float>();
-  }
+  dst.ensure((size_t)tab_rows * (T + 1) * ctx->pm.ncta * kPushCondRows * sizeof(float));
   dim3 grid((T + 1 + FT - 1) / FT, tab_rows);
   size_t smem = (size_t)(c.feat_dims + c.res_out_dims) * FT * sizeof(float);
-  push_cond_table_kernel<FT><<<grid, 256, smem, st>>>(ctx->pcw, d_mel, aux_frames, src_rows, T, dst);
+  push_cond_table_kernel<FT><<<grid, 256, smem, st>>>(ctx->pcw, d_mel, aux_frames, src_rows, T, dst.as<float>());
   B200_CUDA(cudaGetLastError());
   ctx->launches++;
-  return dst;
+  return dst.as<float>();
 }
 
 // ---- small-batch push kernel (wavernn_push.cuh) --------------------------------------------------------------------------
-template <int G>
-static void launch_push_t(b200tts_wavernn* ctx, PushArgs& a, const MolIO* mol, cudaStream_t st) {
-  PushModel pm = ctx->pm;
-  size_t smem = ((size_t)pm.blob + (size_t)PushTraits<G>::scratch_floats(a.hop, a.NT)) * sizeof(float);
-  MolIO io = mol ? *mol : MolIO{};
-  void* args[] = {(void*)&pm, (void*)&a, (void*)&io};
-  if (mol) coop_launch(ctx, (const void*)wavernn_push_mol_kernel<G>, "push kernel", pm.ncta, kPushThreads, smem, args, st);
-  else coop_launch(ctx, (const void*)wavernn_push_kernel<G>, "push kernel", pm.ncta, kPushThreads, smem, args, st);
-}
-
 // rows of the push kernel variant: up to 8 rows run the 8-row variant (on the previous GPU a 4-row variant was slower, its
 // 64 hot L2 lines being polled by 65 536 threads)
 static inline int push_rows(int B) { return B <= 8 ? 8 : (B <= 16 ? 16 : kPushMaxRows); }
 
-// `fold` != null: rows are the folds of ONE source utterance of T0 frames (conditioning tables of utterance 0, row u
-// starts at sample u * stride); otherwise row u is utterance u.
-struct PackInfo {            // gen_opts.d_pack_*: kernel rows run queues of utterances
-  const int* utt;
-  const int* start;
-  int rows, segs, steps, n_utt;
-};
-static void launch_push(b200tts_wavernn* ctx, const float* d_mel, const GenArgs& ua, const MolIO* mol, bool prof, cudaStream_t st,
-                        const FoldGeom* fold, int T0, const PackInfo* pack) {
-  const PushModel& pm = ctx->pm;
-  const int rows = pack ? pack->rows : ua.B;
+// What a push launch runs: a RAW or a MOL generate call, or a run of RAW generation sessions.
+enum class PushFlavour { RAW, MOL, SESSION };
+
+// The G-row push kernel of `f`, and the floats of shared memory it needs past the weight blob.
+template <int G>
+static const void* push_kernel(PushFlavour f, int hop, int NT, size_t* scratch_floats) {
+  *scratch_floats = PushTraits<G>::scratch_floats(hop, NT);
+  if (f == PushFlavour::MOL) return (const void*)wavernn_push_mol_kernel<G>;
+  if (f == PushFlavour::SESSION) return (const void*)wavernn_push_session_kernel<G>;
+  return (const void*)wavernn_push_kernel<G>;
+}
+
+// Launches the push kernel of `f` on `rows` rows, with `io` (MolIO or SessIO; the RAW kernel takes none) as its third argument.
+// `a` comes with the fields of its flavour set; this arms the exchange buffers and sets the fields every push launch shares.
+static void launch_push_kernel(b200tts_wavernn* ctx, PushFlavour f, int rows, PushArgs& a, void* io, bool prof, cudaStream_t st) {
+  PushModel pm = ctx->pm;
   const int G = push_rows(rows);
-  const int T = fold ? T0 : ua.T, hop = ctx->cfg.hop_length;
-  const int tab_rows = fold ? 1 : (pack ? pack->n_utt : G), src_rows = fold ? 1 : (pack ? pack->n_utt : rows);
-  PushArgs a{};
-  a.tab = launch_cond_table(ctx, d_mel, ua.aux_frames, src_rows, tab_rows, T, st);
   const size_t nvec = (size_t)kPushVecs * 2 * pm.ncta * G * 4, nbest = (size_t)pm.ncta * G;
   ctx->push_vec.ensure(nvec * sizeof(float));
   ctx->push_best.ensure(nbest * sizeof(unsigned long long));
@@ -655,17 +646,38 @@ static void launch_push(b200tts_wavernn* ctx, const float* d_mel, const GenArgs&
   a.error = ctx->error.as<int>();
   a.fir = ctx->d_fir;
   a.NT = ctx->NT;
-  a.B = pack ? pack->n_utt : rows; a.S = ua.S; a.T = T; a.hop = hop; a.steps = pack ? pack->steps : ua.steps;
+  a.hop = ctx->cfg.hop_length;
+  a.prof = phase_counters(ctx, prof, pm.ncta, st);
+  size_t scratch = 0;
+  const void* kern = G == 8 ? push_kernel<8>(f, a.hop, a.NT, &scratch)
+                   : G == 16 ? push_kernel<16>(f, a.hop, a.NT, &scratch) : push_kernel<32>(f, a.hop, a.NT, &scratch);
+  void* args[] = {(void*)&pm, (void*)&a, io};
+  const bool sess = f == PushFlavour::SESSION;
+  launch_step(ctx, sess ? SK_SESSION : SK_PUSH, kern, sess ? "push session kernel" : "push kernel", pm.ncta, kPushThreads,
+              ((size_t)pm.blob + scratch) * sizeof(float), args, prof, st);
+}
+
+// `fold` != null: rows are the folds of ONE source utterance of T0 frames (conditioning tables of utterance 0, row u
+// starts at sample u * stride); otherwise row u is utterance u.
+struct PackInfo {            // gen_opts.d_pack_*: kernel rows run queues of utterances
+  const int* utt;
+  const int* start;
+  int rows, segs, steps, n_utt;
+};
+static void launch_push(b200tts_wavernn* ctx, const float* d_mel, const GenArgs& ua, const MolIO* mol, bool prof, cudaStream_t st,
+                        const FoldGeom* fold, int T0, const PackInfo* pack) {
+  const int rows = pack ? pack->rows : ua.B;
+  const int T = fold ? T0 : ua.T;
+  const int tab_rows = fold ? 1 : (pack ? pack->n_utt : push_rows(rows)), src_rows = fold ? 1 : (pack ? pack->n_utt : rows);
+  PushArgs a{};
+  a.tab = launch_cond_table(ctx, d_mel, ua.aux_frames, src_rows, tab_rows, T, ctx->push_tab, st);
+  a.B = pack ? pack->n_utt : rows; a.S = ua.S; a.T = T; a.steps = pack ? pack->steps : ua.steps;
   if (pack) { a.pack_utt = pack->utt; a.pack_start = pack->start; a.pack_segs = pack->segs; a.pack_rows = pack->rows; }
   a.row_stride = fold ? fold->stride : 0;
-  a.S_src = T * hop;
+  a.S_src = T * ctx->cfg.hop_length;
   copy_gen_fields(a, ua);
-  a.prof = phase_counters(ctx, prof, pm.ncta, st);
-  switch (G) {
-    case 8: launch_push_t<8>(ctx, a, mol, st); break;
-    case 16: launch_push_t<16>(ctx, a, mol, st); break;
-    default: launch_push_t<32>(ctx, a, mol, st); break;
-  }
+  MolIO io = mol ? *mol : MolIO{};
+  launch_push_kernel(ctx, mol ? PushFlavour::MOL : PushFlavour::RAW, rows, a, &io, prof, st);
 }
 
 // ---- tensor-core pipeline (wavernn_tc.cuh): plain batches of up to 256 rows ----------------------------------------------
@@ -673,7 +685,7 @@ static void launch_tc(b200tts_wavernn* ctx, const float* d_mel, const GenArgs& u
   const int rows = ua.B, T = ua.T;
   const int ng = (rows + kTcRows - 1) / kTcRows;
   TcArgs a{};
-  a.tab = launch_cond_table(ctx, d_mel, ua.aux_frames, rows, rows, T, st);
+  a.tab = launch_cond_table(ctx, d_mel, ua.aux_frames, rows, rows, T, ctx->push_tab, st);
   ctx->tc_vec.ensure((size_t)TV_COUNT * ng * 2 * kTcVecBytes);
   ctx->tc_x1f.ensure((size_t)ng * 2 * kTcRows * 512 * sizeof(float));
   ctx->tc_win.ensure((size_t)ng * 2 * kTcWinCopies * kTcRows * 16 * sizeof(unsigned long long));
@@ -694,14 +706,7 @@ static void launch_tc(b200tts_wavernn* ctx, const float* d_mel, const GenArgs& u
   copy_gen_fields(a, ua);
   a.prof = phase_counters(ctx, prof, kTcCtas, st);
   void* args[] = {(void*)&a};
-  coop_launch(ctx, (const void*)wavernn_tc_kernel, "tensor-core kernel", kTcCtas, kTcThreads, kTcSmemBytes, args, st);
-}
-
-// After the stream has been synchronised: did a kernel of the last generate call give up waiting for a peer CTA?
-static void check_call_error(b200tts_wavernn* ctx) {
-  int flag = 0;
-  B200_CUDA(cudaMemcpy(&flag, ctx->error.p, sizeof(int), cudaMemcpyDeviceToHost));
-  REQUIRE(flag == 0, B200TTS_ECUDA, "grid kernel: a grid-barrier wait timed out (co-resident CTA missing); results are invalid");
+  launch_step(ctx, SK_TC, (const void*)wavernn_tc_kernel, "tensor-core kernel", kTcCtas, kTcThreads, kTcSmemBytes, args, prof, st);
 }
 
 // Smallest batch kernel=auto gives the tensor cores.  On an H100 80GB HBM3 at a 400 W power limit the tensor-core pipeline costs
@@ -792,8 +797,6 @@ static void run_generate_rows(b200tts_wavernn* ctx, const float* d_mel, int B, i
   const int GB = folding ? fg.nfold : B;            // rows the generation kernels see
   const int GS = folding ? fg.L : S;                // steps per row
   const StepKernel kernel = choose_kernel(ctx, GB, o);
-  ctx->last_kernel = kernel;
-  ctx->prof_ncta = 0;
   ctx->aux_frames.ensure((size_t)B * T * O * sizeof(float));
   // the rows' output, RAW labels or MOL samples: the context's scratch when the caller passed no buffer
   int16_t* labels = d_labels;
@@ -827,7 +830,6 @@ static void run_generate_rows(b200tts_wavernn* ctx, const float* d_mel, int B, i
     case SK_PUSH: launch_push(ctx, d_mel, a, ctx->mol ? &mol : nullptr, prof, st, fold, T, packing ? &pi : nullptr); break;
     case SK_TC: launch_tc(ctx, d_mel, a, prof, st); break;
   }
-  ctx->ev_valid = true;
   if (d_wave) {
     const int* err = ctx->error.as<int>();
     if (folding) {
@@ -1037,13 +1039,12 @@ extern "C" int b200tts_wavernn_session_open(b200tts_wavernn* ctx, const float* d
   s->wave_len = (int64_t)(T - 1) * hop;
   s->seed = rng->seed;
   s->id = rng->utterance_offset;
-  s->tab.ensure((size_t)(T + 1) * ctx->pm.ncta * kPushCondRows * sizeof(float));
   s->state.ensure((size_t)kSessStateFloats * sizeof(float));
   // the conditioning of a one-shot run of this mel, once: MelResNet into the context's scratch, consumed in stream order by the
   // tables, which the session owns (the next generate overwrites every scratch buffer)
   ctx->aux_frames.ensure((size_t)T * ctx->cfg.res_out_dims * sizeof(float));
   run_upsample(ctx, d_mel, 1, T, nullptr, ctx->aux_frames.as<float>(), nullptr, st);
-  launch_cond_table(ctx, d_mel, ctx->aux_frames.as<float>(), 1, 1, T, st, s->tab.as<float>());
+  launch_cond_table(ctx, d_mel, ctx->aux_frames.as<float>(), 1, 1, T, s->tab, st);
   ctx->sessions.insert(s.get());
   *out = s.release();
   API_END
@@ -1064,14 +1065,6 @@ extern "C" int b200tts_wavernn_session_info(const b200tts_wavernn_session* s, in
   if (steps) *steps = s->S;
   if (wave_len) *wave_len = s->wave_len;
   API_END
-}
-
-template <int G>
-static void launch_session_t(b200tts_wavernn* ctx, PushArgs& a, SessIO& io, cudaStream_t st) {
-  PushModel pm = ctx->pm;
-  const size_t smem = ((size_t)pm.blob + (size_t)PushTraits<G>::scratch_floats(a.hop, a.NT)) * sizeof(float);
-  void* args[] = {(void*)&pm, (void*)&a, (void*)&io};
-  coop_launch(ctx, (const void*)wavernn_push_session_kernel<G>, "push session kernel", pm.ncta, kPushThreads, smem, args, st);
 }
 
 extern "C" int b200tts_wavernn_session_run(b200tts_wavernn* ctx, b200tts_wavernn_session* const* s, int n, int max_steps,
@@ -1110,30 +1103,10 @@ extern "C" int b200tts_wavernn_session_run(b200tts_wavernn* ctx, b200tts_wavernn
   }
   B200_CUDA(cudaMemsetAsync(ctx->error.p, 0, sizeof(int), st));     // b200tts_wavernn_check reports this run
   if (steps > 0) {
-    const PushModel& pm = ctx->pm;
-    const int G = push_rows(n);
-    const size_t nvec = (size_t)kPushVecs * 2 * pm.ncta * G * 4, nbest = (size_t)pm.ncta * G;
-    ctx->push_vec.ensure(nvec * sizeof(float));
-    ctx->push_best.ensure(nbest * sizeof(unsigned long long));
-    launch_push_init(ctx->push_vec.as<uint32_t>(), nvec, ctx->push_best.as<unsigned long long>(), nbest, nullptr, ctx->sm_count, st);
-    ctx->launches++;
     PushArgs a{};
-    a.wblob = ctx->push_blob.as<float>();
-    a.vec = ctx->push_vec.as<float>();
-    a.best = ctx->push_best.as<unsigned long long>();
-    a.error = ctx->error.as<int>();
-    a.fir = ctx->d_fir;
-    a.NT = ctx->NT;
-    a.B = n; a.hop = ctx->cfg.hop_length; a.steps = steps;
+    a.B = n; a.steps = steps;
     a.rng_mode = B200TTS_RNG_PHILOX;
-    switch (G) {
-      case 8: launch_session_t<8>(ctx, a, io, st); break;
-      case 16: launch_session_t<16>(ctx, a, io, st); break;
-      default: launch_session_t<32>(ctx, a, io, st); break;
-    }
-    ctx->last_kernel = SK_SESSION;
-    ctx->prof_ncta = 0;
-    ctx->ev_valid = true;
+    launch_push_kernel(ctx, PushFlavour::SESSION, n, a, &io, false, st);
   }
   if (d_wave) {
     dim3 grid((max_steps + 255) / 256, n);

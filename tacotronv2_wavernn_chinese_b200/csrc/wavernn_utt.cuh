@@ -79,6 +79,12 @@ __device__ __forceinline__ void warp_rows_dot(const float* __restrict__ W, int l
     for (int g = 0; g < G; ++g) out[r][g] = warp_sum(acc[r][g]);
 }
 
+// Host side: the floats of dynamic shared memory utt_run<G, *> carves up below, buffer by buffer.
+inline size_t utt_smem_floats(const StepWeights& W, int G) {
+  const int KX = W.R + W.aux, KF = W.F + W.aux;
+  return (size_t)G * (W.ldI + W.R + 2 * W.R + 2 * W.R + KX + KX + KF + W.F + W.NC);
+}
+
 // The whole loop; MOL selects the sampler (fc3 then has NC = 32 rows, the 30 parameters padded to whole quads).
 template <int G, bool MOL>
 __device__ __forceinline__ void utt_run(StepWeights W, GenArgs A, MolIO M) {

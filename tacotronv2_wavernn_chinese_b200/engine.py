@@ -34,6 +34,15 @@ def _ptr(t):
     return C.c_void_p(t.data_ptr()) if t is not None else C.c_void_p(0)
 
 
+def _rng(mode: int, seed: int, utterance_offset: int) -> Rng:
+    """The noise of a call: `mode`, keyed by the 64-bit seed and the utterance id of row 0."""
+    rng = Rng()
+    rng.mode = mode
+    rng.seed = int(seed) & 0xFFFFFFFFFFFFFFFF
+    rng.utterance_offset = int(utterance_offset) & 0xFFFFFFFFFFFFFFFF
+    return rng
+
+
 MOL_PARAMS, MOL_U = 30, 11          # fc3 outputs and uniforms per step of a mixture-of-logistics model (voc_mode = 'MOL')
 
 
@@ -151,9 +160,7 @@ class WaveRNNEngine:
             if want_wave and steps == GS:
                 wave = torch.empty(B, (T - 1) * self.hop, device=dev, dtype=torch.float64)
             keep = [m]                          # inputs the stream reads after this call returns
-            rng = Rng()
-            rng.seed = int(seed) & 0xFFFFFFFFFFFFFFFF
-            rng.utterance_offset = int(utterance_offset)
+            rng = _rng(_lib.RNG_PHILOX if noise is None else noise_mode, seed, utterance_offset)
             if utterance_ids is not None:       # rows that are NOT consecutive utterances (length-sorted chunks): per-row global index
                 ids = torch.as_tensor(np.asarray(utterance_ids, dtype=np.int64)).to(dev).contiguous()
                 if tuple(ids.shape) != (B,) or fold is not None:
@@ -164,11 +171,8 @@ class WaveRNNEngine:
                 nd = torch.as_tensor(noise).to(device=dev, dtype=torch.float32).contiguous()
                 if nd.dim() != 3 or tuple(nd.shape[1:]) != (GB, noise_width) or nd.shape[0] < steps:
                     raise ValueError(f'{noise_name} must be [>= {steps}, {GB}, {noise_width}], got {tuple(nd.shape)}')
-                rng.mode = noise_mode
                 rng.d_q = nd.data_ptr()
                 keep.append(nd)
-            else:
-                rng.mode = _lib.RNG_PHILOX
             opts = GenOpts()
             opts.kernel = _lib.KERNELS[kernel]
             opts.mu_law = 1 if mu_law and not mol else 0
@@ -221,10 +225,7 @@ class WaveRNNEngine:
             raise ValueError(f'mel must be [{self.feat}, T], got {tuple(m.shape)}')
         with torch.cuda.device(self.device):
             m = m.to(device=self._dev(), dtype=torch.float32).contiguous()
-            rng = Rng()
-            rng.mode = _lib.RNG_PHILOX
-            rng.seed = int(seed) & 0xFFFFFFFFFFFFFFFF
-            rng.utterance_offset = int(utterance_id) & 0xFFFFFFFFFFFFFFFF
+            rng = _rng(_lib.RNG_PHILOX, seed, utterance_id)
             h = C.c_void_p()
             _lib.check(self.lib.b200tts_wavernn_session_open(self._h, _ptr(m), int(m.shape[1]), C.byref(rng), 1 if mu_law else 0,
                                                              C.byref(h), self._stream()))
@@ -273,10 +274,7 @@ class WaveRNNEngine:
         S = T * self.hop
         labels = np.empty((B, S), dtype=np.int16) if want_labels else None
         wave = np.empty((B, (T - 1) * self.hop), dtype=np.float64) if want_wave else None
-        rng = Rng()
-        rng.mode = _lib.RNG_PHILOX
-        rng.seed = int(seed) & 0xFFFFFFFFFFFFFFFF
-        rng.utterance_offset = int(utterance_offset)
+        rng = _rng(_lib.RNG_PHILOX, seed, utterance_offset)
         opts = GenOpts()
         opts.kernel = _lib.KERNELS[kernel]
         opts.mu_law = 1 if mu_law else 0
