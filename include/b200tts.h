@@ -190,7 +190,7 @@ int64_t b200tts_wavernn_launch_count(const b200tts_wavernn* ctx);
  * generate call; blocks until that kernel has finished.  Negative on error. */
 double b200tts_wavernn_last_kernel_ms(b200tts_wavernn* ctx);
 /* Which step kernel the last generate call ran: 1 utterance, 2 wide grid, 3 push, 5 tensor-core pipeline, 6 push for a session
- * run (0: none yet; 4 is no longer returned).  Instrumentation for bench.py's roofline; no reference counterpart. */
+ * run, 7 tensor-core pipeline for a session run (0: none yet; 4 is no longer returned).  Instrumentation for bench.py's roofline; no reference counterpart. */
 int b200tts_wavernn_last_kernel(const b200tts_wavernn* ctx);
 
 /* Synchronises the device and reports whether the most recent generate call on this context completed: the persistent
@@ -199,28 +199,37 @@ int b200tts_wavernn_last_kernel(const b200tts_wavernn* ctx);
  * user (WaveRNN.generate <- fatchord_version.py:169, wavernn_gen.py:41) call this after their own synchronisation point. */
 int b200tts_wavernn_check(b200tts_wavernn* ctx);
 
-/* Generation sessions: one RAW utterance whose sample loop runs in pieces on the push kernel (<= 32 sessions per launch), so
- * audio can be handed out after every run and the set of utterances can change between runs.  The pieces of a session,
- * concatenated, are bit for bit the labels and wave of a one-shot b200tts_wavernn_generate of that mel with the same seed and
- * utterance id, however the steps are cut and whichever sessions share a run.  Refused (B200TTS_EINVAL, before any CUDA call)
- * for a MOL context and a model the push kernel cannot run (rnn_dims = fc_dims = 512 on >= 128 SMs).
+/* Generation sessions: one RAW utterance whose sample loop runs in pieces, so audio can be handed out after every run and the
+ * set of utterances can change between runs.  A session runs on the kernel it was opened for: the push kernel (<= 32 sessions
+ * per launch, any cut) or the tensor-core pipeline (<= 256 sessions per launch, cuts on frame boundaries).  The pieces of a
+ * session, concatenated, are bit for bit the labels and wave of a one-shot b200tts_wavernn_generate of that mel with the same
+ * seed and utterance id on the same kernel family (kernel = AUTO / GRID at <= 32 rows, or TC), however the steps are cut and
+ * whichever sessions share a run.  Refused (B200TTS_EINVAL, before any CUDA call) for a MOL context and a model the push
+ * kernel cannot run (rnn_dims = fc_dims = 512 on >= 128 SMs).
  *
- * session_open: d_mel [feat][T], T >= 21.  rng: PHILOX only, rng->utterance_offset is the utterance id (d_utterance_ids must be
- *   NULL).  The conditioning tables are computed once, on `stream`, into memory the session owns.
+ * session_open: a push session (session_open_kernel with kernel = B200TTS_KERNEL_AUTO).
+ * session_open_kernel: d_mel [feat][T], T >= 21.  kernel: B200TTS_KERNEL_AUTO (push) or B200TTS_KERNEL_TC (tensor cores; refused
+ *   where kernel=tc cannot run).  rng: PHILOX only, rng->utterance_offset is the utterance id (d_utterance_ids must be NULL).
+ *   The conditioning tables are computed once, on `stream`, into memory the session owns.
  * session_destroy: null-safe; waits for the runs still queued.  b200tts_wavernn_destroy frees the sessions still open.
  * session_info: next step, steps of the utterance (T*hop) and samples of its wave ((T-1)*hop); any pointer may be NULL.
- * session_run: n (1..32) distinct sessions of ctx advance by min(max_steps, steps - pos) steps each in one push-kernel launch
- *   (a finished session takes part with 0 steps).  d_labels [n][max_steps] int16 and d_wave [n][max_steps] float64 (either may
+ * session_run: n distinct sessions of ctx advance by min(max_steps, steps - pos) steps each in one launch (a finished session
+ *   takes part with 0 steps): 1..32 push sessions, or 1..256 tensor-core sessions with max_steps a multiple of hop_length, never
+ *   a mix of the two.  d_labels [n][max_steps] int16 and d_wave [n][max_steps] float64 (either may
  *   be NULL) receive each session's steps from its old position: wave entry i is sample pos + i of the one-shot wave (0 from
  *   (T-1)*hop on) and entries past the session's count are 0.  Positions advance on the host at enqueue.  Poll timeouts are
  *   reported by b200tts_wavernn_check as for generate. */
 typedef struct b200tts_wavernn_session b200tts_wavernn_session;
 int b200tts_wavernn_session_open(b200tts_wavernn* ctx, const float* d_mel, int T, const b200tts_rng* rng, int mu_law,
                                  b200tts_wavernn_session** out, void* stream);
+int b200tts_wavernn_session_open_kernel(b200tts_wavernn* ctx, const float* d_mel, int T, const b200tts_rng* rng, int mu_law,
+                                        int kernel, b200tts_wavernn_session** out, void* stream);
 void b200tts_wavernn_session_destroy(b200tts_wavernn_session* s);
 int b200tts_wavernn_session_info(const b200tts_wavernn_session* s, int64_t* pos, int64_t* steps, int64_t* wave_len);
 int b200tts_wavernn_session_run(b200tts_wavernn* ctx, b200tts_wavernn_session* const* s, int n, int max_steps,
                                 int16_t* d_labels, double* d_wave, void* stream);
+/* The most sessions one session_run takes on ctx: 256 where the tensor-core pipeline runs (kernel=tc), else 32. */
+int b200tts_wavernn_session_max_rows(const b200tts_wavernn* ctx);
 
 /* Measured fp32 CUDA-core ceiling of `device` in TFLOP/s (register-only packed FFMA2 loop on every SM): the denominator
  * of bench.py's FLOP-form roofline. */

@@ -107,6 +107,9 @@ SIGNATURES = {
     'b200tts_debug_fp32_peak': (C.c_int, [C.c_int, C.POINTER(C.c_double)]),
     'b200tts_wavernn_session_open': (C.c_int, [C.c_void_p, C.c_void_p, C.c_int, C.POINTER(Rng), C.c_int, C.POINTER(C.c_void_p),
                                                C.c_void_p]),
+    'b200tts_wavernn_session_open_kernel': (C.c_int, [C.c_void_p, C.c_void_p, C.c_int, C.POINTER(Rng), C.c_int, C.c_int,
+                                                      C.POINTER(C.c_void_p), C.c_void_p]),
+    'b200tts_wavernn_session_max_rows': (C.c_int, [C.c_void_p]),
     'b200tts_wavernn_session_destroy': (None, [C.c_void_p]),
     'b200tts_wavernn_session_info': (C.c_int, [C.c_void_p, C.POINTER(C.c_int64), C.POINTER(C.c_int64), C.POINTER(C.c_int64)]),
     'b200tts_wavernn_session_run': (C.c_int, [C.c_void_p, C.POINTER(C.c_void_p), C.c_int, C.c_int, C.c_void_p, C.c_void_p,

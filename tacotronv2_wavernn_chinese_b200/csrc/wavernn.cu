@@ -17,10 +17,12 @@
 
 using namespace b200tts;
 
-// One RAW utterance generated in pieces on the push kernel (b200tts_wavernn_session_*): its conditioning tables, computed once
-// at open, and the state its last run saved (SessRow).  Owned by its context, which frees the sessions still open.
+// One RAW utterance generated in pieces on the push kernel or the tensor cores (b200tts_wavernn_session_*): its conditioning
+// tables, computed once at open, and the state its last run saved (SessRow; its layout depends on the kernel, so a session stays
+// on the kernel it was opened for).  Owned by its context, which frees the sessions still open.
 struct b200tts_wavernn_session {
   b200tts_wavernn* ctx = nullptr;
+  bool tc = false;                          // runs on wavernn_tc_session_kernel (else the push session kernel)
   int T = 0, mu_law = 1;
   int64_t pos = 0, S = 0, wave_len = 0;     // next step; steps of the utterance; samples of its wave
   uint64_t seed = 0, id = 0;
@@ -410,7 +412,7 @@ extern "C" int b200tts_wavernn_upsample(b200tts_wavernn* ctx, const float* d_mel
 
 // ---- generation -----------------------------------------------------------------------------------
 // The step kernel a launch runs; the values are those b200tts_wavernn_last_kernel reports.
-enum StepKernel { SK_UTTERANCE = 1, SK_GRID = 2, SK_PUSH = 3, SK_TC = 5, SK_SESSION = 6 };
+enum StepKernel { SK_UTTERANCE = 1, SK_GRID = 2, SK_PUSH = 3, SK_TC = 5, SK_SESSION = 6, SK_TC_SESSION = 7 };
 
 // The fields every step kernel's arguments take from GenArgs as they are: noise, debug buffers, labels.
 template <class Args>
@@ -681,11 +683,13 @@ static void launch_push(b200tts_wavernn* ctx, const float* d_mel, const GenArgs&
 }
 
 // ---- tensor-core pipeline (wavernn_tc.cuh): plain batches of up to 256 rows ----------------------------------------------
-static void launch_tc(b200tts_wavernn* ctx, const float* d_mel, const GenArgs& ua, bool prof, cudaStream_t st) {
+// `sess` != null: a run of generation sessions (wavernn_tc_session_kernel), row u = session u of *sess, whose tables the
+// sessions own; `ua` gives B = sessions and the lock-steps, `d_mel` is unused.
+static void launch_tc(b200tts_wavernn* ctx, const float* d_mel, const GenArgs& ua, const TcSessIO* sess, bool prof, cudaStream_t st) {
   const int rows = ua.B, T = ua.T;
   const int ng = (rows + kTcRows - 1) / kTcRows;
   TcArgs a{};
-  a.tab = launch_cond_table(ctx, d_mel, ua.aux_frames, rows, rows, T, ctx->push_tab, st);
+  if (!sess) a.tab = launch_cond_table(ctx, d_mel, ua.aux_frames, rows, rows, T, ctx->push_tab, st);
   ctx->tc_vec.ensure((size_t)TV_COUNT * ng * 2 * kTcVecBytes);
   ctx->tc_x1f.ensure((size_t)ng * 2 * kTcRows * 512 * sizeof(float));
   ctx->tc_win.ensure((size_t)ng * 2 * kTcWinCopies * kTcRows * 16 * sizeof(unsigned long long));
@@ -705,8 +709,12 @@ static void launch_tc(b200tts_wavernn* ctx, const float* d_mel, const GenArgs& u
   a.NT = ctx->NT; a.B = rows; a.S = ua.S; a.T = T; a.hop = ctx->cfg.hop_length; a.steps = ua.steps; a.ng = ng; a.NC = ctx->NC;
   copy_gen_fields(a, ua);
   a.prof = phase_counters(ctx, prof, kTcCtas, st);
-  void* args[] = {(void*)&a};
-  launch_step(ctx, SK_TC, (const void*)wavernn_tc_kernel, "tensor-core kernel", kTcCtas, kTcThreads, kTcSmemBytes, args, prof, st);
+  void* args[] = {(void*)&a, (void*)sess};
+  if (sess)
+    launch_step(ctx, SK_TC_SESSION, (const void*)wavernn_tc_session_kernel, "tensor-core session kernel", kTcCtas, kTcThreads,
+                kTcSmemBytes, args, prof, st);
+  else
+    launch_step(ctx, SK_TC, (const void*)wavernn_tc_kernel, "tensor-core kernel", kTcCtas, kTcThreads, kTcSmemBytes, args, prof, st);
 }
 
 // Smallest batch kernel=auto gives the tensor cores.  On an H100 80GB HBM3 at a 400 W power limit the tensor-core pipeline costs
@@ -828,7 +836,7 @@ static void run_generate_rows(b200tts_wavernn* ctx, const float* d_mel, int B, i
     case SK_UTTERANCE: launch_utterance(ctx, a, ctx->mol ? &mol : nullptr, st, fold, S); break;
     case SK_GRID: launch_grid(ctx, d_mel, a, ctx->mol ? &mol : nullptr, prof, st, fold, S); break;
     case SK_PUSH: launch_push(ctx, d_mel, a, ctx->mol ? &mol : nullptr, prof, st, fold, T, packing ? &pi : nullptr); break;
-    case SK_TC: launch_tc(ctx, d_mel, a, prof, st); break;
+    case SK_TC: launch_tc(ctx, d_mel, a, nullptr, prof, st); break;
   }
   if (d_wave) {
     const int* err = ctx->error.as<int>();
@@ -1011,19 +1019,35 @@ extern "C" int b200tts_wavernn_debug_phase_cycles(b200tts_wavernn* ctx, double* 
   API_END
 }
 
-// ---- generation sessions: one RAW utterance in pieces on the push kernel (wavernn_push_session_kernel) ---------------------
+// ---- generation sessions: one RAW utterance in pieces on the push kernel (wavernn_push_session_kernel) or the tensor cores
+//      (wavernn_tc_session_kernel) ---------------------------------------------------------------------------------------------
 // Every refusal below comes before the first CUDA call, so a refused call has launched and allocated nothing.
 static void require_session_model(const b200tts_wavernn* ctx) {
   REQUIRE(!ctx->mol, B200TTS_EINVAL, "generation sessions are RAW only: this context holds a MOL model");
   REQUIRE(ctx->pm.ok, B200TTS_EINVAL, "generation sessions need the push kernel (rnn_dims = fc_dims = 512 on >= 128 SMs)");
 }
 
+// The most sessions one run takes on ctx: a tensor-core run where that kernel runs, else a push run.
+extern "C" int b200tts_wavernn_session_max_rows(const b200tts_wavernn* ctx) {
+  return ctx && ctx->tc_ok ? kTcSessRows : kPushMaxRows;
+}
+
 extern "C" int b200tts_wavernn_session_open(b200tts_wavernn* ctx, const float* d_mel, int T, const b200tts_rng* rng, int mu_law,
                                             b200tts_wavernn_session** out, void* stream) {
+  return b200tts_wavernn_session_open_kernel(ctx, d_mel, T, rng, mu_law, B200TTS_KERNEL_AUTO, out, stream);
+}
+
+extern "C" int b200tts_wavernn_session_open_kernel(b200tts_wavernn* ctx, const float* d_mel, int T, const b200tts_rng* rng,
+                                                   int mu_law, int kernel, b200tts_wavernn_session** out, void* stream) {
   API_BEGIN
   REQUIRE(ctx && d_mel && rng && out, B200TTS_EINVAL, "null argument");
   *out = nullptr;
   require_session_model(ctx);
+  REQUIRE(kernel == B200TTS_KERNEL_AUTO || kernel == B200TTS_KERNEL_TC, B200TTS_EINVAL,
+          "a session runs on kernel = AUTO (the push kernel) or TC (the tensor cores)");
+  const bool tc = kernel == B200TTS_KERNEL_TC;
+  REQUIRE(!tc || ctx->tc_ok, B200TTS_EINVAL, "tensor-core sessions need a model and device that run kernel=tc (rnn_dims = fc_dims = "
+                                             "512, 10-bit classes, hop_length x FIR taps <= 8192, >= 128 SMs)");
   REQUIRE(rng->mode == B200TTS_RNG_PHILOX && !rng->d_utterance_ids, B200TTS_EINVAL,
           "a session takes PHILOX noise keyed by (seed, rng->utterance_offset as the utterance id); d_utterance_ids must be NULL");
   const int hop = ctx->cfg.hop_length;
@@ -1033,6 +1057,7 @@ extern "C" int b200tts_wavernn_session_open(b200tts_wavernn* ctx, const float* d
   const cudaStream_t st = (cudaStream_t)stream;
   std::unique_ptr<b200tts_wavernn_session> s(new b200tts_wavernn_session());
   s->ctx = ctx;
+  s->tc = tc;
   s->T = T;
   s->mu_law = mu_law ? 1 : 0;
   s->S = (int64_t)T * hop;
@@ -1072,16 +1097,24 @@ extern "C" int b200tts_wavernn_session_run(b200tts_wavernn* ctx, b200tts_wavernn
   API_BEGIN
   REQUIRE(ctx && s, B200TTS_EINVAL, "null argument");
   require_session_model(ctx);
-  REQUIRE(n >= 1 && n <= kPushMaxRows, B200TTS_EINVAL, "a session run takes 1..32 sessions");
+  // the first session says which kernel the run takes; every other must be on the same one
+  const bool tc = n >= 1 && s[0] && s[0]->tc;
+  if (tc) REQUIRE(n <= kTcSessRows, B200TTS_EINVAL, "a tensor-core session run takes 1..256 sessions");
+  else REQUIRE(n >= 1 && n <= kPushMaxRows, B200TTS_EINVAL, "a session run takes 1..32 sessions");
   REQUIRE(max_steps >= 1, B200TTS_EINVAL, "max_steps must be >= 1");
+  const int hop = ctx->cfg.hop_length;
+  REQUIRE(!tc || max_steps % hop == 0, B200TTS_EINVAL,
+          "a tensor-core session run takes max_steps a multiple of hop_length (every position stays on a frame boundary)");
   for (int i = 0; i < n; ++i) {
     REQUIRE(s[i], B200TTS_EINVAL, "null session");
     REQUIRE(s[i]->ctx == ctx, B200TTS_EINVAL, "the session belongs to another context");
+    REQUIRE(s[i]->tc == tc, B200TTS_EINVAL, "a session run cannot mix push and tensor-core sessions");
     for (int j = 0; j < i; ++j) REQUIRE(s[j] != s[i], B200TTS_EINVAL, "the same session appears twice in one run");
   }
   DeviceGuard dg(ctx->device);
   const cudaStream_t st = (cudaStream_t)stream;
-  SessIO io{};
+  // the rows of either kernel: TcSessIO holds 256 SessRow, of which a push run passes the first 32 as its SessIO
+  TcSessIO io{};
   int steps = 0;
   for (int i = 0; i < n; ++i) {
     SessRow& r = io.row[i];
@@ -1102,15 +1135,30 @@ extern "C" int b200tts_wavernn_session_run(b200tts_wavernn* ctx, b200tts_wavernn
     io.labels = ctx->sess_labels.as<int16_t>();
   }
   B200_CUDA(cudaMemsetAsync(ctx->error.p, 0, sizeof(int), st));     // b200tts_wavernn_check reports this run
-  if (steps > 0) {
+  if (steps > 0 && tc) {
+    GenArgs a{};
+    a.B = n; a.steps = steps; a.hop = hop;
+    a.rng_mode = B200TTS_RNG_PHILOX;
+    launch_tc(ctx, nullptr, a, &io, false, st);
+  } else if (steps > 0) {
     PushArgs a{};
     a.B = n; a.steps = steps;
     a.rng_mode = B200TTS_RNG_PHILOX;
-    launch_push_kernel(ctx, PushFlavour::SESSION, n, a, &io, false, st);
+    SessIO pio{};
+    std::copy(io.row, io.row + n, pio.row);
+    pio.labels = io.labels;
+    pio.ld = io.ld;
+    launch_push_kernel(ctx, PushFlavour::SESSION, n, a, &pio, false, st);
   }
-  if (d_wave) {
-    dim3 grid((max_steps + 255) / 256, n);
-    session_wave_kernel<<<grid, 256, 0, st>>>(io, ctx->cfg.hop_length, 20 * ctx->cfg.hop_length, ctx->NC, ctx->error.as<int>(), d_wave);
+  // the wave: session_wave_kernel takes 32 sessions per launch
+  for (int i0 = 0; d_wave && i0 < n; i0 += kPushMaxRows) {
+    const int m = std::min(n - i0, kPushMaxRows);
+    SessIO wio{};
+    std::copy(io.row + i0, io.row + i0 + m, wio.row);
+    wio.labels = io.labels + (size_t)i0 * max_steps;
+    wio.ld = max_steps;
+    dim3 grid((max_steps + 255) / 256, m);
+    session_wave_kernel<<<grid, 256, 0, st>>>(wio, hop, 20 * hop, ctx->NC, ctx->error.as<int>(), d_wave + (size_t)i0 * max_steps);
     B200_CUDA(cudaGetLastError());
     ctx->launches++;
   }

@@ -216,10 +216,16 @@ class WaveRNNEngine:
                 t.record_stream(torch.cuda.current_stream(self.device))
         return {'samples' if mol else 'labels': out, 'wave': wave, 'logits': logits, 'steps': steps}
 
-    def open_session(self, mel, *, seed: int = 0, utterance_id: int = 0, mu_law: bool = True) -> 'WaveRNNSession':
+    def open_session(self, mel, *, seed: int = 0, utterance_id: int = 0, mu_law: bool = True, kernel: str = 'auto') -> 'WaveRNNSession':
         """A generation session of one RAW utterance: mel [feat, T] (T >= 21) in [0, 1].  Its sample loop then runs in pieces
         (`advance`), and the pieces, concatenated, are bit for bit `generate(mel[None], seed=seed, utterance_ids=[utterance_id])`.
-        The conditioning is computed here, once, on the current stream."""
+        The conditioning is computed here, once, on the current stream.
+
+        kernel: 'auto' runs the session on the push kernel (up to 32 sessions per run, any cut); 'tc' on the tensor cores (up to
+        `max_session_rows` sessions per run, runs of a multiple of hop steps), and its pieces are then bit for bit
+        `generate(..., kernel='tc')`.  A session stays on the kernel it was opened for."""
+        if kernel not in ('auto', 'tc'):
+            raise ValueError(f"kernel must be 'auto' (push) or 'tc', got {kernel!r}")
         m = torch.as_tensor(mel)
         if m.dim() != 2 or m.shape[0] != self.feat:
             raise ValueError(f'mel must be [{self.feat}, T], got {tuple(m.shape)}')
@@ -227,15 +233,16 @@ class WaveRNNEngine:
             m = m.to(device=self._dev(), dtype=torch.float32).contiguous()
             rng = _rng(_lib.RNG_PHILOX, seed, utterance_id)
             h = C.c_void_p()
-            _lib.check(self.lib.b200tts_wavernn_session_open(self._h, _ptr(m), int(m.shape[1]), C.byref(rng), 1 if mu_law else 0,
-                                                             C.byref(h), self._stream()))
+            _lib.check(self.lib.b200tts_wavernn_session_open_kernel(self._h, _ptr(m), int(m.shape[1]), C.byref(rng), 1 if mu_law else 0,
+                                                                    _lib.KERNELS[kernel], C.byref(h), self._stream()))
             m.record_stream(torch.cuda.current_stream(self.device))
         s = WaveRNNSession(self, h)
         self._sessions.add(s)
         return s
 
     def advance(self, sessions, max_steps: int):
-        """Runs up to `max_steps` more steps of each session (1..32 distinct open sessions of this engine) in one launch.
+        """Runs up to `max_steps` more steps of each session in one launch: 1..32 distinct open push sessions of this engine, or
+        1..`max_session_rows` tensor-core sessions with `max_steps` a multiple of hop.
         Returns, for each session, (labels int16 [n], wave float64 [w]) cuda tensors: its n = min(max_steps, steps - position)
         labels from its old position, and the w samples of its wave among them (none past wave_len)."""
         sessions = list(sessions)
@@ -257,6 +264,11 @@ class WaveRNNEngine:
             w = max(0, min(pos + k, wave_len) - pos)
             out.append((labels[i, :k], wave[i, :w]))
         return out
+
+    @property
+    def max_session_rows(self) -> int:
+        """The most sessions one `advance` takes on this engine: 256 where the tensor-core kernel runs, else 32."""
+        return int(self.lib.b200tts_wavernn_session_max_rows(self._h))
 
     def fold_geometry(self, T: int, target: int, overlap: int):
         """(n_folds, fold_len) of fold_with_overlap for a T-frame utterance."""
@@ -323,7 +335,7 @@ class WaveRNNEngine:
         return int(self.lib.b200tts_wavernn_launch_count(self._h))
 
     KERNEL_NAMES = {0: None, 1: 'wavernn_utt_kernel', 2: 'wavernn_grid_kernel', 3: 'wavernn_push_kernel', 5: 'wavernn_tc_kernel',
-                    6: 'wavernn_push_session_kernel'}
+                    6: 'wavernn_push_session_kernel', 7: 'wavernn_tc_session_kernel'}
 
     def last_kernel(self):
         """Name of the step kernel the last generate call ran."""

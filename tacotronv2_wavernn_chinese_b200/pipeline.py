@@ -189,17 +189,25 @@ def _host(x):
 
 class StreamingVocoder:
     """Continuous batching of vocoder sessions on one engine.  `submit` queues requests; every `step` admits queued requests
-    first come first served into free rows (at most `max_rows` <= 32 sessions per launch), advances every session by up to
+    first come first served into free rows (at most `max_rows` sessions per launch), advances every session by up to
     `chunk_steps` samples in one launch and returns [(key, wave piece float64 numpy, finished)].  A key's pieces concatenate to
-    the wave vocode_ragged gives its mel with the same seed and id; mels shorter than MIN_FRAMES are zero-padded to it, as there."""
+    the wave vocode_ragged gives its mel with the same seed and id; mels shorter than MIN_FRAMES are zero-padded to it, as there.
+
+    `max_rows` is the service's capacity, up to the engine's `max_session_rows`.  Up to 32 rows the sessions run on the push
+    kernel; above 32 they run on the tensor cores (which then also serve the one-shot reference, `kernel='tc'`), and
+    `chunk_steps` must be a multiple of the engine's hop."""
 
     def __init__(self, engine, seed=0, chunk_steps=2750, max_rows=32):
-        if not 1 <= int(max_rows) <= 32:
-            raise ValueError('max_rows must be 1..32 (the push kernel runs at most 32 sessions per launch)')
+        cap = int(getattr(engine, 'max_session_rows', 32))
+        if not 1 <= int(max_rows) <= cap:
+            raise ValueError(f'max_rows must be 1..{cap} (the most sessions one launch of this engine takes)')
         if int(chunk_steps) < 1:
             raise ValueError('chunk_steps must be >= 1')
         self.engine, self.seed = engine, int(seed)
         self.chunk_steps, self.max_rows = int(chunk_steps), int(max_rows)
+        self._tc = self.max_rows > 32                       # the push kernel runs at most 32 sessions per launch
+        if self._tc and self.chunk_steps % int(engine.hop):
+            raise ValueError(f'above 32 rows the sessions run on the tensor cores: chunk_steps must be a multiple of hop ({engine.hop})')
         self._queue = collections.deque()       # (key, mel [T, feat], utterance id)
         self._active = []                       # (key, session) in admission order
 
@@ -227,7 +235,8 @@ class StreamingVocoder:
             T = max(m.shape[0], MIN_FRAMES)
             padded = np.zeros((m.shape[1], T), dtype=np.float32)         # zero frames past the end, as vocode_ragged pads
             padded[:, :m.shape[0]] = m.T
-            self._active.append((key, self.engine.open_session(padded, seed=self.seed, utterance_id=uid)))
+            kw = {'kernel': 'tc'} if self._tc else {}
+            self._active.append((key, self.engine.open_session(padded, seed=self.seed, utterance_id=uid, **kw)))
         if not self._active:
             return []
         pieces = self.engine.advance([s for _, s in self._active], self.chunk_steps)
