@@ -97,14 +97,19 @@ def import_reference():
     return fv
 
 
-def build_model(state_dict=None):
-    """Reference WaveRNN with the shipped hparams; loads `state_dict` (numpy/torch) or the shipped checkpoint."""
+def build_model(state_dict=None, dims=None, mode=None):
+    """Reference WaveRNN with the shipped hparams, or with `dims` (keys of synth.DEFAULT_DIMS) and voc_mode `mode` when given;
+    loads `state_dict` (numpy/torch) or the shipped checkpoint."""
     fv = import_reference()
     hp = fv._hp
+    if dims is None:
+        args = (hp.voc_rnn_dims, hp.voc_fc_dims, hp.bits, hp.voc_pad, hp.voc_upsample_factors, hp.num_mels, hp.voc_compute_dims,
+                hp.voc_res_out_dims, hp.voc_res_blocks, hp.hop_length, hp.sample_rate)
+    else:
+        args = tuple(dims[k] for k in ('rnn_dims', 'fc_dims', 'bits', 'pad', 'upsample_factors', 'feat_dims', 'compute_dims',
+                                       'res_out_dims', 'res_blocks', 'hop_length', 'sample_rate'))
     with contextlib.redirect_stdout(open(os.devnull, 'w')):
-        m = fv.WaveRNN(hp.voc_rnn_dims, hp.voc_fc_dims, hp.bits, hp.voc_pad, hp.voc_upsample_factors, hp.num_mels,
-                       hp.voc_compute_dims, hp.voc_res_out_dims, hp.voc_res_blocks, hp.hop_length,
-                       hp.sample_rate, hp.voc_mode)
+        m = fv.WaveRNN(*args, mode if mode is not None else hp.voc_mode)
     if state_dict is None:
         m.load(REF_CKPT)
     else:
@@ -136,8 +141,8 @@ class _RaceCategorical:
         return lab
 
 
-def reference_generate(model, mels, q, capture_logits_at=(), batched=False, target=None, overlap=None):
-    """Runs the reference `generate` (fatchord_version.py:169) unbatched with injected noise.
+def reference_generate(model, mels, q, capture_logits_at=(), batched=False, target=None, overlap=None, mu_law=None):
+    """Runs the reference `generate` (fatchord_version.py:169) unbatched with injected noise (mu_law None: the hparams' value).
 
     Returns dict(wave0 float64 [wave_len] (utterance 0 only -- :253), labels [B,S] int16, logits {step: [B,ncls]}).
     """
@@ -160,7 +165,7 @@ def reference_generate(model, mels, q, capture_logits_at=(), batched=False, targ
     try:
         hp = fv._hp
         wave = model.generate(torch.as_tensor(mels), '/dev/null', bool(batched), target if target is not None else hp.voc_target,
-                              overlap if overlap is not None else hp.voc_overlap, hp.mu_law)
+                              overlap if overlap is not None else hp.voc_overlap, hp.mu_law if mu_law is None else mu_law)
     finally:
         torch.distributions.Categorical = orig
         h.remove()

@@ -8,26 +8,16 @@ captures the mixture parameters.
 """
 from __future__ import annotations
 
-import contextlib
-import os
-
 import numpy as np
 import torch
 
 from oracle import ref_harness as rh
 
 
-def build_model_mol(state_dict):
-    """Reference WaveRNN(mode='MOL') with the shipped hparams, loaded from a numpy/torch state_dict."""
-    fv = rh.import_reference()
-    hp = fv._hp
-    with contextlib.redirect_stdout(open(os.devnull, 'w')):
-        m = fv.WaveRNN(hp.voc_rnn_dims, hp.voc_fc_dims, hp.bits, hp.voc_pad, hp.voc_upsample_factors, hp.num_mels,
-                       hp.voc_compute_dims, hp.voc_res_out_dims, hp.voc_res_blocks, hp.hop_length, hp.sample_rate, 'MOL')
-    sd = {k: torch.as_tensor(np.asarray(v)) for k, v in state_dict.items()}
-    missing = m.load_state_dict(sd, strict=False)
-    assert not missing.missing_keys, missing
-    return m
+def build_model_mol(state_dict, dims=None):
+    """Reference WaveRNN(mode='MOL') with the shipped hparams, or with `dims` (keys of synth.DEFAULT_DIMS), loaded from a
+    numpy/torch state_dict."""
+    return rh.build_model(state_dict, dims, 'MOL')
 
 
 class _UniformFeeder:

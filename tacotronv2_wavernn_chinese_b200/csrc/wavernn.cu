@@ -251,6 +251,12 @@ static int create_context(b200tts_wavernn** out, int device, const b200tts_waver
   REQUIRE(c.rnn_dims % 128 == 0 && c.fc_dims % 128 == 0, B200TTS_EINVAL, "rnn_dims / fc_dims must be multiples of 128");
   REQUIRE(mol || (c.bits >= 2 && c.bits <= 15), B200TTS_EINVAL, "bits must be 2..15 (labels are int16)");
   REQUIRE(c.compute_dims <= 1024 && c.res_out_dims <= 1024, B200TTS_EINVAL, "compute/res_out dims too large");
+  REQUIRE(c.pad >= 1, B200TTS_EINVAL,
+          "pad must be >= 1: the reference trims pad * hop_length samples from each end of the upsampled mels "
+          "(fatchord_version.py:88), which leaves nothing at pad 0");
+  REQUIRE(c.feat_dims >= 1, B200TTS_EINVAL, "feat_dims must be >= 1 (mel channels)");
+  REQUIRE(c.compute_dims >= 1, B200TTS_EINVAL, "compute_dims must be >= 1 (MelResNet channels)");
+  REQUIRE(c.res_blocks >= 0, B200TTS_EINVAL, "res_blocks must be >= 0");
   const int AUX = c.res_out_dims / 4, FEAT = c.feat_dims;
   REQUIRE(AUX % 4 == 0, B200TTS_EINVAL, "aux dims (res_out_dims/4) must be a multiple of 4");
   check_device(device);
@@ -500,11 +506,15 @@ static void launch_utterance(b200tts_wavernn* ctx, GenArgs a, const MolIO* mol, 
     a.mels_up = ctx->fold_mels.as<float>();
     a.aux_frames = ctx->fold_aux.as<float>();
   }
-  // utterances per CTA: enough CTAs to cover the SMs first, then amortise the L2 weight stream over more rows
-  int per = (a.B + ctx->sm_count - 1) / ctx->sm_count;
-  if (per <= 1) launch_utt<1>(ctx, a, mol, st);
-  else if (per <= 2) launch_utt<2>(ctx, a, mol, st);
-  else if (per <= 4) launch_utt<4>(ctx, a, mol, st);
+  // utterances per CTA: enough CTAs to cover the SMs first, then amortise the L2 weight stream over more rows, as many as fit in
+  // shared memory (wide or many-class models: 8 rows of 12-bit classes need 285 KB); choose_kernel refuses a model whose
+  // single row does not fit
+  const int per = (a.B + ctx->sm_count - 1) / ctx->sm_count;
+  int G = per <= 1 ? 1 : per <= 2 ? 2 : per <= 4 ? 4 : 8;
+  while (G > 1 && !utt_fits(ctx->sw, G)) G /= 2;
+  if (G == 1) launch_utt<1>(ctx, a, mol, st);
+  else if (G == 2) launch_utt<2>(ctx, a, mol, st);
+  else if (G == 4) launch_utt<4>(ctx, a, mol, st);
   else launch_utt<8>(ctx, a, mol, st);
 }
 
@@ -754,7 +764,11 @@ static StepKernel choose_kernel(b200tts_wavernn* ctx, int rows, const b200tts_ge
     default: throw Error(B200TTS_EINVAL, "unknown kernel selector");
   }
   REQUIRE(!packing, B200TTS_EINVAL, "packed generation needs the push kernel (kernel=auto/grid, rnn_dims = fc_dims = 512)");
-  if (kernel == B200TTS_KERNEL_UTTERANCE) return SK_UTTERANCE;
+  if (kernel == B200TTS_KERNEL_UTTERANCE) {
+    REQUIRE(utt_fits(ctx->sw, 1), B200TTS_EINVAL,
+            "model too large for the utterance kernel's shared memory (one row of its activations and logits exceeds 227 KB)");
+    return SK_UTTERANCE;
+  }
   REQUIRE(ctx->gm.ok, B200TTS_EINVAL, "kernel=grid was requested but this model/device cannot run the weight-stationary grid kernel "
                                       "(needs rnn_dims == fc_dims, n_classes == 2*rnn_dims, cooperative launch, R/4 <= SM count)");
   return SK_GRID;

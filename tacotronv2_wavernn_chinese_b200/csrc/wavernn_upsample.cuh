@@ -5,8 +5,11 @@
 //     afterwards (:84), so aux is constant within a hop and is never materialised at sample rate here.
 //   * the three Stretch2d + Conv2d stages (:73-80, :86-87) collapsed into one polyphase FIR of `hop` phases x NT
 //     taps over the zero-padded frame sequence.  The composite taps are derived on the host (double precision)
-//     by pushing an impulse through the stages; the stages' own zero padding only disturbs samples inside the
-//     `indent` that :88 trims away (reach 341 samples < indent 550 for factors (5,5,11)).
+//     by pushing an impulse through the stages.  The stages' own zero padding only disturbs samples inside the
+//     `indent` = pad * hop that :88 trims away whenever pad >= 1: the padded frame sequence then starts and ends with a
+//     zero frame, and what each stage loses past the ends of its input reaches less than one frame into the output.
+//     This holds even where the composite reach exceeds the indent (341 samples > 275 for factors (5,5,11) at pad 1);
+//     pad = 0 is refused at create time (the reference's trim [indent:-indent] is then empty).
 #pragma once
 #include "common.cuh"
 

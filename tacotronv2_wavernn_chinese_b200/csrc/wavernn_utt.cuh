@@ -85,6 +85,11 @@ inline size_t utt_smem_floats(const StepWeights& W, int G) {
   return (size_t)G * (W.ldI + W.R + 2 * W.R + 2 * W.R + KX + KX + KF + W.F + W.NC);
 }
 
+// Host side: whether G rows per CTA fit the 227 KB of shared memory a CTA may have, the static `red` array of utt_run included.
+inline bool utt_fits(const StepWeights& W, int G) {
+  return utt_smem_floats(W, G) * sizeof(float) + (size_t)G * (kUttThreads / 32) * sizeof(unsigned long long) <= 227 * 1024;
+}
+
 // The whole loop; MOL selects the sampler (fc3 then has NC = 32 rows, the 30 parameters padded to whole quads).
 template <int G, bool MOL>
 __device__ __forceinline__ void utt_run(StepWeights W, GenArgs A, MolIO M) {
