@@ -231,6 +231,24 @@ int b200tts_wavernn_session_run(b200tts_wavernn* ctx, b200tts_wavernn_session* c
 /* The most sessions one session_run takes on ctx: 256 where the tensor-core pipeline runs (kernel=tc), else 32. */
 int b200tts_wavernn_session_max_rows(const b200tts_wavernn* ctx);
 
+/* Batched open: n sessions in three launches whatever n is (mel preparation, MelResNet and the conditioning tables, each over the
+ * rows' own frame counts), with no host copy of the mels.  Session i is bit for bit the session b200tts_wavernn_session_open_kernel
+ * opens from row i's mel in [0, 1], zero-padded to max(h_frames[i], 21) frames, with the same seed, id, mu_law and kernel: its
+ * pieces concatenate to that one-shot run.
+ *   d_mel, layout B200TTS_MEL_FEAT_T: [n][feat][T_max], in [0, 1].
+ *          layout B200TTS_MEL_TACO:   [n][T_max][feat], the Tacotron postnet output, mapped on the device with the float32
+ *          statements of the reference's synthesizer: m = clip(m, -max_abs_value, max_abs_value), clip((m + a) / (2a), 0, 1).
+ *   h_frames [n] (host): frames of each row, 1..T_max; rows shorter than 21 frames get zero frames (in [0, 1]) up to 21.
+ *   n: 1..b200tts_wavernn_session_max_rows(ctx).  rng: PHILOX; session i's utterance id is d_utterance_ids[i] (device memory,
+ *   read back in stream order, which synchronises `stream`) or utterance_offset + i.  kernel: B200TTS_KERNEL_AUTO (push) or
+ *   B200TTS_KERNEL_TC.  out[n] receives the sessions, on success only.
+ * The sessions of one call share one allocation, freed when the last of them is destroyed.  Bad arguments return B200TTS_EINVAL
+ * before any CUDA call, with the refusals of session_open_kernel. */
+enum { B200TTS_MEL_FEAT_T = 0, B200TTS_MEL_TACO = 1 };
+int b200tts_wavernn_session_open_batch(b200tts_wavernn* ctx, const float* d_mel, int layout, float max_abs_value,
+                                       const int32_t* h_frames, int n, int T_max, const b200tts_rng* rng, int mu_law, int kernel,
+                                       b200tts_wavernn_session** out, void* stream);
+
 /* Measured fp32 CUDA-core ceiling of `device` in TFLOP/s (register-only packed FFMA2 loop on every SM): the denominator
  * of bench.py's FLOP-form roofline. */
 int b200tts_debug_fp32_peak(int device, double* tflops);
@@ -309,6 +327,11 @@ int b200tts_taco_encode(b200tts_taco* ctx, const int32_t* d_ids, const int32_t* 
                         void* stream);
 int b200tts_taco_postnet(b200tts_taco* ctx, const float* d_frames, const int32_t* d_nsteps, int B, int max_steps, float* d_mel,
                          void* stream);
+
+/* The reference synthesizer's cut of a free run (tacotron_synthesize.py:104-105): d_len[b] = the first step t < nsteps[b] whose
+ * np.round(stop) is 1, i.e. stop > 0.5 (np.round(0.5) is 0), else nsteps[b].  d_stop [B][max_steps], d_nsteps [B] as
+ * b200tts_taco_decode writes them; nsteps is clamped to max_steps, and a negative nsteps (a failed decode) is passed through. */
+int b200tts_taco_target_lengths(const float* d_stop, const int32_t* d_nsteps, int B, int max_steps, int32_t* d_len, void* stream);
 
 /* The keep flags the PHILOX dropout mode draws: d_masks [B][steps][2][prenet_units]. */
 int b200tts_taco_philox_masks(int device, uint64_t seed, uint64_t utterance_offset, int B, int steps, int prenet_units,

@@ -17,6 +17,7 @@ OK = 0
 RNG_PHILOX, RNG_EXT_EXPONENTIAL, RNG_EXT_UNIFORM = 0, 1, 2
 KERNEL_AUTO, KERNEL_UTTERANCE, KERNEL_GRID, KERNEL_TC = 0, 1, 2, 3
 KERNELS = {'auto': KERNEL_AUTO, 'utterance': KERNEL_UTTERANCE, 'grid': KERNEL_GRID, 'tc': KERNEL_TC}
+MEL_LAYOUTS = {'feat_t': 0, 'taco': 1}      # B200TTS_MEL_FEAT_T, B200TTS_MEL_TACO
 
 
 class B200TTSError(RuntimeError):
@@ -110,6 +111,8 @@ SIGNATURES = {
     'b200tts_wavernn_session_open_kernel': (C.c_int, [C.c_void_p, C.c_void_p, C.c_int, C.POINTER(Rng), C.c_int, C.c_int,
                                                       C.POINTER(C.c_void_p), C.c_void_p]),
     'b200tts_wavernn_session_max_rows': (C.c_int, [C.c_void_p]),
+    'b200tts_wavernn_session_open_batch': (C.c_int, [C.c_void_p, C.c_void_p, C.c_int, C.c_float, C.POINTER(C.c_int32), C.c_int,
+                                                     C.c_int, C.POINTER(Rng), C.c_int, C.c_int, C.POINTER(C.c_void_p), C.c_void_p]),
     'b200tts_wavernn_session_destroy': (None, [C.c_void_p]),
     'b200tts_wavernn_session_info': (C.c_int, [C.c_void_p, C.POINTER(C.c_int64), C.POINTER(C.c_int64), C.POINTER(C.c_int64)]),
     'b200tts_wavernn_session_run': (C.c_int, [C.c_void_p, C.POINTER(C.c_void_p), C.c_int, C.c_int, C.c_void_p, C.c_void_p,
@@ -125,6 +128,7 @@ SIGNATURES = {
                                           C.c_void_p, C.c_int, C.c_void_p, C.c_void_p, C.c_void_p]),
     'b200tts_taco_encode': (C.c_int, [C.c_void_p, C.c_void_p, C.c_void_p, C.c_int, C.c_int, C.c_void_p, C.c_void_p]),
     'b200tts_taco_postnet': (C.c_int, [C.c_void_p, C.c_void_p, C.c_void_p, C.c_int, C.c_int, C.c_void_p, C.c_void_p]),
+    'b200tts_taco_target_lengths': (C.c_int, [C.c_void_p, C.c_void_p, C.c_int, C.c_int, C.c_void_p, C.c_void_p]),
     'b200tts_taco_philox_masks': (C.c_int, [C.c_int, C.c_uint64, C.c_uint64, C.c_int, C.c_int, C.c_int, C.c_void_p, C.c_void_p]),
     'b200tts_gl_create': (C.c_int, [C.POINTER(C.c_void_p), C.c_int, C.POINTER(GlCfg), C.c_void_p]),
     'b200tts_gl_destroy': (None, [C.c_void_p]),

@@ -382,6 +382,29 @@ extern "C" int b200tts_taco_philox_masks(int device, uint64_t seed, uint64_t utt
   API_END
 }
 
+// One block per sentence: the first step whose stop token exceeds 0.5.
+__global__ void taco_target_lengths_kernel(const float* __restrict__ stop, const int32_t* __restrict__ nsteps, int max_steps,
+                                           int32_t* __restrict__ len) {
+  __shared__ int first;
+  const int b = blockIdx.x, n = min(nsteps[b], max_steps);
+  if (threadIdx.x == 0) first = n;
+  __syncthreads();
+  for (int t = threadIdx.x; t < n; t += blockDim.x)
+    if (stop[(size_t)b * max_steps + t] > 0.5f) atomicMin(&first, t);
+  __syncthreads();
+  if (threadIdx.x == 0) len[b] = first;
+}
+
+extern "C" int b200tts_taco_target_lengths(const float* d_stop, const int32_t* d_nsteps, int B, int max_steps, int32_t* d_len,
+                                           void* stream) {
+  API_BEGIN
+  REQUIRE(d_stop && d_nsteps && d_len, B200TTS_EINVAL, "null argument");
+  REQUIRE(B >= 1 && max_steps >= 1, B200TTS_EINVAL, "B / max_steps out of range");
+  taco_target_lengths_kernel<<<B, 256, 0, (cudaStream_t)stream>>>(d_stop, d_nsteps, max_steps, d_len);
+  B200_CUDA(cudaGetLastError());
+  API_END
+}
+
 static void taco_launch_conv(b200tts_taco* ctx, const TacoConvW& cw, const float* x, const int* ids, const int* lengths, int B, int Tmax,
                              int act, bool clip_in, float lo, float hi, float* y, cudaStream_t st) {
   ConvArgs a{};

@@ -6,6 +6,7 @@
 #include <cmath>
 #include <cstdio>
 #include <cstdlib>
+#include <memory>
 #include <set>
 
 #include "api.h"
@@ -14,6 +15,7 @@
 #include "wavernn_grid.cuh"
 #include "wavernn_push.cuh"
 #include "wavernn_tc.cuh"
+#include "wavernn_open.cuh"
 
 using namespace b200tts;
 
@@ -26,7 +28,10 @@ struct b200tts_wavernn_session {
   int T = 0, mu_law = 1;
   int64_t pos = 0, S = 0, wave_len = 0;     // next step; steps of the utterance; samples of its wave
   uint64_t seed = 0, id = 0;
-  DeviceBuf tab, state;
+  DeviceBuf tab, state;                     // session_open(_kernel): memory of this session alone
+  std::shared_ptr<DeviceBuf> batch;         // session_open_batch: one allocation for the batch, freed with its last session
+  float* tab_p = nullptr;                   // the tables and the state, in `tab` / `state` or in `batch`
+  float* state_p = nullptr;
 };
 
 struct b200tts_wavernn {
@@ -1083,13 +1088,111 @@ extern "C" int b200tts_wavernn_session_open_kernel(b200tts_wavernn* ctx, const f
   // tables, which the session owns (the next generate overwrites every scratch buffer)
   ctx->aux_frames.ensure((size_t)T * ctx->cfg.res_out_dims * sizeof(float));
   run_upsample(ctx, d_mel, 1, T, nullptr, ctx->aux_frames.as<float>(), nullptr, st);
-  launch_cond_table(ctx, d_mel, ctx->aux_frames.as<float>(), 1, 1, T, s->tab, st);
+  s->tab_p = const_cast<float*>(launch_cond_table(ctx, d_mel, ctx->aux_frames.as<float>(), 1, 1, T, s->tab, st));
+  s->state_p = s->state.as<float>();
   ctx->sessions.insert(s.get());
   *out = s.release();
   API_END
 }
 
-// cudaFree waits for the work queued on the device, so no run still in flight reads the memory freed here.
+// n sessions in three launches (wavernn_open.cuh), bit for bit the sessions session_open_kernel opens one by one from the same mels.
+// Their tables and states share one allocation: a one-by-one open spends two cudaMalloc on every session (DESIGN 3.11.1).
+extern "C" int b200tts_wavernn_session_open_batch(b200tts_wavernn* ctx, const float* d_mel, int layout, float max_abs_value,
+                                                  const int32_t* h_frames, int n, int T_max, const b200tts_rng* rng, int mu_law,
+                                                  int kernel, b200tts_wavernn_session** out, void* stream) {
+  API_BEGIN
+  REQUIRE(ctx && d_mel && h_frames && rng && out, B200TTS_EINVAL, "null argument");
+  require_session_model(ctx);
+  REQUIRE(kernel == B200TTS_KERNEL_AUTO || kernel == B200TTS_KERNEL_TC, B200TTS_EINVAL,
+          "a session runs on kernel = AUTO (the push kernel) or TC (the tensor cores)");
+  const bool tc = kernel == B200TTS_KERNEL_TC;
+  REQUIRE(!tc || ctx->tc_ok, B200TTS_EINVAL, "tensor-core sessions need a model and device that run kernel=tc (rnn_dims = fc_dims = "
+                                             "512, 10-bit classes, hop_length x FIR taps <= 8192, >= 128 SMs)");
+  REQUIRE(rng->mode == B200TTS_RNG_PHILOX, B200TTS_EINVAL,
+          "sessions take PHILOX noise keyed by (seed, utterance id: d_utterance_ids[i], or utterance_offset + i)");
+  REQUIRE(layout == B200TTS_MEL_FEAT_T || layout == B200TTS_MEL_TACO, B200TTS_EINVAL,
+          "unknown mel layout (B200TTS_MEL_FEAT_T or B200TTS_MEL_TACO)");
+  REQUIRE(layout != B200TTS_MEL_TACO || (std::isfinite(max_abs_value) && max_abs_value > 0.f), B200TTS_EINVAL,
+          "max_abs_value must be positive and finite");
+  REQUIRE(n >= 1 && n <= b200tts_wavernn_session_max_rows(ctx), B200TTS_EINVAL, "n must be 1..session_max_rows");
+  REQUIRE(T_max >= 1, B200TTS_EINVAL, "T_max must be >= 1");
+  const int hop = ctx->cfg.hop_length, FEAT = ctx->cfg.feat_dims, O = ctx->cfg.res_out_dims, ncta = ctx->pm.ncta;
+  OpenRows R{};
+  R.n = n;
+  size_t tab_floats = 0;
+  for (int i = 0; i < n; ++i) {
+    REQUIRE(h_frames[i] >= 1 && h_frames[i] <= T_max, B200TTS_EINVAL, "every row needs 1..T_max frames");
+    const int T = std::max(h_frames[i], 21);     // zero-padded to the 21 frames the 20-hop fade-out needs, as StreamingVocoder pads
+    REQUIRE((long long)T * hop <= INT_MAX, B200TTS_EINVAL, "utterance longer than 2^31 - 1 samples");
+    R.frames[i] = h_frames[i];
+    R.T[i] = T;
+    REQUIRE((long long)R.f0[i] + T <= INT_MAX / std::max(FEAT, O), B200TTS_EINVAL, "mels too long for one batch");
+    R.f0[i + 1] = R.f0[i] + T;
+    R.res0[i + 1] = R.res0[i] + (T + kOpenFT - 1) / kOpenFT;
+    R.tab0[i + 1] = R.tab0[i] + (T + 1 + kOpenFT - 1) / kOpenFT;
+    tab_floats += (size_t)(T + 1) * ncta * kPushCondRows;
+  }
+  DeviceGuard dg(ctx->device);
+  const cudaStream_t st = (cudaStream_t)stream;
+  std::vector<uint64_t> ids(n);
+  if (rng->d_utterance_ids) {       // the run kernels take each session's id as a parameter: read them back, in stream order
+    B200_CUDA(cudaMemcpyAsync(ids.data(), rng->d_utterance_ids, n * sizeof(uint64_t), cudaMemcpyDeviceToHost, st));
+    B200_CUDA(cudaStreamSynchronize(st));
+  } else {
+    for (int i = 0; i < n; ++i) ids[i] = rng->utterance_offset + (uint64_t)i;
+  }
+  // one allocation: the n tables, then the n states (each state 256-byte aligned)
+  const size_t state_floats = ((size_t)kSessStateFloats + 63) / 64 * 64;
+  auto block = std::make_shared<DeviceBuf>();
+  block->ensure((tab_floats + (size_t)n * state_floats) * sizeof(float));
+  float* base = block->as<float>();
+  std::vector<std::unique_ptr<b200tts_wavernn_session>> ss(n);
+  size_t off = 0;
+  for (int i = 0; i < n; ++i) {
+    ss[i].reset(new b200tts_wavernn_session());
+    b200tts_wavernn_session& s = *ss[i];
+    s.ctx = ctx;
+    s.tc = tc;
+    s.T = R.T[i];
+    s.mu_law = mu_law ? 1 : 0;
+    s.S = (int64_t)R.T[i] * hop;
+    s.wave_len = (int64_t)(R.T[i] - 1) * hop;
+    s.seed = rng->seed;
+    s.id = ids[i];
+    s.batch = block;
+    s.tab_p = R.tab[i] = base + off;
+    s.state_p = base + tab_floats + (size_t)i * state_floats;
+    off += (size_t)(R.T[i] + 1) * ncta * kPushCondRows;
+  }
+  // the prepared mels and MelResNet's output go to the context's scratch, consumed in stream order by the table launch
+  const int frames = R.f0[n];
+  ctx->mel_in.ensure((size_t)frames * FEAT * sizeof(float));
+  ctx->aux_frames.ensure((size_t)frames * O * sizeof(float));
+  float* mel = ctx->mel_in.as<float>();
+  float* aux = ctx->aux_frames.as<float>();
+  session_mel_prep_kernel<<<dim3((unsigned)std::min((FEAT * 2048 + 255) / 256, 64), n), 256, 0, st>>>(
+      d_mel, layout, T_max, FEAT, max_abs_value, R, mel);
+  B200_CUDA(cudaGetLastError());
+  const b200tts_wavernn_cfg& c = ctx->cfg;
+  const int threads = ((std::max(c.compute_dims, 32) + 31) / 32) * 32;
+  const size_t res_smem = ((size_t)c.feat_dims * (2 * c.pad + 1) * kOpenFT + 2 * (size_t)c.compute_dims * kOpenFT) * sizeof(float);
+  if (res_smem > 48 * 1024)
+    B200_CUDA(cudaFuncSetAttribute(melresnet_ragged_kernel<kOpenFT>, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)res_smem));
+  melresnet_ragged_kernel<kOpenFT><<<R.res0[n], threads, res_smem, st>>>(ctx->rp, mel, R, aux);
+  B200_CUDA(cudaGetLastError());
+  const size_t tab_smem = (size_t)(FEAT + O) * kOpenFT * sizeof(float);
+  push_cond_table_ragged_kernel<kOpenFT><<<R.tab0[n], 256, tab_smem, st>>>(ctx->pcw, mel, aux, R);
+  B200_CUDA(cudaGetLastError());
+  ctx->launches += 3;
+  for (int i = 0; i < n; ++i) {
+    ctx->sessions.insert(ss[i].get());
+    out[i] = ss[i].release();
+  }
+  API_END
+}
+
+// cudaFree waits for the work queued on the device, so no run still in flight reads the memory freed here (a batch's memory is
+// freed with the last of its sessions).
 extern "C" void b200tts_wavernn_session_destroy(b200tts_wavernn_session* s) {
   if (!s) return;
   DeviceGuard dg(s->ctx->device, true);
@@ -1132,8 +1235,8 @@ extern "C" int b200tts_wavernn_session_run(b200tts_wavernn* ctx, b200tts_wavernn
   int steps = 0;
   for (int i = 0; i < n; ++i) {
     SessRow& r = io.row[i];
-    r.tab = s[i]->tab.as<float>();
-    r.state = s[i]->state.as<float>();
+    r.tab = s[i]->tab_p;
+    r.state = s[i]->state_p;
     r.seed = s[i]->seed;
     r.id = s[i]->id;
     r.T = s[i]->T;

@@ -368,14 +368,14 @@ struct PushCondW {
   const float* bias;    // [ncta][36]
   int ncta, feat, aux;
 };
+// Frames [f0, f0 + FT) of table row u (rows u >= B are zero).
 template <int FT>
-__global__ void push_cond_table_kernel(PushCondW W, const float* __restrict__ mel /*[B][feat][T]*/,
-                                       const float* __restrict__ aux_frames /*[B][T][4*aux]*/, int B, int T,
-                                       float* __restrict__ tab /*[Brows][T+1][ncta][52]*/) {
+__device__ __forceinline__ void push_cond_table_tile(const PushCondW& W, const float* __restrict__ mel /*[B][feat][T]*/,
+                                                     const float* __restrict__ aux_frames /*[B][T][4*aux]*/, int B, int T, int u,
+                                                     int f0, float* __restrict__ tab /*[Brows][T+1][ncta][52]*/) {
   extern __shared__ float sm[];
   float* sm_mel = sm;                          // [feat][FT]
   float* sm_aux = sm + W.feat * FT;            // [4*aux][FT]
-  const int u = blockIdx.y, f0 = blockIdx.x * FT;
   const int O = 4 * W.aux;
   const bool real = u < B;
   for (int i = threadIdx.x; i < W.feat * FT; i += blockDim.x) {
@@ -429,6 +429,13 @@ __global__ void push_cond_table_kernel(PushCondW W, const float* __restrict__ me
       if (ff <= T) tab[(((size_t)u * (T + 1) + ff) * W.ncta + c) * kPushCondRows + row] = (row < 16 && ff >= T) ? 0.f : acc[i];
     }
   }
+}
+
+template <int FT>
+__global__ void push_cond_table_kernel(PushCondW W, const float* __restrict__ mel /*[B][feat][T]*/,
+                                       const float* __restrict__ aux_frames /*[B][T][4*aux]*/, int B, int T,
+                                       float* __restrict__ tab /*[Brows][T+1][ncta][52]*/) {
+  push_cond_table_tile<FT>(W, mel, aux_frames, B, T, blockIdx.y, blockIdx.x * FT, tab);
 }
 
 // fills the exchange buffers with the sentinel pattern and clears the winner slots and, if given, the error flag

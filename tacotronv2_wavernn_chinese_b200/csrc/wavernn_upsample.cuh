@@ -28,16 +28,16 @@ struct ResnetParams {
   int feat, k, C, O, blocks, pad;
 };
 
-// One CTA = FT frames of one utterance; thread c owns channel c for all FT frames.
+// Frames [f0, f0 + FT) of utterance b; thread c owns channel c for all FT frames.
 template <int FT>
-__global__ void melresnet_kernel(ResnetParams P, const float* __restrict__ mel /*[B][feat][T]*/,
-                                                        int T, float* __restrict__ aux_frames /*[B][T][O]*/) {
+__device__ __forceinline__ void melresnet_tile(const ResnetParams& P, const float* __restrict__ mel /*[B][feat][T]*/, int T, int b,
+                                               int f0, float* __restrict__ aux_frames /*[B][T][O]*/) {
   extern __shared__ float sm[];
   const int C = P.C;
   float* xin = sm;                              // [feat*k][FT]
   float* act = xin + P.feat * P.k * FT;         // [C][FT]
   float* tmp = act + C * FT;                    // [C][FT]
-  const int b = blockIdx.y, f0 = blockIdx.x * FT, c = threadIdx.x;
+  const int c = threadIdx.x;
   const float* melb = mel + (size_t)b * P.feat * T;
   // gather the k-frame windows; frame index into the padded sequence is f + j, i.e. unpadded f + j - pad
   for (int e = threadIdx.x; e < P.feat * P.k * FT; e += blockDim.x) {
@@ -104,6 +104,13 @@ __global__ void melresnet_kernel(ResnetParams P, const float* __restrict__ mel /
     for (int t = 0; t < FT; ++t)
       if (f0 + t < T) aux_frames[((size_t)b * T + f0 + t) * P.O + o] = acc[t] + bias;
   }
+}
+
+// One CTA = FT frames of one utterance.
+template <int FT>
+__global__ void melresnet_kernel(ResnetParams P, const float* __restrict__ mel /*[B][feat][T]*/,
+                                                        int T, float* __restrict__ aux_frames /*[B][T][O]*/) {
+  melresnet_tile<FT>(P, mel, T, blockIdx.y, blockIdx.x * FT, aux_frames);
 }
 
 // mels_up[b][n][c] = sum_j fir[ph][j] * melpad[b][c][fr + j - NT/2],  n' = n + pad*hop, fr = n'/hop, ph = n'%hop

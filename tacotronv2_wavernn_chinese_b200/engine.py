@@ -240,6 +240,46 @@ class WaveRNNEngine:
         self._sessions.add(s)
         return s
 
+    def open_sessions(self, mels, frames, *, seed: int = 0, utterance_ids, mu_law: bool = True, kernel: str = 'auto',
+                      layout: str = 'feat_t', max_abs_value: float = 4.0) -> list:
+        """n generation sessions opened in three launches, whatever n is (b200tts_wavernn_session_open_batch); device tensors are
+        read in place.  Session i is bit for bit `open_session` of row i's first frames[i] frames, zero-padded to 21 frames
+        when shorter, with utterance_id utterance_ids[i].
+
+        layout 'feat_t': mels [n, feat, T_max] in [0, 1].  layout 'taco': mels [n, T_max, feat], the Tacotron postnet output,
+        mapped on the device like Synthesizer.mels: clip(m, -max_abs_value, max_abs_value), then clip((m + a) / (2a), 0, 1).
+        frames: n ints in 1..T_max (host).  n is 1..max_session_rows; kernel 'auto' (push) or 'tc'."""
+        if kernel not in ('auto', 'tc'):
+            raise ValueError(f"kernel must be 'auto' (push) or 'tc', got {kernel!r}")
+        if layout not in _lib.MEL_LAYOUTS:
+            raise ValueError(f"layout must be 'feat_t' or 'taco', got {layout!r}")
+        m = torch.as_tensor(mels)
+        if m.dim() != 3 or m.shape[1 if layout == 'feat_t' else 2] != self.feat:
+            want = f'[n, {self.feat}, T_max]' if layout == 'feat_t' else f'[n, T_max, {self.feat}]'
+            raise ValueError(f'mels must be {want} for layout {layout!r}, got {tuple(m.shape)}')
+        n = int(m.shape[0])
+        T_max = int(m.shape[2 if layout == 'feat_t' else 1])
+        fr = np.ascontiguousarray(np.asarray(frames).reshape(-1), dtype=np.int32)
+        ids = [int(u) & 0xFFFFFFFFFFFFFFFF for u in utterance_ids]
+        if len(fr) != n or len(ids) != n:
+            raise ValueError(f'need one frame count and one utterance id per row ({n} rows)')
+        with torch.cuda.device(self.device):
+            m = m.to(device=self._dev(), dtype=torch.float32).contiguous()
+            d_ids = torch.tensor(np.array(ids, dtype=np.uint64).view(np.int64), device=self._dev())
+            rng = _rng(_lib.RNG_PHILOX, seed, 0)
+            rng.d_utterance_ids = d_ids.data_ptr()
+            handles = (C.c_void_p * n)()
+            _lib.check(self.lib.b200tts_wavernn_session_open_batch(
+                self._h, _ptr(m), _lib.MEL_LAYOUTS[layout], float(max_abs_value), fr.ctypes.data_as(C.POINTER(C.c_int32)), n,
+                T_max, C.byref(rng), 1 if mu_law else 0, _lib.KERNELS[kernel], handles, self._stream()))
+            m.record_stream(torch.cuda.current_stream(self.device))
+        out = []
+        for h in handles:
+            s = WaveRNNSession(self, C.c_void_p(h))
+            self._sessions.add(s)
+            out.append(s)
+        return out
+
     def advance(self, sessions, max_steps: int):
         """Runs up to `max_steps` more steps of each session in one launch: 1..32 distinct open push sessions of this engine, or
         1..`max_session_rows` tensor-core sessions with `max_steps` a multiple of hop.

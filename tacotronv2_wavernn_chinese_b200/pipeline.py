@@ -255,6 +255,113 @@ class StreamingVocoder:
         return out
 
 
+class StreamingSynthesizer:
+    """Text in, audio pieces out: continuous batching of text requests through Tacotron and vocoder sessions on one GPU.
+    `submit` queues a pinyin text; every `step`
+      * admits queued texts first come, first served, up to min(free rows, `max_admit`), and gives them ONE Tacotron batch
+        (encode, decode, postnet: `synth.decode_device`), one device-side stop-token cut (`target_lengths`) and one batched
+        session open from the postnet output (`engine.open_sessions(layout='taco')`), so no mel goes through the host;
+      * advances every active session by up to `chunk_steps` samples in one launch,
+    and returns [(key, wave piece float64 numpy, finished)] in admission order, like StreamingVocoder.step.  A request's mel is
+    `Synthesizer.mels` of its admission group with the same ids, and its pieces concatenate to the one-shot generate of that mel
+    (zero-padded to 21 frames when shorter) with (seed, utterance_id) on the same kernel family.  A sentence whose stop token
+    fires at its first step has an empty mel: it finishes at admission with an empty piece, after the pieces of the sessions.
+
+    Everything runs on the current stream, in order: the Tacotron kernels never run beside the vocoder's persistent kernels,
+    whose co-residency on the SMs they could break.  `max_rows` > 32 runs tensor-core sessions, and `chunk_steps` must then be
+    a multiple of the engine's hop."""
+
+    def __init__(self, synth, engine, seed=0, chunk_steps=2750, max_rows=32, max_admit=None):
+        cap = int(getattr(engine, 'max_session_rows', 32))
+        if not 1 <= int(max_rows) <= cap:
+            raise ValueError(f'max_rows must be 1..{cap} (the most sessions one launch of this engine takes)')
+        if int(chunk_steps) < 1:
+            raise ValueError('chunk_steps must be >= 1')
+        if max_admit is not None and int(max_admit) < 1:
+            raise ValueError('max_admit must be >= 1 (or None: as many as there are free rows)')
+        self.synth, self.engine, self.seed = synth, engine, int(seed)
+        self.chunk_steps, self.max_rows = int(chunk_steps), int(max_rows)
+        self.max_admit = None if max_admit is None else int(max_admit)
+        self._tc = self.max_rows > 32                       # the push kernel runs at most 32 sessions per launch
+        if self._tc and self.chunk_steps % int(engine.hop):
+            raise ValueError(f'above 32 rows the sessions run on the tensor cores: chunk_steps must be a multiple of hop ({engine.hop})')
+        self._queue = collections.deque()       # (key, text, utterance id)
+        self._active = []                       # (key, session) in admission order
+        self._mels = {}                         # key -> (postnet output of its batch, row, frames)
+        self._gone = []                         # keys whose last piece the previous step returned
+
+    def submit(self, key, text, utterance_id):
+        """Queues a pinyin text; its prenet dropout and sampling noise are keyed by (seed, utterance_id).  A text the encoder
+        would refuse, more than MAX_TOKENS symbols with its end mark, is refused here."""
+        from .tacotron.engine import MAX_TOKENS
+        n = len(self.synth.symbols.text_to_sequence(text))
+        if n > MAX_TOKENS:
+            raise ValueError(f'text of {n} symbols: the encoder takes at most {MAX_TOKENS}')
+        self._queue.append((key, text, int(utterance_id)))
+
+    @property
+    def pending(self) -> int:
+        return len(self._queue)
+
+    @property
+    def active(self) -> int:
+        return len(self._active)
+
+    def idle(self) -> bool:
+        return not self._queue and not self._active
+
+    def mel(self, key):
+        """The [T, 80] float32 mel in [0, 1] of an admitted request, until the step after the one that returned its last piece."""
+        from .tacotron.synthesizer import unit_mel
+        post, b, frames = self._mels[key]
+        return unit_mel(_host(post[b, :frames]))
+
+    def _admit(self):
+        k = min(len(self._queue), self.max_rows - len(self._active))
+        if self.max_admit is not None:
+            k = min(k, self.max_admit)
+        if k <= 0:
+            return []
+        batch = [self._queue.popleft() for _ in range(k)]
+        keys = [b[0] for b in batch]
+        ids = [b[2] for b in batch]
+        post, lens = self.synth.decode_device([b[1] for b in batch], ids, seed=self.seed)
+        frames = [int(f) for f in _host(lens)]
+        if min(frames) < 0:
+            raise RuntimeError('Tacotron decoder kernel gave up waiting for a peer thread block (nsteps < 0); results are invalid')
+        for b, key in enumerate(keys):
+            self._mels[key] = (post, b, frames[b])
+        rows = [b for b in range(k) if frames[b] > 0]
+        if rows:
+            mels = post if len(rows) == k else post[rows]
+            sessions = self.engine.open_sessions(mels, [frames[b] for b in rows], seed=self.seed, utterance_ids=[ids[b] for b in rows],
+                                                 kernel='tc' if self._tc else 'auto', layout='taco')
+            self._active += [(keys[b], s) for b, s in zip(rows, sessions)]
+        return [(keys[b], np.zeros(0, dtype=np.float64), True) for b in range(k) if frames[b] == 0]
+
+    def step(self):
+        for key in self._gone:
+            self._mels.pop(key, None)
+        empty = self._admit()
+        out, still = [], []
+        if self._active:
+            pieces = self.engine.advance([s for _, s in self._active], self.chunk_steps)
+            for (key, s), (_labels, wave) in zip(self._active, pieces):
+                finished = s.done
+                out.append((key, _host(wave), finished))
+                if finished:
+                    s.close()
+                else:
+                    still.append((key, s))
+        self._active = still
+        out += empty
+        self._gone = [key for key, _piece, finished in out if finished]
+        check = getattr(self.engine, 'check', None)
+        if out and check is not None:
+            check()                              # a timed-out run raises here instead of handing out NaN audio
+        return out
+
+
 def synthesize_stream(synth, wavernn_engine, text, seed=0, utterance_id=0, chunk_steps=2750):
     """One sentence as a stream: yields its Tacotron mel [T, 80] first, then its wave pieces (float64 numpy) as the vocoder
     makes them.  The pieces concatenate to synthesize_batch's wave of the sentence with utterance_offset = utterance_id."""

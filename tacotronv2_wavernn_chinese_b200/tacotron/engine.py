@@ -9,6 +9,8 @@ import torch
 from .. import _lib
 from .._lib import TacoCfg, TacoDropout
 
+MAX_TOKENS = 512       # kTacoMaxTx: the longest sentence, in symbols, the encoder and decoders take
+
 DEFAULT_CFG = dict(num_mels=80, prenet_units=256, lstm_units=256, enc_dim=512, attn_dim=128, attn_filters=32,
                    attn_kernel=31, zoneout=0.1)      # tacotron_hparams.py:99-215 of the reference
 
@@ -204,6 +206,24 @@ class TacoDecoderEngine:
             _lib.check(self.lib.b200tts_taco_postnet(self._h, _ptr(f), _ptr(n), B, ms, _ptr(mel), self._stream()))
             f.record_stream(torch.cuda.current_stream(self.device)); n.record_stream(torch.cuda.current_stream(self.device))
         return mel
+
+    def target_lengths(self, stop, nsteps):
+        """The reference's cut of a free run (tacotron_synthesize.py:104-105), on the device: per sentence the first step
+        t < nsteps whose np.round(stop) is 1 (stop > 0.5), else nsteps.  stop [B, max_steps] and nsteps [B] as `decode` returns
+        them -> int32 [B] CUDA tensor (a negative nsteps, a failed decode, is passed through)."""
+        dev = self._dev()
+        st = torch.as_tensor(stop).to(device=dev, dtype=torch.float32).contiguous()
+        if st.dim() != 2 or st.shape[0] < 1 or st.shape[1] < 1:
+            raise ValueError('stop must be [B, max_steps]')
+        B, ms = st.shape
+        n = torch.as_tensor(nsteps).to(device=dev, dtype=torch.int32).contiguous()
+        if tuple(n.shape) != (B,):
+            raise ValueError('nsteps must be [B]')
+        with torch.cuda.device(self.device):
+            out = torch.empty(B, device=dev, dtype=torch.int32)
+            _lib.check(self.lib.b200tts_taco_target_lengths(_ptr(st), _ptr(n), B, ms, _ptr(out), self._stream()))
+            st.record_stream(torch.cuda.current_stream(self.device)); n.record_stream(torch.cuda.current_stream(self.device))
+        return out
 
     def philox_masks(self, seed, utterance_offset, B, steps):
         with torch.cuda.device(self.device):

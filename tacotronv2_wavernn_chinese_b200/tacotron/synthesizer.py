@@ -28,6 +28,12 @@ from .text import Symbols, build_symbols
 MAX_ABS_VALUE = 4.0          # tacotron_hparams.py:99, symmetric_mels=True -> T2_output_range = (-4, 4)
 
 
+def unit_mel(m):
+    """A postnet output [T, 80] (numpy, float32) -> the [0, 1] mel the reference saves (tacotron_synthesize.py:107-108, :115)."""
+    m = np.clip(m, -MAX_ABS_VALUE, MAX_ABS_VALUE)
+    return np.clip((m + MAX_ABS_VALUE) / (2 * MAX_ABS_VALUE), 0, 1).astype(np.float32)
+
+
 class Synthesizer:
     def __init__(self):
         self.engine = None
@@ -77,9 +83,40 @@ class Synthesizer:
         for b in range(B):
             rounded = np.round(stop[b, :n[b]])
             target = int(np.argmax(rounded == 1)) if (rounded == 1).any() else int(n[b])       # :104-105
-            m = np.clip(mel_h[b, :target], -MAX_ABS_VALUE, MAX_ABS_VALUE)                        # :107-108
-            out.append(np.clip((m + MAX_ABS_VALUE) / (2 * MAX_ABS_VALUE), 0, 1).astype(np.float32))   # :115
+            out.append(unit_mel(mel_h[b, :target]))
         return out, dict(decode=dec, memory=mem, lengths=lengths)
+
+    def decode_device(self, texts, ids, seed=0, window=False, max_iters=None):
+        """Batch of pinyin strings -> (postnet output [B, max_iters, 80] on the +-4 scale, target lengths [B] int32), both
+        CUDA tensors: what `mels` computes before its host copy (rows past a sentence's length are unspecified).  The prenet
+        dropout of sentence b is keyed by ids[b], an arbitrary global id, so a sentence's mel does not depend on which others
+        share its batch.  Consecutive ids draw the PHILOX stream directly; otherwise each run of consecutive ids gets its keep
+        flags from philox_masks, which by its contract equal that stream."""
+        seqs = [self.symbols.text_to_sequence(t) for t in texts]
+        ids = [int(i) for i in ids]
+        if len(ids) != len(seqs) or not seqs:
+            raise ValueError('need one id per text, and at least one text')
+        B, Tx = len(seqs), max(len(s) for s in seqs)
+        tok = np.zeros((B, Tx), dtype=np.int32)
+        for b, s in enumerate(seqs):
+            tok[b, :len(s)] = s
+        lengths = np.array([len(s) for s in seqs], dtype=np.int32)
+        eng = self.engine
+        mem = eng.encode(tok, lengths)
+        ms = int(max_iters or self.max_iters)
+        runs = [[ids[0], 1]]
+        for i in ids[1:]:
+            if i == runs[-1][0] + runs[-1][1]:
+                runs[-1][1] += 1
+            else:
+                runs.append([i, 1])
+        if len(runs) == 1:
+            dec = eng.decode(mem, lengths, seed=seed, utterance_offset=ids[0], max_steps=ms, window=window, want_align=False)
+        else:
+            masks = torch.cat([eng.philox_masks(seed, start, count, ms) for start, count in runs])
+            dec = eng.decode(mem, lengths, masks=masks, max_steps=ms, window=window, want_align=False)
+        mel = eng.postnet(dec['frames'], dec['nsteps'])
+        return mel, eng.target_lengths(dec['stop'], dec['nsteps'])
 
     def synthesize(self, text, out_dir, idx, step=None, seed=0):
         step = self.step if step is None else step
