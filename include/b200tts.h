@@ -303,6 +303,19 @@ int b200tts_taco_decode_forced(b200tts_taco* ctx, const float* d_memory, const i
                                const b200tts_taco_dropout* dropout, int n_steps, int window, const float* d_states,
                                float* d_frames, float* d_stop, float* d_align, int32_t* d_nsteps, void* stream);
 
+/* Speaking-rate control: the forward-attention speed bias of attention.py:163-165 / forward_attention.py:163-165 (the branch the
+ * reference ships switched off with `and False`), one bias per sentence.  Sentence b's recursion (attention.py:167) uses
+ *   mu' = clip(mu + h_mu_bias[b], 0, 1)      (fp32 add rounded once, then tf.clip_by_value: min with 1, max with 0)
+ * instead of mu at every step, the first (mu = 0.5) included; the carried mu, the fresh sigmoid of [context | query]
+ * (attention.py:229), stays unbiased, and the window (window != 0) acts on the biased recursion.  Positive biases move attention
+ * on sooner: faster speech, shorter mels; a bias of 0 gives exactly b200tts_taco_decode.  h_mu_bias [B] host floats, each finite
+ * and in [-1, 1] (anything else returns B200TTS_EINVAL before any launch); the library uploads them on `stream`.  d_states NULL
+ * is a free run; otherwise it holds the teacher-forcing records of b200tts_taco_decode_forced with n_steps = max_steps (their mu
+ * is the unbiased one).  Kernel selection, outputs and the remaining arguments are those of b200tts_taco_decode. */
+int b200tts_taco_decode_biased(b200tts_taco* ctx, const float* d_memory, const int32_t* d_lengths, int B, int Tx_max,
+                               const b200tts_taco_dropout* dropout, int max_steps, int window, const float* h_mu_bias,
+                               const float* d_states, float* d_frames, float* d_stop, float* d_align, int32_t* d_nsteps, void* stream);
+
 /* Ground-truth-aligned (GTA) decoding, the teacher-forced loop of wavernn_preprocess.py (TacoTrainingHelper, helpers.py:111-151):
  * the step-t input is d_targets[b][t-1] (the zero GO frame at t = 0) instead of the previous output, and exactly
  * clamp(d_target_lengths[b], 0, Ty_max) steps run.  No stop rule, no inference window (the reference builds this attention with

@@ -73,9 +73,15 @@ def main(argv=None):
     ap.add_argument('--voc_weights', default=None, help='WaveRNN checkpoint: also write the preview wav step-..-wav-from-mel.wav')
     ap.add_argument('--voc_hp_file', default='wavernn_hparams.py', help='WaveRNN hyper-parameter file (with --voc_weights)')
     ap.add_argument('--griffin_lim', action='store_true', help='also write the preview wav step-..-wav-from-mel.wav by Griffin-Lim')
+    ap.add_argument('--mu_bias', type=float, default=0.0,
+                    help='speaking rate: the forward-attention speed bias the reference ships switched off '
+                         '(tacotron/models/attention.py:163-165, delta_val), added to the transition agent mu at every decoder '
+                         'step; finite in [-1, 1], positive is faster (DESIGN.md 3.13 has the measured length response)')
     args = ap.parse_args(argv)
     if args.griffin_lim and args.voc_weights:
         ap.error('--griffin_lim and --voc_weights both choose the preview vocoder; give one')
+    if not (abs(args.mu_bias) <= 1.0):
+        ap.error('--mu_bias must be finite and in [-1, 1]')
     hp = hparams.parse(args.hparams)
     from tacotronv2_wavernn_chinese_b200.tacotron.pinyin import get_pyin
     pyin, text = get_pyin(args.text)                    # reference :187: pinyin feeds the model, the normalised text names the files
@@ -86,7 +92,7 @@ def main(argv=None):
     synth = Synthesizer().load(args.checkpoint, hp, symbols=symbols, train_txt=args.train_txt)
     idx = hashlib.md5(text.encode('utf8')).hexdigest()
     t0 = time.time()
-    mel_path, align_path = synth.synthesize(pyin, args.out_dir, idx, seed=args.seed)
+    mel_path, align_path = synth.synthesize(pyin, args.out_dir, idx, seed=args.seed, mu_bias=args.mu_bias)
     print(f'pred_mel_path: {mel_path}')
     if args.voc_weights:
         print(f'wav_path: {preview_wav(mel_path, args.voc_weights, args.voc_hp_file, hp.sample_rate, args.seed)}')

@@ -124,6 +124,9 @@ SIGNATURES = {
     'b200tts_taco_state_floats': (C.c_int, [C.c_void_p, C.c_int]),
     'b200tts_taco_decode_forced': (C.c_int, [C.c_void_p, C.c_void_p, C.c_void_p, C.c_int, C.c_int, C.POINTER(TacoDropout), C.c_int,
                                              C.c_int, C.c_void_p, C.c_void_p, C.c_void_p, C.c_void_p, C.c_void_p, C.c_void_p]),
+    'b200tts_taco_decode_biased': (C.c_int, [C.c_void_p, C.c_void_p, C.c_void_p, C.c_int, C.c_int, C.POINTER(TacoDropout), C.c_int,
+                                             C.c_int, C.POINTER(C.c_float), C.c_void_p, C.c_void_p, C.c_void_p, C.c_void_p,
+                                             C.c_void_p, C.c_void_p]),
     'b200tts_taco_decode_gta': (C.c_int, [C.c_void_p, C.c_void_p, C.c_void_p, C.c_int, C.c_int, C.POINTER(TacoDropout), C.c_void_p,
                                           C.c_void_p, C.c_int, C.c_void_p, C.c_void_p, C.c_void_p]),
     'b200tts_taco_encode': (C.c_int, [C.c_void_p, C.c_void_p, C.c_void_p, C.c_int, C.c_int, C.c_void_p, C.c_void_p]),

@@ -151,10 +151,14 @@ __device__ __forceinline__ float block_max(float v, float* red) {
 
 // kTeacher = false: free running (b200tts_taco_decode / _decode_forced).  kTeacher = true: GTA (b200tts_taco_decode_gta) --
 // no forced-state reload, no window, no stop projection or rule, no stop / nsteps outputs (A.stop, A.nsteps unused).
-template <bool kTeacher>
-__global__ void __launch_bounds__(kTacoThreads, 1) taco_decoder_kernel(TacoWeights W, TacoArgs A, TacoGtaArgs G) {
+// kBias (free running only): the speaking-rate bias of attention.py:163-165 -- every step's recursion uses
+// mu' = clip(mu + mu_bias[b], 0, 1) instead of mu; the carried mu (s_mu, a forced record's mu) stays unbiased.
+template <bool kTeacher, bool kBias>
+__device__ __forceinline__ void taco_decoder_run(const TacoWeights& W, const TacoArgs& A, const TacoGtaArgs& G, const float* mu_bias) {
   extern __shared__ __align__(1024) float sm[];   // 1024: the base these kernels were settled with (tacotron.cu)
   const int b = blockIdx.x, tid = threadIdx.x;
+  float dmu = 0.f;
+  if constexpr (kBias) dmu = mu_bias[b];
   const int Tx = min(A.lengths[b], A.Tx_max);
   if (Tx < 1) {                                        // empty sentence: nothing to attend to
     if (!kTeacher && tid == 0) A.nsteps[b] = 0;
@@ -300,7 +304,8 @@ __global__ void __launch_bounds__(kTacoThreads, 1) taco_decoder_kernel(TacoWeigh
     float es = 0.f;
     for (int t = tid; t < Tx; t += kTacoThreads) { const float e = expf(al[t] - emax); al[t] = e; es += e; }
     const float esum = block_sum(es, red);
-    const float mu = s_mu;
+    float mu = s_mu;
+    if constexpr (kBias) mu = fmaxf(fminf(__fadd_rn(mu, dmu), 1.f), 0.f);   // tf.clip_by_value(mu + delta, 0, 1): min, then max
     float fs = 0.f;
     for (int t = tid; t < Tx; t += kTacoThreads) {
       const float a = al[t] / esum;
@@ -408,6 +413,16 @@ __global__ void __launch_bounds__(kTacoThreads, 1) taco_decoder_kernel(TacoWeigh
   if constexpr (!kTeacher) {
     if (tid == 0) A.nsteps[b] = step;
   }
+}
+
+template <bool kTeacher>
+__global__ void __launch_bounds__(kTacoThreads, 1) taco_decoder_kernel(TacoWeights W, TacoArgs A, TacoGtaArgs G) {
+  taco_decoder_run<kTeacher, false>(W, A, G, nullptr);
+}
+
+// free or forced run with a per-sentence speaking-rate bias: mu_bias [B] (b200tts_taco_decode_biased)
+__global__ void __launch_bounds__(kTacoThreads, 1) taco_decoder_biased_kernel(TacoWeights W, TacoArgs A, const float* mu_bias) {
+  taco_decoder_run<false, true>(W, A, TacoGtaArgs{}, mu_bias);
 }
 
 // keep flags the PHILOX mode uses, [B][steps][2][P] (lets a test replay them through the oracle)

@@ -139,9 +139,14 @@ __device__ __forceinline__ void tg_gather(const float* src, int n4, PollGuard& p
   }
 }
 
-__global__ void __launch_bounds__(kTgThreads, 1) taco_grid_kernel(TacoGridModel Md, TacoGridArgs A) {
+// kBias: the speaking-rate bias of attention.py:163-165 (see taco_decoder_run); every block applies the same mu_bias[0]
+// redundantly, so alignments and stop decisions still agree bit for bit everywhere.
+template <bool kBias>
+__device__ __forceinline__ void taco_grid_run(const TacoGridModel& Md, const TacoGridArgs& A, const float* mu_bias) {
   extern __shared__ __align__(1024) float sm[];   // 1024: the base these kernels were settled with (tacotron.cu)
   const int tid = threadIdx.x, c = blockIdx.x;
+  float dmu = 0.f;
+  if constexpr (kBias) dmu = mu_bias[0];
   const int M = Md.M, P = Md.P, U = Md.U, E = Md.E, KW = Md.KW;
   const int Tx = min(A.lengths[0], A.Tx), Txp = A.Txp;
   if (Tx < 1) {                                        // empty sentence: nothing to attend to
@@ -363,7 +368,8 @@ __global__ void __launch_bounds__(kTgThreads, 1) taco_grid_kernel(TacoGridModel 
     float es = 0.f;
     for (int t = tid; t < Tx; t += kTgThreads) { const float e = expf(al[t] - emax); al[t] = e; es += e; }
     const float esum = tg_block_sum(es, red);
-    const float mu = s_mu;
+    float mu = s_mu;
+    if constexpr (kBias) mu = fmaxf(fminf(__fadd_rn(mu, dmu), 1.f), 0.f);   // tf.clip_by_value(mu + delta, 0, 1): min, then max
     __syncthreads();
     float fs = 0.f;
     for (int t = tid; t < Tx; t += kTgThreads) {
@@ -440,6 +446,15 @@ __global__ void __launch_bounds__(kTgThreads, 1) taco_grid_kernel(TacoGridModel 
     if (s_stop > 0.5f && !A.forced) { ++step; break; }     // finished = round(stop) (half-to-even -> strictly > 0.5)
   }
   if (tid == 0 && c == 0) A.nsteps[0] = step;
+}
+
+__global__ void __launch_bounds__(kTgThreads, 1) taco_grid_kernel(TacoGridModel Md, TacoGridArgs A) {
+  taco_grid_run<false>(Md, A, nullptr);
+}
+
+// one sentence with a speaking-rate bias: mu_bias [1] (b200tts_taco_decode_biased)
+__global__ void __launch_bounds__(kTgThreads, 1) taco_grid_biased_kernel(TacoGridModel Md, TacoGridArgs A, const float* mu_bias) {
+  taco_grid_run<true>(Md, A, mu_bias);
 }
 
 // a poll that timed out leaves the outputs half written: mark the sentence as failed instead of returning a plausible step count

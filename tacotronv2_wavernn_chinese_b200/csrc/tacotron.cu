@@ -36,6 +36,7 @@ struct b200tts_taco {
   DeviceBuf tg_blob, tg_vec;
   bool tg_ok = false;
   int sm_count = 0;
+  DeviceBuf mu_bias;          // [B] speaking-rate biases of the last b200tts_taco_decode_biased call
 };
 
 // Split-K partials of taco_decoder_kernel, in floats.  The matvecs and the context sum need at most 4096 of them; the attention
@@ -254,9 +255,10 @@ extern "C" void b200tts_taco_destroy(b200tts_taco* ctx) {
   delete ctx;
 }
 
+// h_mu_bias: NULL for the unbiased kernels, else [B] host speaking-rate biases (b200tts_taco_decode_biased)
 static int taco_decode_impl(b200tts_taco* ctx, const float* d_memory, const int32_t* d_lengths, int B, int Tx_max,
-                            const b200tts_taco_dropout* dropout, int max_steps, int window, const float* d_forced, float* d_frames,
-                            float* d_stop, float* d_align, int32_t* d_nsteps, void* stream) {
+                            const b200tts_taco_dropout* dropout, int max_steps, int window, const float* h_mu_bias,
+                            const float* d_forced, float* d_frames, float* d_stop, float* d_align, int32_t* d_nsteps, void* stream) {
   API_BEGIN
   REQUIRE(ctx && d_memory && d_lengths && d_frames && d_stop && d_nsteps, B200TTS_EINVAL, "null argument");
   REQUIRE(B >= 1 && Tx_max >= 1 && Tx_max <= kTacoMaxTx && max_steps >= 1, B200TTS_EINVAL, "B, Tx_max (<= 512), max_steps out of range");
@@ -264,9 +266,19 @@ static int taco_decode_impl(b200tts_taco* ctx, const float* d_memory, const int3
   if (dropout) d = *dropout;
   REQUIRE(d.mode == B200TTS_TACO_DROPOUT_PHILOX || (d.mode == B200TTS_TACO_DROPOUT_EXT && d.d_masks), B200TTS_EINVAL,
           "bad dropout descriptor");
+  if (h_mu_bias)
+    for (int b = 0; b < B; ++b)
+      REQUIRE(std::isfinite(h_mu_bias[b]) && h_mu_bias[b] >= -1.f && h_mu_bias[b] <= 1.f, B200TTS_EINVAL,
+              "mu_bias[" + std::to_string(b) + "] must be finite and in [-1, 1]");
   DeviceGuard dg(ctx->device);
   cudaStream_t st = (cudaStream_t)stream;
   const TacoWeights& w = ctx->tw;
+  const float* d_mu_bias = nullptr;
+  if (h_mu_bias) {
+    ctx->mu_bias.ensure((size_t)B * sizeof(float));
+    B200_CUDA(cudaMemcpyAsync(ctx->mu_bias.p, h_mu_bias, (size_t)B * sizeof(float), cudaMemcpyHostToDevice, st));
+    d_mu_bias = ctx->mu_bias.as<float>();
+  }
   ctx->keys.ensure((size_t)B * Tx_max * w.A * sizeof(float));
   taco_keys_kernel<<<B * Tx_max, 128, w.E * sizeof(float), st>>>(d_memory, w.mem_k, B * Tx_max, w.E, w.A, ctx->keys.as<float>());
   B200_CUDA(cudaGetLastError());
@@ -299,18 +311,24 @@ static int taco_decode_impl(b200tts_taco* ctx, const float* d_memory, const int3
     const size_t fl = (size_t)g.blob + (size_t)(w.P + w.E + w.U) + 2 * w.U + (w.U + w.E) + w.P + 128 + 24 * (size_t)Txp + 176;
     const size_t smem = fl * sizeof(float);
     REQUIRE(smem <= 227 * 1024, B200TTS_EINVAL, "taco_grid_kernel: shared memory budget exceeded");
-    B200_CUDA(cudaFuncSetAttribute(taco_grid_kernel, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)smem));
+    const void* kernel = d_mu_bias ? (const void*)taco_grid_biased_kernel : (const void*)taco_grid_kernel;
+    B200_CUDA(cudaFuncSetAttribute(kernel, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)smem));
     TacoGridModel gm = g;
-    void* args[] = {(void*)&gm, (void*)&ga};
-    B200_CUDA(cudaLaunchCooperativeKernel((const void*)taco_grid_kernel, dim3(kTgCtas), dim3(kTgThreads), args, smem, st));
+    void* args[] = {(void*)&gm, (void*)&ga, (void*)&d_mu_bias};
+    B200_CUDA(cudaLaunchCooperativeKernel(kernel, dim3(kTgCtas), dim3(kTgThreads), args, smem, st));
     taco_grid_finish_kernel<<<1, 1, 0, st>>>(d_err, d_nsteps);
     B200_CUDA(cudaGetLastError());
     ctx->launches += 4;
     return B200TTS_OK;
   }
   const size_t smem = taco_decoder_smem_bytes(w);
-  B200_CUDA(cudaFuncSetAttribute(taco_decoder_kernel<false>, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)smem));
-  taco_decoder_kernel<false><<<B, kTacoThreads, smem, st>>>(w, a, TacoGtaArgs{});
+  if (d_mu_bias) {
+    B200_CUDA(cudaFuncSetAttribute(taco_decoder_biased_kernel, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)smem));
+    taco_decoder_biased_kernel<<<B, kTacoThreads, smem, st>>>(w, a, d_mu_bias);
+  } else {
+    B200_CUDA(cudaFuncSetAttribute(taco_decoder_kernel<false>, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)smem));
+    taco_decoder_kernel<false><<<B, kTacoThreads, smem, st>>>(w, a, TacoGtaArgs{});
+  }
   B200_CUDA(cudaGetLastError());
   ctx->launches += 2;
   API_END
@@ -319,8 +337,20 @@ static int taco_decode_impl(b200tts_taco* ctx, const float* d_memory, const int3
 extern "C" int b200tts_taco_decode(b200tts_taco* ctx, const float* d_memory, const int32_t* d_lengths, int B, int Tx_max,
                                    const b200tts_taco_dropout* dropout, int max_steps, int window, float* d_frames, float* d_stop,
                                    float* d_align, int32_t* d_nsteps, void* stream) {
-  return taco_decode_impl(ctx, d_memory, d_lengths, B, Tx_max, dropout, max_steps, window, nullptr, d_frames, d_stop, d_align, d_nsteps,
-                          stream);
+  return taco_decode_impl(ctx, d_memory, d_lengths, B, Tx_max, dropout, max_steps, window, nullptr, nullptr, d_frames, d_stop, d_align,
+                          d_nsteps, stream);
+}
+
+extern "C" int b200tts_taco_decode_biased(b200tts_taco* ctx, const float* d_memory, const int32_t* d_lengths, int B, int Tx_max,
+                                          const b200tts_taco_dropout* dropout, int max_steps, int window, const float* h_mu_bias,
+                                          const float* d_states, float* d_frames, float* d_stop, float* d_align, int32_t* d_nsteps,
+                                          void* stream) {
+  if (!h_mu_bias) {
+    g_err = "b200tts_taco_decode_biased needs h_mu_bias";
+    return B200TTS_EINVAL;
+  }
+  return taco_decode_impl(ctx, d_memory, d_lengths, B, Tx_max, dropout, max_steps, window, h_mu_bias, d_states, d_frames, d_stop,
+                          d_align, d_nsteps, stream);
 }
 
 extern "C" int b200tts_taco_state_floats(const b200tts_taco* ctx, int Tx_max) {
@@ -335,8 +365,8 @@ extern "C" int b200tts_taco_decode_forced(b200tts_taco* ctx, const float* d_memo
     g_err = "b200tts_taco_decode_forced needs d_states";
     return B200TTS_EINVAL;
   }
-  return taco_decode_impl(ctx, d_memory, d_lengths, B, Tx_max, dropout, n_steps, window, d_states, d_frames, d_stop, d_align, d_nsteps,
-                          stream);
+  return taco_decode_impl(ctx, d_memory, d_lengths, B, Tx_max, dropout, n_steps, window, nullptr, d_states, d_frames, d_stop, d_align,
+                          d_nsteps, stream);
 }
 
 extern "C" int b200tts_taco_decode_gta(b200tts_taco* ctx, const float* d_memory, const int32_t* d_lengths, int B, int Tx_max,

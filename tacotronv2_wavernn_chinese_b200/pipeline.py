@@ -141,20 +141,31 @@ def vocode_ragged(voc, mels, ids, seed=0, max_rows=32, kernel='auto', allow_pack
     return waves
 
 
-def synthesize_batch(synth, wavernn_engine, texts, seed=0, utterance_offset=0, kernel='auto', max_rows=32, allow_pack=True):
+def _rate_kw(mu_bias, n):
+    """The keyword that carries the speaking-rate biases of n sentences to the Synthesizer: none when every bias is 0, so an
+    unbiased call is exactly the call made without biases.  Refuses bad biases (ValueError) before anything runs."""
+    from .tacotron.engine import mu_bias_array
+    b = mu_bias_array(mu_bias, n)
+    return {} if b is None else {'mu_bias': b}
+
+
+def synthesize_batch(synth, wavernn_engine, texts, seed=0, utterance_offset=0, kernel='auto', max_rows=32, allow_pack=True,
+                     mu_bias=None):
     """synth: tacotron.synthesizer.Synthesizer (loaded); wavernn_engine: engine.WaveRNNEngine; texts: pinyin strings.
-    Returns (list of float64 waves, list of mels [T_b, 80]) for sentences utterance_offset ... of a larger set."""
-    mels, _ = synth.mels(texts, seed=seed, utterance_offset=utterance_offset)
+    Returns (list of float64 waves, list of mels [T_b, 80]) for sentences utterance_offset ... of a larger set.
+    mu_bias: speaking-rate bias, a scalar or one per text (Synthesizer.mels; positive speaks faster)."""
+    mels, _ = synth.mels(texts, seed=seed, utterance_offset=utterance_offset, **_rate_kw(mu_bias, len(texts)))
     ids = [utterance_offset + b for b in range(len(mels))]
     return vocode_ragged(wavernn_engine, mels, ids, seed=seed, max_rows=max_rows, kernel=kernel, allow_pack=allow_pack), list(mels)
 
 
-def synthesize_sharded(synth, wavernn_engine, texts, seed=0, group=None, kernel='auto', max_rows=32):
-    """All ranks call this with the SAME `texts`; every rank returns all waves (input order) and all mels.
+def synthesize_sharded(synth, wavernn_engine, texts, seed=0, group=None, kernel='auto', max_rows=32, mu_bias=None):
+    """All ranks call this with the SAME `texts` (and `mu_bias`, a scalar or one speaking-rate bias per text); every rank
+    returns all waves (input order) and all mels.
     One process per GPU (`torch.distributed`); the only collective is the final all-gather of the padded waves."""
     world = dist.get_world_size(group) if dist.is_initialized() else 1
     rank = dist.get_rank(group) if dist.is_initialized() else 0
-    mels, _ = synth.mels(texts, seed=seed, utterance_offset=0)           # replicated (see module docstring)
+    mels, _ = synth.mels(texts, seed=seed, utterance_offset=0, **_rate_kw(mu_bias, len(texts)))   # replicated (module docstring)
     n = len(mels)
     frames = [int(m.shape[0]) for m in mels]
     mine = deal_round_robin(frames, world)[rank]
@@ -285,19 +296,23 @@ class StreamingSynthesizer:
         self._tc = self.max_rows > 32                       # the push kernel runs at most 32 sessions per launch
         if self._tc and self.chunk_steps % int(engine.hop):
             raise ValueError(f'above 32 rows the sessions run on the tensor cores: chunk_steps must be a multiple of hop ({engine.hop})')
-        self._queue = collections.deque()       # (key, text, utterance id)
+        self._queue = collections.deque()       # (key, text, utterance id, speaking-rate bias)
         self._active = []                       # (key, session) in admission order
         self._mels = {}                         # key -> (postnet output of its batch, row, frames)
         self._gone = []                         # keys whose last piece the previous step returned
 
-    def submit(self, key, text, utterance_id):
+    def submit(self, key, text, utterance_id, mu_bias=0.0):
         """Queues a pinyin text; its prenet dropout and sampling noise are keyed by (seed, utterance_id).  A text the encoder
-        would refuse, more than MAX_TOKENS symbols with its end mark, is refused here."""
-        from .tacotron.engine import MAX_TOKENS
+        would refuse, more than MAX_TOKENS symbols with its end mark, is refused here, and so is a speaking-rate bias `mu_bias`
+        that is not a finite number in [-1, 1] (Synthesizer.mels; positive speaks faster)."""
+        from .tacotron.engine import MAX_TOKENS, mu_bias_array
         n = len(self.synth.symbols.text_to_sequence(text))
         if n > MAX_TOKENS:
             raise ValueError(f'text of {n} symbols: the encoder takes at most {MAX_TOKENS}')
-        self._queue.append((key, text, int(utterance_id)))
+        if np.ndim(mu_bias) != 0:
+            raise ValueError('mu_bias of one request must be a number')
+        b = mu_bias_array(mu_bias, 1)
+        self._queue.append((key, text, int(utterance_id), 0.0 if b is None else float(b[0])))
 
     @property
     def pending(self) -> int:
@@ -325,7 +340,8 @@ class StreamingSynthesizer:
         batch = [self._queue.popleft() for _ in range(k)]
         keys = [b[0] for b in batch]
         ids = [b[2] for b in batch]
-        post, lens = self.synth.decode_device([b[1] for b in batch], ids, seed=self.seed)
+        post, lens = self.synth.decode_device([b[1] for b in batch], ids, seed=self.seed,
+                                              **_rate_kw([b[3] for b in batch], k))      # per-row biases, one batch
         frames = [int(f) for f in _host(lens)]
         if min(frames) < 0:
             raise RuntimeError('Tacotron decoder kernel gave up waiting for a peer thread block (nsteps < 0); results are invalid')
@@ -362,10 +378,11 @@ class StreamingSynthesizer:
         return out
 
 
-def synthesize_stream(synth, wavernn_engine, text, seed=0, utterance_id=0, chunk_steps=2750):
+def synthesize_stream(synth, wavernn_engine, text, seed=0, utterance_id=0, chunk_steps=2750, mu_bias=0.0):
     """One sentence as a stream: yields its Tacotron mel [T, 80] first, then its wave pieces (float64 numpy) as the vocoder
-    makes them.  The pieces concatenate to synthesize_batch's wave of the sentence with utterance_offset = utterance_id."""
-    mels, _ = synth.mels([text], seed=seed, utterance_offset=utterance_id)
+    makes them.  The pieces concatenate to synthesize_batch's wave of the sentence with utterance_offset = utterance_id and
+    the same speaking-rate bias `mu_bias`."""
+    mels, _ = synth.mels([text], seed=seed, utterance_offset=utterance_id, **_rate_kw(mu_bias, 1))
     mel = mels[0]
     yield mel
     sv = StreamingVocoder(wavernn_engine, seed=seed, chunk_steps=chunk_steps, max_rows=1)

@@ -19,6 +19,22 @@ def _ptr(t):
     return C.c_void_p(t.data_ptr()) if t is not None else C.c_void_p(0)
 
 
+def mu_bias_array(mu_bias, B):
+    """Speaking-rate biases of a batch of B sentences (b200tts_taco_decode_biased): a scalar or [B] -> float32 [B], or None when
+    there is none (None, or every bias 0: the unbiased decoder, bit for bit).  Each must be finite and in [-1, 1]; positive
+    biases speak faster.  Raises ValueError otherwise."""
+    if mu_bias is None:
+        return None
+    b = np.asarray(mu_bias, dtype=np.float32)
+    if b.ndim == 0:
+        b = np.full(B, b, dtype=np.float32)
+    if b.shape != (B,):
+        raise ValueError(f'mu_bias must be a scalar or [{B}] (one per sentence), got shape {b.shape}')
+    if not (np.isfinite(b).all() and (np.abs(b) <= 1).all()):
+        raise ValueError('mu_bias must be finite and in [-1, 1]')
+    return None if not b.any() else np.ascontiguousarray(b)
+
+
 class TacoDecoderEngine:
     def __init__(self, weights: dict, cfg: dict | None = None, device: int | None = None):
         if not torch.cuda.is_available():
@@ -59,17 +75,20 @@ class TacoDecoderEngine:
         return C.c_void_p(torch.cuda.current_stream(self.device).cuda_stream)
 
     def decode(self, memory, lengths=None, *, masks=None, seed=0, utterance_offset=0, max_steps=2000, window=False,
-               want_align=True, forced_states=None):
+               want_align=True, forced_states=None, mu_bias=None):
         """memory [B, Tx, enc_dim] (tensor/ndarray); lengths [B] or None (= Tx).  masks: optional uint8 keep flags
         [B, max_steps, 2, prenet_units] (EXT mode) else Philox(seed).  Returns dict(frames [B,max_steps,80], stop
         [B,max_steps], align [B,max_steps,Tx] or None, nsteps [B]) as CUDA tensors (rows beyond nsteps are undefined).
         forced_states: optional [B, max_steps, state_floats(Tx)] teacher-forcing records (see include/b200tts.h,
-        b200tts_taco_decode_forced): the whole recurrent state is reloaded before every step and exactly max_steps steps run."""
+        b200tts_taco_decode_forced): the whole recurrent state is reloaded before every step and exactly max_steps steps run.
+        mu_bias: speaking-rate bias, a scalar or one per sentence, each finite in [-1, 1] (b200tts_taco_decode_biased: the
+        forward-attention speed bias of attention.py:163-165; positive is faster).  None or all zeros: the unbiased decoder."""
         dev = self._dev()
         m = torch.as_tensor(memory).to(device=dev, dtype=torch.float32).contiguous()
         if m.dim() != 3 or m.shape[2] != self.cfg['enc_dim']:
             raise ValueError(f'memory must be [B, Tx, {self.cfg["enc_dim"]}]')
         B, Tx, _ = m.shape
+        bias = mu_bias_array(mu_bias, B)
         ln = torch.full((B,), Tx, dtype=torch.int32) if lengths is None else torch.as_tensor(lengths, dtype=torch.int32)
         if int(ln.max()) > Tx or int(ln.min()) < 1:
             raise ValueError('lengths must be in [1, Tx]')
@@ -94,6 +113,12 @@ class TacoDecoderEngine:
                 fs = torch.as_tensor(forced_states).to(device=dev, dtype=torch.float32).contiguous()
                 if tuple(fs.shape) != (B, max_steps, self.state_floats(Tx)):
                     raise ValueError(f'forced_states must be [B, max_steps, {self.state_floats(Tx)}]')
+            if bias is not None:
+                _lib.check(self.lib.b200tts_taco_decode_biased(self._h, _ptr(m), _ptr(ln), B, Tx, C.byref(d), int(max_steps),
+                                                               1 if window else 0, bias.ctypes.data_as(C.POINTER(C.c_float)),
+                                                               _ptr(fs), _ptr(frames), _ptr(stop), _ptr(align), _ptr(nsteps),
+                                                               self._stream()))
+            elif fs is not None:
                 _lib.check(self.lib.b200tts_taco_decode_forced(self._h, _ptr(m), _ptr(ln), B, Tx, C.byref(d), int(max_steps),
                                                                1 if window else 0, _ptr(fs), _ptr(frames), _ptr(stop), _ptr(align),
                                                                _ptr(nsteps), self._stream()))

@@ -21,7 +21,7 @@ import numpy as np
 import torch
 
 from . import ckpt
-from .engine import TacoDecoderEngine
+from .engine import TacoDecoderEngine, mu_bias_array
 from .pinyin import get_pyin
 from .text import Symbols, build_symbols
 
@@ -58,9 +58,11 @@ class Synthesizer:
         self.engine = TacoDecoderEngine(w, device=device)
         return self
 
-    def mels(self, texts, seed=0, window=False, max_iters=None, utterance_offset=0):
+    def mels(self, texts, seed=0, window=False, max_iters=None, utterance_offset=0, mu_bias=None):
         """Batch of pinyin strings -> (list of np.float32 mel [T_b, 80] scaled to [0,1] like the .npy the reference saves,
-        dict with device tensors).  Each sentence decodes until its own stop token (reference graph is batch 1)."""
+        dict with device tensors).  Each sentence decodes until its own stop token (reference graph is batch 1).
+        mu_bias: speaking-rate bias, a scalar or one per text (TacoDecoderEngine.decode; positive speaks faster)."""
+        mu_bias = mu_bias_array(mu_bias, len(texts))
         seqs = [self.symbols.text_to_sequence(t) for t in texts]
         B, Tx = len(seqs), max(len(s) for s in seqs)
         ids = np.zeros((B, Tx), dtype=np.int32)
@@ -72,7 +74,8 @@ class Synthesizer:
         ms = int(max_iters or self.max_iters)
         # the prenet-dropout Philox stream is keyed by the GLOBAL sentence index: a sentence's mel must not depend on
         # how the batch is sharded over ranks
-        dec = eng.decode(mem, lengths, seed=seed, utterance_offset=utterance_offset, max_steps=ms, window=window, want_align=True)
+        dec = eng.decode(mem, lengths, seed=seed, utterance_offset=utterance_offset, max_steps=ms, window=window, want_align=True,
+                         mu_bias=mu_bias)
         mel = eng.postnet(dec['frames'], dec['nsteps'])
         n = dec['nsteps'].cpu().numpy()
         if (n < 0).any():
@@ -86,16 +89,17 @@ class Synthesizer:
             out.append(unit_mel(mel_h[b, :target]))
         return out, dict(decode=dec, memory=mem, lengths=lengths)
 
-    def decode_device(self, texts, ids, seed=0, window=False, max_iters=None):
+    def decode_device(self, texts, ids, seed=0, window=False, max_iters=None, mu_bias=None):
         """Batch of pinyin strings -> (postnet output [B, max_iters, 80] on the +-4 scale, target lengths [B] int32), both
         CUDA tensors: what `mels` computes before its host copy (rows past a sentence's length are unspecified).  The prenet
         dropout of sentence b is keyed by ids[b], an arbitrary global id, so a sentence's mel does not depend on which others
         share its batch.  Consecutive ids draw the PHILOX stream directly; otherwise each run of consecutive ids gets its keep
-        flags from philox_masks, which by its contract equal that stream."""
+        flags from philox_masks, which by its contract equal that stream.  mu_bias: as in `mels`."""
         seqs = [self.symbols.text_to_sequence(t) for t in texts]
         ids = [int(i) for i in ids]
         if len(ids) != len(seqs) or not seqs:
             raise ValueError('need one id per text, and at least one text')
+        mu_bias = mu_bias_array(mu_bias, len(seqs))
         B, Tx = len(seqs), max(len(s) for s in seqs)
         tok = np.zeros((B, Tx), dtype=np.int32)
         for b, s in enumerate(seqs):
@@ -111,17 +115,18 @@ class Synthesizer:
             else:
                 runs.append([i, 1])
         if len(runs) == 1:
-            dec = eng.decode(mem, lengths, seed=seed, utterance_offset=ids[0], max_steps=ms, window=window, want_align=False)
+            dec = eng.decode(mem, lengths, seed=seed, utterance_offset=ids[0], max_steps=ms, window=window, want_align=False,
+                             mu_bias=mu_bias)
         else:
             masks = torch.cat([eng.philox_masks(seed, start, count, ms) for start, count in runs])
-            dec = eng.decode(mem, lengths, masks=masks, max_steps=ms, window=window, want_align=False)
+            dec = eng.decode(mem, lengths, masks=masks, max_steps=ms, window=window, want_align=False, mu_bias=mu_bias)
         mel = eng.postnet(dec['frames'], dec['nsteps'])
         return mel, eng.target_lengths(dec['stop'], dec['nsteps'])
 
-    def synthesize(self, text, out_dir, idx, step=None, seed=0):
+    def synthesize(self, text, out_dir, idx, step=None, seed=0, mu_bias=None):
         step = self.step if step is None else step
+        mels, info = self.mels([text], seed=seed, mu_bias=mu_bias)
         os.makedirs(out_dir, exist_ok=True)
-        mels, info = self.mels([text], seed=seed)
         pred_mel_path = os.path.join(out_dir, f'step-{step}-{idx}-mel-pred.npy')
         np.save(pred_mel_path, mels[0], allow_pickle=False)
         align = info['decode']['align'][0, :mels[0].shape[0] + 1].cpu().numpy()
