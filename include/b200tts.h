@@ -346,6 +346,37 @@ int b200tts_taco_postnet(b200tts_taco* ctx, const float* d_frames, const int32_t
  * b200tts_taco_decode writes them; nsteps is clamped to max_steps, and a negative nsteps (a failed decode) is passed through. */
 int b200tts_taco_target_lengths(const float* d_stop, const int32_t* d_nsteps, int B, int max_steps, int32_t* d_len, void* stream);
 
+/* Decoder sessions: free runs decoded in slices of at most k steps, so a service can bound the decoder work it does between two
+ * vocoder runs, and decodes opened at different times can share a slice (continuous batching).  The frames, stop values and step
+ * count of a session, however its steps are cut and whichever sessions share its slices, are bit for bit those of
+ * b200tts_taco_decode_biased with B >= 2 (taco_decoder_kernel, one thread block per sentence) on the same encoder output, with the
+ * same seed, utterance id, bias, window flag and max_steps.  A slice is one launch of 1..128 thread blocks: one wave of the SMs.
+ * Refusals return B200TTS_EINVAL before any CUDA call.
+ *
+ * session_open_batch: n (1..128) sessions from d_memory [n][Tx_max][enc_dim] (Tx_max <= 512) with h_lengths [n] (host, each
+ *   1..Tx_max).  dropout: PHILOX only (EXT masks are refused); session i's utterance id is h_ids[i] (host; NULL: utterance_offset
+ *   + i).  h_mu_bias [n] host speaking-rate biases, each finite and in [-1, 1] (NULL: 0).  The memory is copied and its keys
+ *   computed once, on `stream`, into memory the sessions own; each starts at position 0.  The sessions of one call share one
+ *   allocation, freed when the last of them is destroyed.  out[n] receives the sessions, on success only.
+ * session_destroy: null-safe; waits for the work still queued.  b200tts_taco_destroy frees the sessions still open.
+ * session_info: steps decoded so far (the position of the next slice), whether the decode is done (its stop token fired, or
+ *   it reached max_steps), and its max_steps; any pointer may be NULL.
+ * session_run: n (1..128) distinct sessions of ctx advance by up to max_steps (>= 1) steps each in one launch; a session stops
+ *   early at the step whose stop token exceeds 0.5, and a finished session takes part with 0 steps.  Where a decode stops is known
+ *   on the device only, so the call waits for the slice (it synchronises `stream`) and returns with every position updated.
+ * session_outputs: the decoded steps of n (1..128) sessions of one context in the batch layout b200tts_taco_decode writes, ready
+ *   for b200tts_taco_postnet and b200tts_taco_target_lengths: d_frames [n][T_max][num_mels], d_stop [n][T_max] (zeros from each
+ *   session's position on) and d_nsteps [n] = the positions.  T_max must be at least every position.  One launch on `stream`. */
+typedef struct b200tts_taco_session b200tts_taco_session;
+int b200tts_taco_session_open_batch(b200tts_taco* ctx, const float* d_memory, const int32_t* h_lengths, int n, int Tx_max,
+                                    const b200tts_taco_dropout* dropout, const uint64_t* h_ids, int max_steps, int window,
+                                    const float* h_mu_bias, b200tts_taco_session** out, void* stream);
+void b200tts_taco_session_destroy(b200tts_taco_session* s);
+int b200tts_taco_session_info(const b200tts_taco_session* s, int32_t* pos, int32_t* done, int32_t* max_steps);
+int b200tts_taco_session_run(b200tts_taco* ctx, b200tts_taco_session* const* s, int n, int max_steps, void* stream);
+int b200tts_taco_session_outputs(b200tts_taco_session* const* s, int n, int T_max, float* d_frames, float* d_stop,
+                                 int32_t* d_nsteps, void* stream);
+
 /* The keep flags the PHILOX dropout mode draws: d_masks [B][steps][2][prenet_units]. */
 int b200tts_taco_philox_masks(int device, uint64_t seed, uint64_t utterance_offset, int B, int steps, int prenet_units,
                               uint8_t* d_masks, void* stream);

@@ -132,6 +132,14 @@ SIGNATURES = {
     'b200tts_taco_encode': (C.c_int, [C.c_void_p, C.c_void_p, C.c_void_p, C.c_int, C.c_int, C.c_void_p, C.c_void_p]),
     'b200tts_taco_postnet': (C.c_int, [C.c_void_p, C.c_void_p, C.c_void_p, C.c_int, C.c_int, C.c_void_p, C.c_void_p]),
     'b200tts_taco_target_lengths': (C.c_int, [C.c_void_p, C.c_void_p, C.c_int, C.c_int, C.c_void_p, C.c_void_p]),
+    'b200tts_taco_session_open_batch': (C.c_int, [C.c_void_p, C.c_void_p, C.POINTER(C.c_int32), C.c_int, C.c_int,
+                                                  C.POINTER(TacoDropout), C.POINTER(C.c_uint64), C.c_int, C.c_int,
+                                                  C.POINTER(C.c_float), C.POINTER(C.c_void_p), C.c_void_p]),
+    'b200tts_taco_session_destroy': (None, [C.c_void_p]),
+    'b200tts_taco_session_info': (C.c_int, [C.c_void_p, C.POINTER(C.c_int32), C.POINTER(C.c_int32), C.POINTER(C.c_int32)]),
+    'b200tts_taco_session_run': (C.c_int, [C.c_void_p, C.POINTER(C.c_void_p), C.c_int, C.c_int, C.c_void_p]),
+    'b200tts_taco_session_outputs': (C.c_int, [C.POINTER(C.c_void_p), C.c_int, C.c_int, C.c_void_p, C.c_void_p, C.c_void_p,
+                                               C.c_void_p]),
     'b200tts_taco_philox_masks': (C.c_int, [C.c_int, C.c_uint64, C.c_uint64, C.c_int, C.c_int, C.c_int, C.c_void_p, C.c_void_p]),
     'b200tts_gl_create': (C.c_int, [C.POINTER(C.c_void_p), C.c_int, C.POINTER(GlCfg), C.c_void_p]),
     'b200tts_gl_destroy': (None, [C.c_void_p]),

@@ -17,7 +17,7 @@ PKG = os.path.dirname(os.path.abspath(__file__))
 CSRC = os.path.join(PKG, 'csrc')
 LIB = os.path.join(CSRC, 'libb200tts.so')
 # One translation unit per model stage, so that no stage's device code can change the code ptxas generates for another's.
-SOURCES = ['api.cu', 'wavernn.cu', 'tacotron.cu', 'griffin_lim.cu', 'mel_analysis.cu', 'resample.cu']
+SOURCES = ['api.cu', 'wavernn.cu', 'tacotron.cu', 'taco_session.cu', 'griffin_lim.cu', 'mel_analysis.cu', 'resample.cu']
 NVCC_FLAGS = ['-gencode', 'arch=compute_90a,code=sm_90a', '-lineinfo', '-O3', '-std=c++17',
               '-Xcompiler', '-fPIC', '--expt-relaxed-constexpr']
 

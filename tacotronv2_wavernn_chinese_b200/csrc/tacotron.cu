@@ -1,10 +1,12 @@
 // libb200tts.so -- Tacotron-2 encoder, decoder and postnet (taco_decoder.cuh, taco_encpost.cuh, taco_grid.cuh): b200tts_taco_*.
+// The kernels of the decoder sessions are in taco_session.cu.
 //
 // In one module, the dynamic shared memory of every kernel starts at the largest alignment any extern __shared__ array of the
 // module asks for.  The Tacotron kernels' code and shared-memory budgets were settled while they shared a module with
 // wavernn_tc_kernel (1024 bytes), so their own `sm` arrays ask for 1024: compiled here, ptxas gives them the same code.
 #include <algorithm>
 #include <cmath>
+#include <set>
 
 #include "api.h"
 #include "taco_decoder.cuh"
@@ -16,6 +18,19 @@ using namespace b200tts;
 struct TacoConvW {          // one conv1d + folded BatchNorm
   const float *K, *bias, *scale, *shift;
   int k, Cin, Cout;
+};
+// One free-running decode cut into slices (b200tts_taco_session_*): its memory and keys, the state record its last slice saved,
+// and its frames and stop values so far.  Owned by its context, which frees the sessions still open.
+struct b200tts_taco_session {
+  b200tts_taco* ctx = nullptr;
+  std::shared_ptr<DeviceBuf> batch;         // the open's one allocation, freed with the last of its sessions
+  const float *memory = nullptr, *keys = nullptr;
+  float *state = nullptr, *frames = nullptr, *stop = nullptr;
+  uint64_t seed = 0, id = 0;
+  float mu_bias = 0.f;
+  int Tx = 0, max_steps = 0, window = 0;
+  int pos = 0;                              // steps decoded
+  bool done = false;                        // the stop token fired, or pos reached max_steps
 };
 struct b200tts_taco {
   int device = 0;
@@ -37,6 +52,12 @@ struct b200tts_taco {
   bool tg_ok = false;
   int sm_count = 0;
   DeviceBuf mu_bias;          // [B] speaking-rate biases of the last b200tts_taco_decode_biased call
+  std::set<b200tts_taco_session*> sessions;   // open decoder sessions, freed with the context
+  DeviceBuf sess_status;                      // [kTacoSessRows][2] status words of the last session run ...
+  HostPinned h_sess_status;                   // ... and their host copy
+  ~b200tts_taco() {
+    for (b200tts_taco_session* s : sessions) delete s;
+  }
 };
 
 // Split-K partials of taco_decoder_kernel, in floats.  The matvecs and the context sum need at most 4096 of them; the attention
@@ -255,6 +276,14 @@ extern "C" void b200tts_taco_destroy(b200tts_taco* ctx) {
   delete ctx;
 }
 
+// Every bias finite and in [-1, 1] (h_mu_bias NULL: none).
+static void require_mu_bias(const float* h_mu_bias, int B) {
+  if (h_mu_bias)
+    for (int b = 0; b < B; ++b)
+      REQUIRE(std::isfinite(h_mu_bias[b]) && h_mu_bias[b] >= -1.f && h_mu_bias[b] <= 1.f, B200TTS_EINVAL,
+              "mu_bias[" + std::to_string(b) + "] must be finite and in [-1, 1]");
+}
+
 // h_mu_bias: NULL for the unbiased kernels, else [B] host speaking-rate biases (b200tts_taco_decode_biased)
 static int taco_decode_impl(b200tts_taco* ctx, const float* d_memory, const int32_t* d_lengths, int B, int Tx_max,
                             const b200tts_taco_dropout* dropout, int max_steps, int window, const float* h_mu_bias,
@@ -266,10 +295,7 @@ static int taco_decode_impl(b200tts_taco* ctx, const float* d_memory, const int3
   if (dropout) d = *dropout;
   REQUIRE(d.mode == B200TTS_TACO_DROPOUT_PHILOX || (d.mode == B200TTS_TACO_DROPOUT_EXT && d.d_masks), B200TTS_EINVAL,
           "bad dropout descriptor");
-  if (h_mu_bias)
-    for (int b = 0; b < B; ++b)
-      REQUIRE(std::isfinite(h_mu_bias[b]) && h_mu_bias[b] >= -1.f && h_mu_bias[b] <= 1.f, B200TTS_EINVAL,
-              "mu_bias[" + std::to_string(b) + "] must be finite and in [-1, 1]");
+  require_mu_bias(h_mu_bias, B);
   DeviceGuard dg(ctx->device);
   cudaStream_t st = (cudaStream_t)stream;
   const TacoWeights& w = ctx->tw;
@@ -432,6 +458,148 @@ extern "C" int b200tts_taco_target_lengths(const float* d_stop, const int32_t* d
   REQUIRE(B >= 1 && max_steps >= 1, B200TTS_EINVAL, "B / max_steps out of range");
   taco_target_lengths_kernel<<<B, 256, 0, (cudaStream_t)stream>>>(d_stop, d_nsteps, max_steps, d_len);
   B200_CUDA(cudaGetLastError());
+  API_END
+}
+
+// ---- decoder sessions: free runs in slices on taco_decoder_session_kernel -----------------------------------------------------
+// Every refusal below comes before the first CUDA call, so a refused call has launched and allocated nothing.
+extern "C" int b200tts_taco_session_open_batch(b200tts_taco* ctx, const float* d_memory, const int32_t* h_lengths, int n, int Tx_max,
+                                               const b200tts_taco_dropout* dropout, const uint64_t* h_ids, int max_steps, int window,
+                                               const float* h_mu_bias, b200tts_taco_session** out, void* stream) {
+  API_BEGIN
+  REQUIRE(ctx && d_memory && h_lengths && dropout && out, B200TTS_EINVAL, "null argument");
+  REQUIRE(n >= 1 && n <= kTacoSessRows, B200TTS_EINVAL, "n must be 1..128 (one wave of thread blocks)");
+  REQUIRE(Tx_max >= 1 && Tx_max <= kTacoMaxTx, B200TTS_EINVAL, "Tx_max must be 1..512");
+  REQUIRE(max_steps >= 1, B200TTS_EINVAL, "max_steps must be >= 1");
+  REQUIRE(dropout->mode == B200TTS_TACO_DROPOUT_PHILOX, B200TTS_EINVAL,
+          "decoder sessions take PHILOX dropout keyed by (seed, utterance id); EXT masks are refused");
+  for (int i = 0; i < n; ++i) REQUIRE(h_lengths[i] >= 1 && h_lengths[i] <= Tx_max, B200TTS_EINVAL, "every length must be 1..Tx_max");
+  require_mu_bias(h_mu_bias, n);
+  const TacoWeights& w = ctx->tw;
+  const int M = w.mels;
+  const size_t mem_f = (size_t)n * Tx_max * w.E, keys_f = (size_t)n * Tx_max * w.A;
+  const size_t state_stride = ((size_t)taco_state_floats(M, w.E, w.U, Tx_max) + 3) / 4 * 4;
+  const size_t out_stride = (size_t)max_steps * (M + 1);      // frames [max_steps][M], then stop [max_steps]
+  const size_t zero_f = (size_t)n * (state_stride + out_stride);
+  DeviceGuard dg(ctx->device);
+  const cudaStream_t st = (cudaStream_t)stream;
+  auto block = std::make_shared<DeviceBuf>();
+  block->ensure((mem_f + keys_f + zero_f) * sizeof(float));
+  float* base = block->as<float>();
+  float* mem = base;
+  float* keys = mem + mem_f;
+  float* rest = keys + keys_f;
+  B200_CUDA(cudaMemcpyAsync(mem, d_memory, mem_f * sizeof(float), cudaMemcpyDeviceToDevice, st));
+  B200_CUDA(cudaMemsetAsync(rest, 0, zero_f * sizeof(float), st));
+  taco_keys_kernel<<<n * Tx_max, 128, w.E * sizeof(float), st>>>(mem, w.mem_k, n * Tx_max, w.E, w.A, keys);
+  B200_CUDA(cudaGetLastError());
+  ctx->launches++;
+  std::vector<std::unique_ptr<b200tts_taco_session>> ss(n);
+  for (int i = 0; i < n; ++i) {
+    ss[i].reset(new b200tts_taco_session());
+    b200tts_taco_session& s = *ss[i];
+    s.ctx = ctx;
+    s.batch = block;
+    s.memory = mem + (size_t)i * Tx_max * w.E;
+    s.keys = keys + (size_t)i * Tx_max * w.A;
+    s.state = rest + (size_t)i * state_stride;
+    s.frames = rest + (size_t)n * state_stride + (size_t)i * out_stride;
+    s.stop = s.frames + (size_t)max_steps * M;
+    s.seed = dropout->seed;
+    s.id = h_ids ? h_ids[i] : dropout->utterance_offset + (uint64_t)i;
+    s.mu_bias = h_mu_bias ? h_mu_bias[i] : 0.f;
+    s.Tx = h_lengths[i];
+    s.max_steps = max_steps;
+    s.window = window ? 1 : 0;
+  }
+  for (int i = 0; i < n; ++i) {
+    ctx->sessions.insert(ss[i].get());
+    out[i] = ss[i].release();
+  }
+  API_END
+}
+
+// cudaFree waits for the work queued on the device, so no slice still in flight reads the memory freed here.
+extern "C" void b200tts_taco_session_destroy(b200tts_taco_session* s) {
+  if (!s) return;
+  DeviceGuard dg(s->ctx->device, true);
+  s->ctx->sessions.erase(s);
+  delete s;
+}
+
+extern "C" int b200tts_taco_session_info(const b200tts_taco_session* s, int32_t* pos, int32_t* done, int32_t* max_steps) {
+  API_BEGIN
+  REQUIRE(s, B200TTS_EINVAL, "null argument");
+  if (pos) *pos = s->pos;
+  if (done) *done = s->done ? 1 : 0;
+  if (max_steps) *max_steps = s->max_steps;
+  API_END
+}
+
+static void require_sessions(const b200tts_taco* ctx, b200tts_taco_session* const* s, int n) {
+  REQUIRE(s, B200TTS_EINVAL, "null argument");
+  REQUIRE(n >= 1 && n <= kTacoSessRows, B200TTS_EINVAL, "n must be 1..128 sessions");
+  for (int i = 0; i < n; ++i) {
+    REQUIRE(s[i], B200TTS_EINVAL, "null session");
+    REQUIRE(!ctx || s[i]->ctx == ctx, B200TTS_EINVAL, "the session belongs to another context");
+    REQUIRE(s[i]->ctx == s[0]->ctx, B200TTS_EINVAL, "the sessions belong to different contexts");
+    for (int j = 0; j < i; ++j) REQUIRE(s[j] != s[i], B200TTS_EINVAL, "the same session appears twice in one call");
+  }
+}
+
+extern "C" int b200tts_taco_session_run(b200tts_taco* ctx, b200tts_taco_session* const* s, int n, int max_steps, void* stream) {
+  API_BEGIN
+  REQUIRE(ctx, B200TTS_EINVAL, "null argument");
+  require_sessions(ctx, s, n);
+  REQUIRE(max_steps >= 1, B200TTS_EINVAL, "max_steps must be >= 1");
+  // finished sessions take part with 0 steps: they get no thread block
+  TacoSessIO io{};
+  int rows[kTacoSessRows], m = 0;
+  for (int i = 0; i < n; ++i) {
+    if (s[i]->done) continue;
+    TacoSessRow& r = io.row[m];
+    r.memory = s[i]->memory; r.keys = s[i]->keys; r.state = s[i]->state;
+    r.frames = s[i]->frames; r.stop = s[i]->stop;
+    r.seed = s[i]->seed; r.id = s[i]->id; r.mu_bias = s[i]->mu_bias;
+    r.Tx = s[i]->Tx; r.pos = s[i]->pos; r.n = std::min(max_steps, s[i]->max_steps - s[i]->pos); r.window = s[i]->window;
+    rows[m++] = i;
+  }
+  if (m == 0) return B200TTS_OK;
+  DeviceGuard dg(ctx->device);
+  const cudaStream_t st = (cudaStream_t)stream;
+  ctx->sess_status.ensure((size_t)kTacoSessRows * 2 * sizeof(int));
+  ctx->h_sess_status.ensure((size_t)kTacoSessRows * 2 * sizeof(int));
+  int* d_status = ctx->sess_status.as<int>();
+  for (int u = 0; u < m; ++u) io.row[u].status = d_status + 2 * u;
+  launch_taco_sessions(ctx->tw, io, m, taco_decoder_smem_bytes(ctx->tw), st);
+  ctx->launches++;
+  // where each decode stopped is decided on the device: wait for the slice and read the positions back
+  int* h = static_cast<int*>(ctx->h_sess_status.p);
+  B200_CUDA(cudaMemcpyAsync(h, d_status, (size_t)m * 2 * sizeof(int), cudaMemcpyDeviceToHost, st));
+  B200_CUDA(cudaStreamSynchronize(st));
+  for (int u = 0; u < m; ++u) {
+    b200tts_taco_session& x = *s[rows[u]];
+    x.pos = h[2 * u];
+    x.done = h[2 * u + 1] != 0 || x.pos >= x.max_steps;
+  }
+  API_END
+}
+
+extern "C" int b200tts_taco_session_outputs(b200tts_taco_session* const* s, int n, int T_max, float* d_frames, float* d_stop,
+                                            int32_t* d_nsteps, void* stream) {
+  API_BEGIN
+  require_sessions(nullptr, s, n);
+  REQUIRE(d_frames && d_stop && d_nsteps, B200TTS_EINVAL, "null argument");
+  REQUIRE(T_max >= 1, B200TTS_EINVAL, "T_max must be >= 1");
+  TacoSessOut g{};
+  for (int i = 0; i < n; ++i) {
+    REQUIRE(s[i]->pos <= T_max, B200TTS_EINVAL, "T_max is shorter than a session's steps");
+    g.frames[i] = s[i]->frames; g.stop[i] = s[i]->stop; g.pos[i] = s[i]->pos;
+  }
+  b200tts_taco* ctx = s[0]->ctx;
+  DeviceGuard dg(ctx->device);
+  launch_taco_session_outputs(g, n, T_max, ctx->tw.mels, d_frames, d_stop, d_nsteps, (cudaStream_t)stream);
+  ctx->launches++;
   API_END
 }
 

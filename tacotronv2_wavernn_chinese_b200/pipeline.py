@@ -280,9 +280,20 @@ class StreamingSynthesizer:
 
     Everything runs on the current stream, in order: the Tacotron kernels never run beside the vocoder's persistent kernels,
     whose co-residency on the SMs they could break.  `max_rows` > 32 runs tensor-core sessions, and `chunk_steps` must then be
-    a multiple of the engine's hop."""
+    a multiple of the engine's hop.
 
-    def __init__(self, synth, engine, seed=0, chunk_steps=2750, max_rows=32, max_admit=None):
+    `decode_steps` = k bounds the Tacotron work done before each vocoder run, whatever the sentence lengths (None: the whole
+    decode at admission, as above).  Admitted texts get one encoder batch and one open of decoder sessions
+    (`synth.open_decodes`); in-flight decodes plus active vocoder sessions stay within `max_rows`, and in-flight decodes within
+    128.  Every step then advances all in-flight decodes by at most k steps in ONE launch, gives the decodes that finished one
+    postnet, one stop-token cut (`synth.finish_decodes`) and one batched vocoder open, and runs the vocoder.  A request's first
+    piece comes in the step its decode finishes.  Its frames are bit for bit those of the batch decoder (`taco_decoder_kernel`,
+    which b200tts_taco_decode runs for B >= 2) on its admission's encoder output with its id, seed and bias, and its pieces
+    concatenate to the one-shot generate of the resulting mel on the same kernel family.  A text admitted alone is therefore
+    decoded on that kernel too, and its mel differs in bits from the default mode's, which decodes a batch of one on the
+    single-sentence kernel."""
+
+    def __init__(self, synth, engine, seed=0, chunk_steps=2750, max_rows=32, max_admit=None, decode_steps=None):
         cap = int(getattr(engine, 'max_session_rows', 32))
         if not 1 <= int(max_rows) <= cap:
             raise ValueError(f'max_rows must be 1..{cap} (the most sessions one launch of this engine takes)')
@@ -293,6 +304,10 @@ class StreamingSynthesizer:
         self.synth, self.engine, self.seed = synth, engine, int(seed)
         self.chunk_steps, self.max_rows = int(chunk_steps), int(max_rows)
         self.max_admit = None if max_admit is None else int(max_admit)
+        if decode_steps is not None and int(decode_steps) < 1:
+            raise ValueError('decode_steps must be >= 1 (or None: the whole decode at admission)')
+        self.decode_steps = None if decode_steps is None else int(decode_steps)
+        self._decoding = []                     # (key, utterance id, decoder session) in admission order
         self._tc = self.max_rows > 32                       # the push kernel runs at most 32 sessions per launch
         if self._tc and self.chunk_steps % int(engine.hop):
             raise ValueError(f'above 32 rows the sessions run on the tensor cores: chunk_steps must be a multiple of hop ({engine.hop})')
@@ -322,8 +337,13 @@ class StreamingSynthesizer:
     def active(self) -> int:
         return len(self._active)
 
+    @property
+    def decoding(self) -> int:
+        """Requests whose Tacotron decode is in flight (decode_steps mode)."""
+        return len(self._decoding)
+
     def idle(self) -> bool:
-        return not self._queue and not self._active
+        return not self._queue and not self._active and not self._decoding
 
     def mel(self, key):
         """The [T, 80] float32 mel in [0, 1] of an admitted request, until the step after the one that returned its last piece."""
@@ -342,9 +362,15 @@ class StreamingSynthesizer:
         ids = [b[2] for b in batch]
         post, lens = self.synth.decode_device([b[1] for b in batch], ids, seed=self.seed,
                                               **_rate_kw([b[3] for b in batch], k))      # per-row biases, one batch
+        return self._open_vocoder(keys, ids, post, lens)
+
+    def _open_vocoder(self, keys, ids, post, lens):
+        """Vocoder sessions for the rows of a postnet output [n, T, 80] with device target lengths `lens`; returns the finished
+        (key, empty piece, True) of the rows whose mel is empty."""
         frames = [int(f) for f in _host(lens)]
         if min(frames) < 0:
             raise RuntimeError('Tacotron decoder kernel gave up waiting for a peer thread block (nsteps < 0); results are invalid')
+        k = len(keys)
         for b, key in enumerate(keys):
             self._mels[key] = (post, b, frames[b])
         rows = [b for b in range(k) if frames[b] > 0]
@@ -355,10 +381,36 @@ class StreamingSynthesizer:
             self._active += [(keys[b], s) for b, s in zip(rows, sessions)]
         return [(keys[b], np.zeros(0, dtype=np.float64), True) for b in range(k) if frames[b] == 0]
 
+    def _decode_slice(self):
+        """decode_steps mode: admits queued texts into decoder sessions, advances every in-flight decode by at most
+        decode_steps steps in one launch, and hands the decodes that finished to the vocoder."""
+        from .tacotron.engine import MAX_DECODE_SESSIONS
+        k = min(len(self._queue), self.max_rows - len(self._active) - len(self._decoding), MAX_DECODE_SESSIONS - len(self._decoding))
+        if self.max_admit is not None:
+            k = min(k, self.max_admit)
+        if k > 0:
+            batch = [self._queue.popleft() for _ in range(k)]
+            ids = [b[2] for b in batch]
+            biases = [b[3] for b in batch]
+            sessions = self.synth.open_decodes([b[1] for b in batch], ids, seed=self.seed, mu_bias=biases if any(biases) else None)
+            self._decoding += [(b[0], b[2], s) for b, s in zip(batch, sessions)]
+        if not self._decoding:
+            return []
+        self.synth.engine.advance_decodes([s for _, _, s in self._decoding], self.decode_steps)
+        done = [d for d in self._decoding if d[2].done]
+        self._decoding = [d for d in self._decoding if not d[2].done]
+        if not done:
+            return []
+        post, lens = self.synth.finish_decodes([s for _, _, s in done])
+        empty = self._open_vocoder([d[0] for d in done], [d[1] for d in done], post, lens)
+        for _, _, s in done:
+            s.close()
+        return empty
+
     def step(self):
         for key in self._gone:
             self._mels.pop(key, None)
-        empty = self._admit()
+        empty = self._admit() if self.decode_steps is None else self._decode_slice()
         out, still = [], []
         if self._active:
             pieces = self.engine.advance([s for _, s in self._active], self.chunk_steps)

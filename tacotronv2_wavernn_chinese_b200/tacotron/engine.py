@@ -2,6 +2,7 @@
 from __future__ import annotations
 
 import ctypes as C
+import weakref
 
 import numpy as np
 import torch
@@ -10,6 +11,7 @@ from .. import _lib
 from .._lib import TacoCfg, TacoDropout
 
 MAX_TOKENS = 512       # kTacoMaxTx: the longest sentence, in symbols, the encoder and decoders take
+MAX_DECODE_SESSIONS = 128     # kTacoSessRows: the most decoder sessions one open or slice takes (one wave of the SMs)
 
 DEFAULT_CFG = dict(num_mels=80, prenet_units=256, lstm_units=256, enc_dim=512, attn_dim=128, attn_filters=32,
                    attn_kernel=31, zoneout=0.1)      # tacotron_hparams.py:99-215 of the reference
@@ -54,11 +56,14 @@ class TacoDecoderEngine:
         _lib.check(self.lib.b200tts_taco_create(C.byref(h), self.device, C.byref(c), arr, len(arr)))
         del keep
         self._h = h
+        self._sessions = weakref.WeakSet()
         emb = host.get('inputs_embedding')
         self.vocab = int(emb.shape[0]) if emb is not None and emb.ndim == 2 else None
 
     def close(self):
         if getattr(self, '_h', None):
+            for s in list(self._sessions):      # the context frees its open sessions
+                s._h = None
             self.lib.b200tts_taco_destroy(self._h)
             self._h = None
 
@@ -175,6 +180,66 @@ class TacoDecoderEngine:
                     t.record_stream(torch.cuda.current_stream(self.device))
         return dict(frames=frames, align=align, nsteps=tl)
 
+    def open_decode_sessions(self, memory, lengths, ids, *, seed=0, max_steps=2000, window=False, mu_bias=None) -> list:
+        """Free runs to be decoded in slices (b200tts_taco_session_open_batch): memory [n, Tx, enc_dim] (n 1..128), lengths [n]
+        in [1, Tx] or None (= Tx), ids: n 64-bit utterance ids keying each row's prenet dropout with `seed`.  mu_bias: a scalar or
+        one per row, as in `decode`.  The memory is copied and its keys computed here, on the current stream; every session
+        starts at step 0.  However `advance_decodes` cuts them, a session's frames, stop values and step count are bit for bit
+        those `decode` gives its row at B >= 2 (one thread block per sentence) with utterance_offset = its id."""
+        dev = self._dev()
+        m = torch.as_tensor(memory).to(device=dev, dtype=torch.float32).contiguous()
+        if m.dim() != 3 or m.shape[2] != self.cfg['enc_dim']:
+            raise ValueError(f'memory must be [n, Tx, {self.cfg["enc_dim"]}]')
+        n, Tx, _ = m.shape
+        ln = np.full(n, Tx, dtype=np.int32) if lengths is None else np.ascontiguousarray(np.asarray(lengths).reshape(-1), dtype=np.int32)
+        uid = np.ascontiguousarray([int(i) & 0xFFFFFFFFFFFFFFFF for i in ids], dtype=np.uint64)
+        if len(ln) != n or len(uid) != n:
+            raise ValueError(f'need one length and one id per row ({n} rows)')
+        bias = mu_bias_array(mu_bias, n)
+        d = TacoDropout()
+        d.seed = int(seed) & 0xFFFFFFFFFFFFFFFF
+        handles = (C.c_void_p * max(n, 1))()
+        with torch.cuda.device(self.device):
+            _lib.check(self.lib.b200tts_taco_session_open_batch(
+                self._h, _ptr(m), ln.ctypes.data_as(C.POINTER(C.c_int32)), n, Tx, C.byref(d), uid.ctypes.data_as(C.POINTER(C.c_uint64)),
+                int(max_steps), 1 if window else 0, None if bias is None else bias.ctypes.data_as(C.POINTER(C.c_float)), handles,
+                self._stream()))
+            m.record_stream(torch.cuda.current_stream(self.device))
+        out = []
+        for h in handles[:n]:
+            s = TacoDecodeSession(self, C.c_void_p(h))
+            self._sessions.add(s)
+            out.append(s)
+        return out
+
+    def advance_decodes(self, sessions, n: int):
+        """Advances 1..128 distinct open decoder sessions of this engine by up to n steps each in one launch (a finished session
+        takes part with 0 steps); a session stops at the step whose stop token exceeds 0.5.  Returns when the slice has finished,
+        with every session's `position` and `done` updated."""
+        sessions = list(sessions)
+        if any(s._h is None for s in sessions):
+            raise ValueError('a session is closed')
+        handles = (C.c_void_p * max(len(sessions), 1))(*[s._h.value for s in sessions])
+        with torch.cuda.device(self.device):
+            _lib.check(self.lib.b200tts_taco_session_run(self._h, handles, len(sessions), int(n), self._stream()))
+
+    def decode_outputs(self, sessions):
+        """The steps decoded so far by 1..128 sessions, in the layout `decode` returns: dict(frames [n, T, 80], stop [n, T],
+        nsteps [n] int32) as CUDA tensors, T the longest position (at least 1), zeros past each session's position."""
+        sessions = list(sessions)
+        if any(s._h is None for s in sessions):
+            raise ValueError('a session is closed')
+        T = max([1] + [s.position for s in sessions])
+        n = len(sessions)
+        dev = self._dev()
+        handles = (C.c_void_p * max(n, 1))(*[s._h.value for s in sessions])
+        with torch.cuda.device(self.device):
+            frames = torch.empty(max(n, 1), T, self.cfg['num_mels'], device=dev, dtype=torch.float32)
+            stop = torch.empty(max(n, 1), T, device=dev, dtype=torch.float32)
+            nsteps = torch.empty(max(n, 1), device=dev, dtype=torch.int32)
+            _lib.check(self.lib.b200tts_taco_session_outputs(handles, n, T, _ptr(frames), _ptr(stop), _ptr(nsteps), self._stream()))
+        return dict(frames=frames, stop=stop, nsteps=nsteps)
+
     def state_floats(self, Tx: int) -> int:
         return int(self.lib.b200tts_taco_state_floats(self._h, int(Tx)))
 
@@ -256,3 +321,51 @@ class TacoDecoderEngine:
             _lib.check(self.lib.b200tts_taco_philox_masks(self.device, int(seed) & 0xFFFFFFFFFFFFFFFF, int(utterance_offset),
                                                           B, steps, self.cfg['prenet_units'], _ptr(m), self._stream()))
         return m
+
+
+class TacoDecodeSession:
+    """One free-running Tacotron decode in slices (TacoDecoderEngine.open_decode_sessions / advance_decodes).  A context
+    manager; close() frees its device memory once the other sessions of its open are closed too (closing the engine frees it)."""
+
+    def __init__(self, engine: TacoDecoderEngine, handle):
+        self.engine = engine
+        self._h = handle
+
+    def _info(self):
+        if self._h is None:
+            raise ValueError('the session is closed')
+        pos, done, ms = C.c_int32(), C.c_int32(), C.c_int32()
+        _lib.check(self.engine.lib.b200tts_taco_session_info(self._h, C.byref(pos), C.byref(done), C.byref(ms)))
+        return pos.value, bool(done.value), ms.value
+
+    @property
+    def position(self) -> int:
+        """Steps decoded so far."""
+        return self._info()[0]
+
+    @property
+    def done(self) -> bool:
+        """The stop token fired, or the decode reached max_steps."""
+        return self._info()[1]
+
+    @property
+    def max_steps(self) -> int:
+        return self._info()[2]
+
+    def close(self):
+        if self._h is not None:
+            self.engine.lib.b200tts_taco_session_destroy(self._h)
+            self._h = None
+            self.engine._sessions.discard(self)
+
+    def __enter__(self):
+        return self
+
+    def __exit__(self, *exc):
+        self.close()
+
+    def __del__(self):
+        try:
+            self.close()
+        except Exception:
+            pass

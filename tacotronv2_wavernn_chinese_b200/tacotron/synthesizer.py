@@ -123,6 +123,32 @@ class Synthesizer:
         mel = eng.postnet(dec['frames'], dec['nsteps'])
         return mel, eng.target_lengths(dec['stop'], dec['nsteps'])
 
+    def open_decodes(self, texts, ids, seed=0, window=False, max_iters=None, mu_bias=None):
+        """Encodes 1..128 pinyin strings in one batch and opens their decoder sessions (TacoDecoderEngine.open_decode_sessions),
+        to be advanced in slices with `engine.advance_decodes` and finished with `finish_decodes`.  Text b's prenet dropout is keyed
+        by (seed, ids[b]) and its frames are bit for bit those of the batch decoder (`taco_decoder_kernel`) on this encoder output.
+        A lone text therefore differs in bits from `decode_device`, which decodes a batch of one on the single-sentence kernel."""
+        seqs = [self.symbols.text_to_sequence(t) for t in texts]
+        if len(ids) != len(seqs) or not seqs:
+            raise ValueError('need one id per text, and at least one text')
+        B, Tx = len(seqs), max(len(s) for s in seqs)
+        tok = np.zeros((B, Tx), dtype=np.int32)
+        for b, s in enumerate(seqs):
+            tok[b, :len(s)] = s
+        lengths = np.array([len(s) for s in seqs], dtype=np.int32)
+        mem = self.engine.encode(tok, lengths)
+        return self.engine.open_decode_sessions(mem, lengths, ids, seed=seed, max_steps=int(max_iters or self.max_iters), window=window,
+                                                mu_bias=mu_bias)
+
+    def finish_decodes(self, sessions):
+        """Finished decoder sessions -> what `decode_device` returns for them: (postnet output [n, T, 80] on the +-4 scale, target
+        lengths [n] int32), both CUDA tensors, T the longest decode (rows past a sentence's length are unspecified).  One postnet
+        and one stop-token cut on the device for the whole set."""
+        eng = self.engine
+        out = eng.decode_outputs(sessions)
+        mel = eng.postnet(out['frames'], out['nsteps'])
+        return mel, eng.target_lengths(out['stop'], out['nsteps'])
+
     def synthesize(self, text, out_dir, idx, step=None, seed=0, mu_bias=None):
         step = self.step if step is None else step
         mels, info = self.mels([text], seed=seed, mu_bias=mu_bias)

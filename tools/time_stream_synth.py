@@ -2,7 +2,7 @@
 pipeline.StreamingSynthesizer fed train.txt sentences at a fixed arrival rate.
 
     python tools/time_stream_synth.py [--frames 401] [--opens 1,32,128,256] [--rows 32,128] [--rate 6,24] [--requests 48,128]
-                                      [--chunk 2750] [--out FILE]
+                                      [--chunk 2750] [--decode_steps whole,8,32] [--slices 1,3,8,32,128] [--out FILE]
 
 Prints the card name and power limit first, and writes the whole report as JSON to --out.
   * opens: host time (synchronised, median of 4 repeats after one warm-up) to open N sessions of `frames` frames one by one
@@ -13,7 +13,11 @@ Prints the card name and power limit first, and writes the whole report as JSON 
     per second, in order, round robin over the set.  Per request the time from arrival to its first piece on the host
     (p50 / p95); per admitting step the admission time (Tacotron encode + decode + postnet, stop cut and batched open, timed
     with a synchronisation around it) and the Tacotron batch size; per step its wall time against the audio each active stream
-    received (chunk / sample rate): a stream keeps real time while step wall <= that duration.
+    received (chunk / sample rate): a stream keeps real time while step wall <= that duration.  The service runs once per
+    --decode_steps value: 'whole' decodes each admission whole (the default service), k slices the decodes (decode_steps=k),
+    and the per-step Tacotron time is then that of the slice, the finishing postnet and cut and the vocoder open.
+  * slices: the Tacotron decoder sessions' step time at 1, 3, 8, 32 and 128 sessions, as the slope between slices of 8 and 40
+    steps (CUDA events), on synthetic decoder weights whose stop never fires.
 Synthetic vocoder weights (time does not depend on their values); the Tacotron travel copy oracle/_ref/tacotron_weights.npz,
 whose stop tokens decide the mel lengths.
 """
@@ -127,22 +131,58 @@ def open_split(eng, frames):
     return out
 
 
-def service(syn, eng, texts, rows, rate, nreq, chunk):
-    ss = pipeline.StreamingSynthesizer(syn, eng, seed=3, chunk_steps=chunk, max_rows=rows)
+def slices(ns, Tx=64, k1=8, k2=40):
+    """us per decoder step of a slice of n sessions: (t(k2) - t(k1)) / (k2 - k1), each the median of 5 (CUDA events)."""
+    sys.path.insert(0, os.path.join(ROOT, 'tests'))
+    from taco_common import synth_taco_weights
+    from tacotronv2_wavernn_chinese_b200.tacotron.engine import TacoDecoderEngine
+    w = synth_taco_weights(3)
+    w['decoder/stop_token_projection/projection_stop_token_projection/bias'][:] = -1e4
+    te = TacoDecoderEngine(w, device=0)
+    res = []
+    for n in ns:
+        mem = torch.as_tensor(np.random.RandomState(n).uniform(-1, 1, (n, Tx, 512)).astype(np.float32)).cuda()
+        ms = {}
+        for k in (k1, k2):
+            t = []
+            for rep in range(6):
+                ss = te.open_decode_sessions(mem, None, list(range(n)), max_steps=k)
+                e0, e1 = torch.cuda.Event(enable_timing=True), torch.cuda.Event(enable_timing=True)
+                _sync()
+                e0.record()
+                te.advance_decodes(ss, k)
+                e1.record()
+                _sync()
+                if rep:
+                    t.append(e0.elapsed_time(e1))
+                for s in ss:
+                    s.close()
+            ms[k] = float(np.median(t))
+        us = (ms[k2] - ms[k1]) / (k2 - k1) * 1e3
+        res.append(dict(sessions=n, us_per_step=us, slice_ms={str(k): v for k, v in ms.items()}))
+        print(f'decoder slice, {n:3d} sessions: {us:7.1f} us per step')
+    te.close()
+    return res
+
+
+def service(syn, eng, texts, rows, rate, nreq, chunk, decode_steps=None):
+    ss = pipeline.StreamingSynthesizer(syn, eng, seed=3, chunk_steps=chunk, max_rows=rows, decode_steps=decode_steps)
     admits = []
-    admit = ss._admit
+    name = '_admit' if decode_steps is None else '_decode_slice'
+    admit = getattr(ss, name)
 
     def timed_admit():
-        k = min(len(ss._queue), ss.max_rows - len(ss._active))
+        k = len(ss._queue)
+        busy = k and ss.max_rows > len(ss._active) + len(ss._decoding) or ss._decoding
         _sync()
         t0 = time.perf_counter()
         out = admit()
         _sync()
-        if k:
-            admits.append(dict(n=k, ms=(time.perf_counter() - t0) * 1e3))
+        if busy:
+            admits.append(dict(n=k - len(ss._queue), ms=(time.perf_counter() - t0) * 1e3))
         return out
 
-    ss._admit = timed_admit
+    setattr(ss, name, timed_admit)
     arrival = [i / rate for i in range(nreq)]
     first, steps = {}, []
     t0 = time.perf_counter()
@@ -156,22 +196,24 @@ def service(syn, eng, texts, rows, rate, nreq, chunk):
             time.sleep(max(0.0, arrival[nxt] - now))
             continue
         s0 = time.perf_counter()
-        na = len(admits)
+        queued = ss.pending
         active = ss.active
         out = ss.step()
         s1 = time.perf_counter()
         for key, piece, _fin in out:
             if key not in first and len(piece):
                 first[key] = s1 - t0 - arrival[key]
-        steps.append(dict(wall_ms=(s1 - s0) * 1e3, streams=len(out), admitted=len(admits) > na, active_before=active))
+        steps.append(dict(wall_ms=(s1 - s0) * 1e3, streams=len(out), admitted=ss.pending < queued, active_before=active))
     audio_ms = chunk / SR * 1e3
     ttfa = np.array([first[k] for k in sorted(first)]) * 1e3
     walls = np.array([s['wall_ms'] for s in steps])
     adm = np.array([s['admitted'] for s in steps])
-    res = dict(max_rows=rows, rate_per_s=rate, requests=nreq, chunk_steps=chunk, chunk_audio_ms=audio_ms,
+    res = dict(decode_steps=decode_steps or 'whole', max_rows=rows, rate_per_s=rate, requests=nreq, chunk_steps=chunk,
+               chunk_audio_ms=audio_ms,
                ttfa_ms_p50=float(np.percentile(ttfa, 50)), ttfa_ms_p95=float(np.percentile(ttfa, 95)),
-               admissions=len(admits), admit_ms_p50=float(np.median([a['ms'] for a in admits])),
-               admit_ms_max=float(max(a['ms'] for a in admits)), admit_batch_mean=float(np.mean([a['n'] for a in admits])),
+               taco_steps=len(admits), taco_ms_p50=float(np.median([a['ms'] for a in admits])),
+               taco_ms_max=float(max(a['ms'] for a in admits)),
+               admit_batch_mean=float(np.mean([a['n'] for a in admits if a['n']] or [0])),
                admit_per_batch=[(a['n'], round(a['ms'], 2)) for a in admits],
                steps=len(steps), step_wall_ms_p50=float(np.median(walls)), step_wall_ms_p95=float(np.percentile(walls, 95)),
                step_wall_ms_p50_admitting=float(np.median(walls[adm])) if adm.any() else None,
@@ -192,6 +234,8 @@ def main():
     ap.add_argument('--rate', default='6,24', help='arrivals per second, one per --rows entry')
     ap.add_argument('--requests', default='48,128', help='requests, one per --rows entry')
     ap.add_argument('--chunk', type=int, default=2750)
+    ap.add_argument('--decode_steps', default='whole', help="'whole' and / or slice lengths k, comma-separated")
+    ap.add_argument('--slices', default='1,3,8,32,128', help='session counts of the decoder slice timing (empty: none)')
     ap.add_argument('--out', default='')
     a = ap.parse_args()
     if not torch.cuda.is_available():
@@ -214,11 +258,13 @@ def main():
         syn.engine = TacoDecoderEngine(dict(np.load(w)), device=0)
         texts = [syn.symbols.sequence_to_text(v['ids'][:-1]) for _k, v in sorted(gold['sentences'].items(), key=lambda kv: int(kv[0]))]
         syn.decode_device(texts[:2], [0, 1])                    # warm-up
-        for rows, rate, nreq in zip(*[[int(x) for x in v.split(',')] for v in (a.rows, a.rate, a.requests)]):
-            report['service'].append(service(syn, eng, texts, rows, rate, nreq, a.chunk))
+        for ds in a.decode_steps.split(','):
+            for rows, rate, nreq in zip(*[[int(x) for x in v.split(',')] for v in (a.rows, a.rate, a.requests)]):
+                report['service'].append(service(syn, eng, texts, rows, rate, nreq, a.chunk, None if ds == 'whole' else int(ds)))
     else:
         report['service'] = 'not measured: no Tacotron weights at oracle/_ref/tacotron_weights.npz'
         print(report['service'])
+    report['slices'] = slices([int(x) for x in a.slices.split(',')]) if a.slices else []
     if a.out:
         os.makedirs(os.path.dirname(os.path.abspath(a.out)), exist_ok=True)
         with open(a.out, 'w') as f:
