@@ -154,6 +154,15 @@ struct Packer {
     h.resize(off + n, 0.f);
     return off;
   }
+  // appends weight tensor `name`, which must have `shape`, as it is; returns its offset
+  size_t copy(const TensorMap& tm, const std::string& name, std::initializer_list<int64_t> shape) {
+    const b200tts_tensor* t = need(tm, name, shape);
+    size_t n = 1;
+    for (int64_t s : shape) n *= (size_t)s;
+    size_t off = add(n);
+    std::memcpy(&h[off], t->data, n * sizeof(float));
+    return off;
+  }
 };
 
 inline int round4(int x) { return (x + 3) & ~3; }

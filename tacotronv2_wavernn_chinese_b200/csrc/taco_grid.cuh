@@ -462,4 +462,87 @@ __global__ void taco_grid_finish_kernel(const int* __restrict__ error, int* __re
   if (*error) nsteps[0] = -1;
 }
 
+// dynamic shared memory of taco_grid_kernel for a sentence buffer of Txp (Tx rounded up to 4) positions
+inline size_t taco_grid_smem_bytes(const TacoGridModel& g, int Txp) {
+  const size_t fl = (size_t)g.blob + (size_t)(g.P + g.E + g.U) + 2 * g.U + (g.U + g.E) + g.P + 128 + 24 * (size_t)Txp + 176;
+  return fl * sizeof(float);
+}
+
+// ---- host: the per-block weight blobs [128][blob], cut from the batch decoder's weights in their original layouts (`w` points
+//      to host memory).  Fills the layout `g`; the blobs are empty when the model or device cannot run this kernel. -----------
+inline std::vector<float> pack_taco_grid_model(const TacoWeights& w, int sm_count, bool coop, TacoGridModel& g) {
+  const int M = w.mels, P = w.P, U = w.U, E = w.E, AD = w.A, NF = w.NF, KW = w.KW;
+  g = TacoGridModel{};
+  if (!(coop && sm_count >= kTgCtas && P == 256 && U == 256 && E == 512 && AD == 128 && M <= 96 && KW <= 64)) return {};
+  g.M = M; g.P = P; g.U = U; g.E = E; g.KW = KW;
+  int off = 0;
+  auto take = [&](int n) { int o0 = off; off += (n + 3) & ~3; return o0; };
+  g.oW1 = take(M * 2); g.oB1 = take(2);
+  g.oWfold = take((U + E) * 2); g.oBfold = take(2);
+  g.oW2 = take(P * 2); g.oB2 = take(2);
+  g.oK1 = take((P + E + U) * 8); g.oBk1 = take(8);
+  g.oK2 = take(2 * U * 8); g.oBk2 = take(8);
+  g.oWq = take(U);
+  g.oFloc = take(KW + 4);
+  g.oProj = take((U + E) * 4 + 4);
+  g.blob = off;
+  const float *W1 = w.pre1_k, *b1 = w.pre1_b, *W2 = w.pre2_k, *b2 = w.pre2_b, *K1 = w.l1_k, *bk1 = w.l1_b, *K2 = w.l2_k,
+              *bk2 = w.l2_b, *Wq = w.q_k, *lock = w.loc_k, *locb = w.loc_b, *locl = w.locl_k, *va = w.v_a, *ba = w.b_a,
+              *muk = w.mu_k, *mub = w.mu_b, *frk = w.fr_k, *frb = w.fr_b, *stk = w.st_k, *stb = w.st_b;
+  // W_f . W_1 and b_f . W_1 + b_1 in float64
+  std::vector<double> fold((size_t)(U + E) * P), bfold(P);
+  for (int i = 0; i < U + E; ++i)
+    for (int p2 = 0; p2 < P; ++p2) {
+      double a = 0;
+      for (int m = 0; m < M; ++m) a += (double)frk[(size_t)i * M + m] * (double)W1[(size_t)m * P + p2];
+      fold[(size_t)i * P + p2] = a;
+    }
+  for (int p2 = 0; p2 < P; ++p2) {
+    double a = b1[p2];
+    for (int m = 0; m < M; ++m) a += (double)frb[m] * (double)W1[(size_t)m * P + p2];
+    bfold[p2] = a;
+  }
+  std::vector<float> hb((size_t)kTgCtas * g.blob, 0.f);
+  for (int c2 = 0; c2 < kTgCtas; ++c2) {
+    float* d = &hb[(size_t)c2 * g.blob];
+    for (int j = 0; j < 2; ++j) {
+      const int col = 2 * c2 + j;
+      for (int m = 0; m < M; ++m) d[g.oW1 + m * 2 + j] = W1[(size_t)m * P + col];
+      d[g.oB1 + j] = b1[col];
+      for (int i = 0; i < U + E; ++i) d[g.oWfold + i * 2 + j] = (float)fold[(size_t)i * P + col];
+      d[g.oBfold + j] = (float)bfold[col];
+      for (int k = 0; k < P; ++k) d[g.oW2 + k * 2 + j] = W2[(size_t)k * P + col];
+      d[g.oB2 + j] = b2[col];
+      for (int gate = 0; gate < 4; ++gate) {
+        const int src = gate * U + col, dst = gate * 2 + j;
+        for (int k = 0; k < P + E + U; ++k) d[g.oK1 + k * 8 + dst] = K1[(size_t)k * 4 * U + src];
+        d[g.oBk1 + dst] = bk1[src];
+        for (int k = 0; k < 2 * U; ++k) d[g.oK2 + k * 8 + dst] = K2[(size_t)k * 4 * U + src];
+        d[g.oBk2 + dst] = bk2[src];
+      }
+    }
+    for (int u = 0; u < U; ++u) d[g.oWq + u] = Wq[(size_t)u * AD + c2];
+    double bl = ba[c2];
+    for (int f = 0; f < NF; ++f) bl += (double)locb[f] * (double)locl[(size_t)f * AD + c2];
+    for (int k = 0; k < KW; ++k) {
+      double a = 0;
+      for (int f = 0; f < NF; ++f) a += (double)lock[(size_t)k * NF + f] * (double)locl[(size_t)f * AD + c2];
+      d[g.oFloc + k] = (float)a;
+    }
+    d[g.oFloc + KW] = (float)bl;
+    d[g.oFloc + KW + 1] = va[c2];
+    d[g.oFloc + KW + 2] = 1.0f - w.zoneout;
+    d[g.oFloc + KW + 3] = w.zoneout;
+    for (int i = 0; i < U + E; ++i) {
+      d[g.oProj + i * 4 + 0] = muk[i < U ? E + i : i - U];          // attention.py:229 concatenates [context, query]
+      d[g.oProj + i * 4 + 1] = stk[i];
+      d[g.oProj + i * 4 + 2] = c2 < M ? frk[(size_t)i * M + c2] : 0.f;
+    }
+    d[g.oProj + (U + E) * 4 + 0] = mub[0];
+    d[g.oProj + (U + E) * 4 + 1] = stb[0];
+    d[g.oProj + (U + E) * 4 + 2] = c2 < M ? frb[c2] : 0.f;
+  }
+  return hb;
+}
+
 }  // namespace b200tts

@@ -45,7 +45,6 @@ struct b200tts_taco {
   const float *enc_kfw = nullptr, *enc_bfw = nullptr, *enc_kbw = nullptr, *enc_bbw = nullptr;
   const float *post_pk = nullptr, *post_pb = nullptr;
   int post_channels = 0;
-  int64_t launches = 0;
   // weight-stationary single-sentence decoder (taco_grid.cuh)
   TacoGridModel tgm{};
   DeviceBuf tg_blob, tg_vec;
@@ -71,6 +70,23 @@ static size_t taco_decoder_smem_bytes(const TacoWeights& w) {
   return fl * sizeof(float);
 }
 
+// Where each decoder weight sits in the packed blob, in floats; bind(base) points the decoder at a copy of the blob at `base`.
+struct TacoWeightOffsets {
+  size_t pre1_k, pre1_b, pre2_k, pre2_b, l1_k, l1_b, l2_k, l2_b, q_k, loc_k, loc_b, locl_k, v_a, b_a, mu_k, mu_b, fr_k, fr_b, st_k,
+      st_b, mem_k;
+  TacoWeights bind(const float* b, const b200tts_taco_cfg& c) const {
+    TacoWeights w{};
+    w.pre1_k = b + pre1_k; w.pre1_b = b + pre1_b; w.pre2_k = b + pre2_k; w.pre2_b = b + pre2_b;
+    w.l1_k = b + l1_k; w.l1_b = b + l1_b; w.l2_k = b + l2_k; w.l2_b = b + l2_b;
+    w.q_k = b + q_k; w.loc_k = b + loc_k; w.loc_b = b + loc_b; w.locl_k = b + locl_k; w.v_a = b + v_a; w.b_a = b + b_a;
+    w.mu_k = b + mu_k; w.mu_b = b + mu_b; w.fr_k = b + fr_k; w.fr_b = b + fr_b; w.st_k = b + st_k; w.st_b = b + st_b;
+    w.mem_k = b + mem_k;
+    w.mels = c.num_mels; w.P = c.prenet_units; w.U = c.lstm_units; w.E = c.enc_dim; w.A = c.attn_dim; w.NF = c.attn_filters;
+    w.KW = c.attn_kernel; w.zoneout = c.zoneout;
+    return w;
+  }
+};
+
 extern "C" int b200tts_taco_create(b200tts_taco** out, int device, const b200tts_taco_cfg* cfg, const b200tts_tensor* weights,
                                    int n_weights) {
   API_BEGIN
@@ -92,32 +108,25 @@ extern "C" int b200tts_taco_create(b200tts_taco** out, int device, const b200tts
   ctx->device = device;
   ctx->cfg = c;
   Packer pk;
-  auto copy = [&](const std::string& name, std::initializer_list<int64_t> shape) {
-    const b200tts_tensor* t = need(tm, name, shape);
-    size_t n = 1;
-    for (int64_t s : shape) n *= (size_t)s;
-    size_t off = pk.add(n);
-    std::memcpy(&pk.h[off], t->data, n * sizeof(float));
-    return off;
-  };
   const std::string D = "decoder/", L = D + "Location_Sensitive_Attention/";
-  size_t o[21];
-  o[0] = copy(D + "decoder_prenet/dense_1/kernel", {M, P}); o[1] = copy(D + "decoder_prenet/dense_1/bias", {P});
-  o[2] = copy(D + "decoder_prenet/dense_2/kernel", {P, P}); o[3] = copy(D + "decoder_prenet/dense_2/bias", {P});
-  o[4] = copy(D + "decoder_LSTM/multi_rnn_cell/cell_0/decoder_LSTM_1/kernel", {P + E + U, 4 * U});
-  o[5] = copy(D + "decoder_LSTM/multi_rnn_cell/cell_0/decoder_LSTM_1/bias", {4 * U});
-  o[6] = copy(D + "decoder_LSTM/multi_rnn_cell/cell_1/decoder_LSTM_2/kernel", {2 * U, 4 * U});
-  o[7] = copy(D + "decoder_LSTM/multi_rnn_cell/cell_1/decoder_LSTM_2/bias", {4 * U});
-  o[8] = copy(L + "query_layer/kernel", {U, AD});
-  o[9] = copy(L + "location_features_convolution/kernel", {KW, 1, NF}); o[10] = copy(L + "location_features_convolution/bias", {NF});
-  o[11] = copy(L + "location_features_layer/kernel", {NF, AD});
-  o[12] = copy(L + "attention_variable_projection", {AD}); o[13] = copy(L + "attention_bias", {AD});
-  o[14] = copy(D + "dense/kernel", {E + U, 1}); o[15] = copy(D + "dense/bias", {1});
-  o[16] = copy(D + "linear_transform_projection/projection_linear_transform_projection/kernel", {U + E, M});
-  o[17] = copy(D + "linear_transform_projection/projection_linear_transform_projection/bias", {M});
-  o[18] = copy(D + "stop_token_projection/projection_stop_token_projection/kernel", {U + E, 1});
-  o[19] = copy(D + "stop_token_projection/projection_stop_token_projection/bias", {1});
-  o[20] = copy("memory_layer/kernel", {E, AD});
+  TacoWeightOffsets o{};
+  o.pre1_k = pk.copy(tm, D + "decoder_prenet/dense_1/kernel", {M, P}); o.pre1_b = pk.copy(tm, D + "decoder_prenet/dense_1/bias", {P});
+  o.pre2_k = pk.copy(tm, D + "decoder_prenet/dense_2/kernel", {P, P}); o.pre2_b = pk.copy(tm, D + "decoder_prenet/dense_2/bias", {P});
+  o.l1_k = pk.copy(tm, D + "decoder_LSTM/multi_rnn_cell/cell_0/decoder_LSTM_1/kernel", {P + E + U, 4 * U});
+  o.l1_b = pk.copy(tm, D + "decoder_LSTM/multi_rnn_cell/cell_0/decoder_LSTM_1/bias", {4 * U});
+  o.l2_k = pk.copy(tm, D + "decoder_LSTM/multi_rnn_cell/cell_1/decoder_LSTM_2/kernel", {2 * U, 4 * U});
+  o.l2_b = pk.copy(tm, D + "decoder_LSTM/multi_rnn_cell/cell_1/decoder_LSTM_2/bias", {4 * U});
+  o.q_k = pk.copy(tm, L + "query_layer/kernel", {U, AD});
+  o.loc_k = pk.copy(tm, L + "location_features_convolution/kernel", {KW, 1, NF});
+  o.loc_b = pk.copy(tm, L + "location_features_convolution/bias", {NF});
+  o.locl_k = pk.copy(tm, L + "location_features_layer/kernel", {NF, AD});
+  o.v_a = pk.copy(tm, L + "attention_variable_projection", {AD}); o.b_a = pk.copy(tm, L + "attention_bias", {AD});
+  o.mu_k = pk.copy(tm, D + "dense/kernel", {E + U, 1}); o.mu_b = pk.copy(tm, D + "dense/bias", {1});
+  o.fr_k = pk.copy(tm, D + "linear_transform_projection/projection_linear_transform_projection/kernel", {U + E, M});
+  o.fr_b = pk.copy(tm, D + "linear_transform_projection/projection_linear_transform_projection/bias", {M});
+  o.st_k = pk.copy(tm, D + "stop_token_projection/projection_stop_token_projection/kernel", {U + E, 1});
+  o.st_b = pk.copy(tm, D + "stop_token_projection/projection_stop_token_projection/bias", {1});
+  o.mem_k = pk.copy(tm, "memory_layer/kernel", {E, AD});
   // ---- optional run-once neighbours: encoder and postnet ----
   struct ConvOff { size_t K, bias, scale, shift; int k, Cin, Cout; };
   auto pack_conv = [&](const std::string& scope) {
@@ -126,8 +135,8 @@ extern "C" int b200tts_taco_create(b200tts_taco** out, int device, const b200tts
     const b200tts_tensor* kt = it->second;
     ConvOff c{};
     c.k = (int)kt->shape[0]; c.Cin = (int)kt->shape[1]; c.Cout = (int)kt->shape[2];
-    c.K = copy(scope + "/conv1d/kernel", {c.k, c.Cin, c.Cout});
-    c.bias = copy(scope + "/conv1d/bias", {c.Cout});
+    c.K = pk.copy(tm, scope + "/conv1d/kernel", {c.k, c.Cin, c.Cout});
+    c.bias = pk.copy(tm, scope + "/conv1d/bias", {c.Cout});
     const float* g = need(tm, scope + "/batch_normalization/gamma", {c.Cout})->data;
     const float* be = need(tm, scope + "/batch_normalization/beta", {c.Cout})->data;
     const float* mu = need(tm, scope + "/batch_normalization/moving_mean", {c.Cout})->data;
@@ -146,14 +155,14 @@ extern "C" int b200tts_taco_create(b200tts_taco** out, int device, const b200tts
     const b200tts_tensor* et = tm["inputs_embedding"];
     REQUIRE(et->ndim == 2, B200TTS_ESHAPE, "inputs_embedding must be 2-D");
     ctx->vocab = (int)et->shape[0]; ctx->emb_dim = (int)et->shape[1];
-    o_emb = copy("inputs_embedding", {ctx->vocab, ctx->emb_dim});
+    o_emb = pk.copy(tm, "inputs_embedding", {ctx->vocab, ctx->emb_dim});
     for (int i = 0; i < 3; ++i) encc[i] = pack_conv("encoder_convolutions/conv_layer_" + std::to_string(i + 1) + "_encoder_convolutions");
     REQUIRE(encc[0].Cin == ctx->emb_dim && encc[2].Cout % 4 == 0 && E % 2 == 0, B200TTS_ESHAPE, "encoder conv shapes");
     const int EU = E / 2, CI = encc[2].Cout;
     REQUIRE(4 * EU == 1024, B200TTS_EINVAL, "encoder LSTM units must be 256");
     const std::string LS = "encoder_LSTM/bidirectional_rnn/";
-    o_kfw = copy(LS + "fw/encoder_fw_LSTM/kernel", {CI + EU, 4 * EU}); o_bfw = copy(LS + "fw/encoder_fw_LSTM/bias", {4 * EU});
-    o_kbw = copy(LS + "bw/encoder_bw_LSTM/kernel", {CI + EU, 4 * EU}); o_bbw = copy(LS + "bw/encoder_bw_LSTM/bias", {4 * EU});
+    o_kfw = pk.copy(tm, LS + "fw/encoder_fw_LSTM/kernel", {CI + EU, 4 * EU}); o_bfw = pk.copy(tm, LS + "fw/encoder_fw_LSTM/bias", {4 * EU});
+    o_kbw = pk.copy(tm, LS + "bw/encoder_bw_LSTM/kernel", {CI + EU, 4 * EU}); o_bbw = pk.copy(tm, LS + "bw/encoder_bw_LSTM/bias", {4 * EU});
     ctx->enc_units = EU;
     ctx->has_encoder = true;
   }
@@ -161,20 +170,14 @@ extern "C" int b200tts_taco_create(b200tts_taco** out, int device, const b200tts
     for (int i = 0; i < 5; ++i) postc[i] = pack_conv("postnet_convolutions/conv_layer_" + std::to_string(i + 1) + "_postnet_convolutions");
     REQUIRE(postc[0].Cin == M, B200TTS_ESHAPE, "postnet conv 1 must take num_mels channels");
     ctx->post_channels = postc[4].Cout;
-    o_pk = copy("postnet_projection/projection_postnet_projection/kernel", {ctx->post_channels, M});
-    o_pb = copy("postnet_projection/projection_postnet_projection/bias", {M});
+    o_pk = pk.copy(tm, "postnet_projection/projection_postnet_projection/kernel", {ctx->post_channels, M});
+    o_pb = pk.copy(tm, "postnet_projection/projection_postnet_projection/bias", {M});
     ctx->has_postnet = true;
   }
   ctx->weights.ensure(pk.h.size() * sizeof(float));
   B200_CUDA(cudaMemcpy(ctx->weights.p, pk.h.data(), pk.h.size() * sizeof(float), cudaMemcpyHostToDevice));
   const float* b = ctx->weights.as<float>();
-  TacoWeights& w = ctx->tw;
-  w.pre1_k = b + o[0]; w.pre1_b = b + o[1]; w.pre2_k = b + o[2]; w.pre2_b = b + o[3];
-  w.l1_k = b + o[4]; w.l1_b = b + o[5]; w.l2_k = b + o[6]; w.l2_b = b + o[7];
-  w.q_k = b + o[8]; w.loc_k = b + o[9]; w.loc_b = b + o[10]; w.locl_k = b + o[11]; w.v_a = b + o[12]; w.b_a = b + o[13];
-  w.mu_k = b + o[14]; w.mu_b = b + o[15]; w.fr_k = b + o[16]; w.fr_b = b + o[17]; w.st_k = b + o[18]; w.st_b = b + o[19];
-  w.mem_k = b + o[20];
-  w.mels = M; w.P = P; w.U = U; w.E = E; w.A = AD; w.NF = NF; w.KW = KW; w.zoneout = c.zoneout;
+  ctx->tw = o.bind(b, c);
   auto bind = [&](const ConvOff& c0) { return TacoConvW{b + c0.K, b + c0.bias, b + c0.scale, b + c0.shift, c0.k, c0.Cin, c0.Cout}; };
   if (ctx->has_encoder) {
     ctx->embedding = b + o_emb;
@@ -186,85 +189,14 @@ extern "C" int b200tts_taco_create(b200tts_taco** out, int device, const b200tts
     ctx->post_pk = b + o_pk; ctx->post_pb = b + o_pb;
   }
   // ---- per-block weight blobs of the weight-stationary single-sentence decoder (taco_grid.cuh) ----
-  {
-    int coop = 0;
-    B200_CUDA(cudaDeviceGetAttribute(&coop, cudaDevAttrCooperativeLaunch, device));
-    B200_CUDA(cudaDeviceGetAttribute(&ctx->sm_count, cudaDevAttrMultiProcessorCount, device));
-    if (coop && ctx->sm_count >= kTgCtas && P == 256 && U == 256 && E == 512 && AD == 128 && M <= 96 && KW <= 64) {
-      TacoGridModel& g = ctx->tgm;
-      g.M = M; g.P = P; g.U = U; g.E = E; g.KW = KW;
-      int off = 0;
-      auto take = [&](int n) { int o0 = off; off += (n + 3) & ~3; return o0; };
-      g.oW1 = take(M * 2); g.oB1 = take(2);
-      g.oWfold = take((U + E) * 2); g.oBfold = take(2);
-      g.oW2 = take(P * 2); g.oB2 = take(2);
-      g.oK1 = take((P + E + U) * 8); g.oBk1 = take(8);
-      g.oK2 = take(2 * U * 8); g.oBk2 = take(8);
-      g.oWq = take(U);
-      g.oFloc = take(KW + 4);
-      g.oProj = take((U + E) * 4 + 4);
-      g.blob = off;
-      const float* H = pk.h.data();
-      const float *W1 = H + o[0], *b1 = H + o[1], *W2 = H + o[2], *b2 = H + o[3], *K1 = H + o[4], *bk1 = H + o[5], *K2 = H + o[6],
-                  *bk2 = H + o[7], *Wq = H + o[8], *lock = H + o[9], *locb = H + o[10], *locl = H + o[11], *va = H + o[12], *ba = H + o[13],
-                  *muk = H + o[14], *mub = H + o[15], *frk = H + o[16], *frb = H + o[17], *stk = H + o[18], *stb = H + o[19];
-      // W_f . W_1 and b_f . W_1 + b_1 in float64
-      std::vector<double> fold((size_t)(U + E) * P), bfold(P);
-      for (int i = 0; i < U + E; ++i)
-        for (int p2 = 0; p2 < P; ++p2) {
-          double a = 0;
-          for (int m = 0; m < M; ++m) a += (double)frk[(size_t)i * M + m] * (double)W1[(size_t)m * P + p2];
-          fold[(size_t)i * P + p2] = a;
-        }
-      for (int p2 = 0; p2 < P; ++p2) {
-        double a = b1[p2];
-        for (int m = 0; m < M; ++m) a += (double)frb[m] * (double)W1[(size_t)m * P + p2];
-        bfold[p2] = a;
-      }
-      std::vector<float> hb((size_t)kTgCtas * g.blob, 0.f);
-      for (int c2 = 0; c2 < kTgCtas; ++c2) {
-        float* d = &hb[(size_t)c2 * g.blob];
-        for (int j = 0; j < 2; ++j) {
-          const int col = 2 * c2 + j;
-          for (int m = 0; m < M; ++m) d[g.oW1 + m * 2 + j] = W1[(size_t)m * P + col];
-          d[g.oB1 + j] = b1[col];
-          for (int i = 0; i < U + E; ++i) d[g.oWfold + i * 2 + j] = (float)fold[(size_t)i * P + col];
-          d[g.oBfold + j] = (float)bfold[col];
-          for (int k = 0; k < P; ++k) d[g.oW2 + k * 2 + j] = W2[(size_t)k * P + col];
-          d[g.oB2 + j] = b2[col];
-          for (int gate = 0; gate < 4; ++gate) {
-            const int src = gate * U + col, dst = gate * 2 + j;
-            for (int k = 0; k < P + E + U; ++k) d[g.oK1 + k * 8 + dst] = K1[(size_t)k * 4 * U + src];
-            d[g.oBk1 + dst] = bk1[src];
-            for (int k = 0; k < 2 * U; ++k) d[g.oK2 + k * 8 + dst] = K2[(size_t)k * 4 * U + src];
-            d[g.oBk2 + dst] = bk2[src];
-          }
-        }
-        for (int u = 0; u < U; ++u) d[g.oWq + u] = Wq[(size_t)u * AD + c2];
-        double bl = ba[c2];
-        for (int f = 0; f < NF; ++f) bl += (double)locb[f] * (double)locl[(size_t)f * AD + c2];
-        for (int k = 0; k < KW; ++k) {
-          double a = 0;
-          for (int f = 0; f < NF; ++f) a += (double)lock[(size_t)k * NF + f] * (double)locl[(size_t)f * AD + c2];
-          d[g.oFloc + k] = (float)a;
-        }
-        d[g.oFloc + KW] = (float)bl;
-        d[g.oFloc + KW + 1] = va[c2];
-        d[g.oFloc + KW + 2] = 1.0f - c.zoneout;
-        d[g.oFloc + KW + 3] = c.zoneout;
-        for (int i = 0; i < U + E; ++i) {
-          d[g.oProj + i * 4 + 0] = muk[i < U ? E + i : i - U];          // attention.py:229 concatenates [context, query]
-          d[g.oProj + i * 4 + 1] = stk[i];
-          d[g.oProj + i * 4 + 2] = c2 < M ? frk[(size_t)i * M + c2] : 0.f;
-        }
-        d[g.oProj + (U + E) * 4 + 0] = mub[0];
-        d[g.oProj + (U + E) * 4 + 1] = stb[0];
-        d[g.oProj + (U + E) * 4 + 2] = c2 < M ? frb[c2] : 0.f;
-      }
-      ctx->tg_blob.ensure(hb.size() * sizeof(float));
-      B200_CUDA(cudaMemcpy(ctx->tg_blob.p, hb.data(), hb.size() * sizeof(float), cudaMemcpyHostToDevice));
-      ctx->tg_ok = true;
-    }
+  int coop = 0;
+  B200_CUDA(cudaDeviceGetAttribute(&coop, cudaDevAttrCooperativeLaunch, device));
+  B200_CUDA(cudaDeviceGetAttribute(&ctx->sm_count, cudaDevAttrMultiProcessorCount, device));
+  const std::vector<float> gb = pack_taco_grid_model(o.bind(pk.h.data(), c), ctx->sm_count, coop != 0, ctx->tgm);
+  if (!gb.empty()) {
+    ctx->tg_blob.ensure(gb.size() * sizeof(float));
+    B200_CUDA(cudaMemcpy(ctx->tg_blob.p, gb.data(), gb.size() * sizeof(float), cudaMemcpyHostToDevice));
+    ctx->tg_ok = true;
   }
   *out = ctx.release();
   API_END
@@ -284,42 +216,46 @@ static void require_mu_bias(const float* h_mu_bias, int B) {
               "mu_bias[" + std::to_string(b) + "] must be finite and in [-1, 1]");
 }
 
-// h_mu_bias: NULL for the unbiased kernels, else [B] host speaking-rate biases (b200tts_taco_decode_biased)
-static int taco_decode_impl(b200tts_taco* ctx, const float* d_memory, const int32_t* d_lengths, int B, int Tx_max,
-                            const b200tts_taco_dropout* dropout, int max_steps, int window, const float* h_mu_bias,
-                            const float* d_forced, float* d_frames, float* d_stop, float* d_align, int32_t* d_nsteps, void* stream) {
-  API_BEGIN
-  REQUIRE(ctx && d_memory && d_lengths && d_frames && d_stop && d_nsteps, B200TTS_EINVAL, "null argument");
-  REQUIRE(B >= 1 && Tx_max >= 1 && Tx_max <= kTacoMaxTx && max_steps >= 1, B200TTS_EINVAL, "B, Tx_max (<= 512), max_steps out of range");
-  b200tts_taco_dropout d{};
-  if (dropout) d = *dropout;
+static void require_dropout(const b200tts_taco_dropout& d) {
   REQUIRE(d.mode == B200TTS_TACO_DROPOUT_PHILOX || (d.mode == B200TTS_TACO_DROPOUT_EXT && d.d_masks), B200TTS_EINVAL,
           "bad dropout descriptor");
-  require_mu_bias(h_mu_bias, B);
+}
+
+// keys[r][:] = memory[r][:] . W_memory for `rows` rows of the encoder output
+static void launch_taco_keys(const TacoWeights& w, const float* memory, int rows, float* keys, cudaStream_t st) {
+  taco_keys_kernel<<<rows, 128, w.E * sizeof(float), st>>>(memory, w.mem_k, rows, w.E, w.A, keys);
+  B200_CUDA(cudaGetLastError());
+}
+
+enum class TacoDecoder { kBatch, kBatchBiased, kGta, kGrid, kGridBiased };
+
+// Teacher-forced (GTA) decoding runs one thread block per sentence at every B: it is a batch job, so the single-sentence grid
+// decoder is not taught the fed frame.  Otherwise a lone sentence runs on the grid decoder where the model and device allow it.
+static TacoDecoder choose_taco_decoder(const b200tts_taco* ctx, int B, bool gta, bool biased) {
+  if (gta) return TacoDecoder::kGta;
+  if (B == 1 && ctx->tg_ok) return biased ? TacoDecoder::kGridBiased : TacoDecoder::kGrid;
+  return biased ? TacoDecoder::kBatchBiased : TacoDecoder::kBatch;
+}
+
+// Every b200tts_taco_decode* call once its arguments have been checked: uploads the biases (h_mu_bias: [B] on the host, or
+// NULL), computes the keys into `a` and runs the decoder choose_taco_decoder picks.  gta: the recorded mels of a GTA run, or NULL.
+static void launch_taco_decoder(b200tts_taco* ctx, TacoArgs a, const TacoGtaArgs* gta, const float* h_mu_bias, cudaStream_t st) {
   DeviceGuard dg(ctx->device);
-  cudaStream_t st = (cudaStream_t)stream;
   const TacoWeights& w = ctx->tw;
   const float* d_mu_bias = nullptr;
   if (h_mu_bias) {
-    ctx->mu_bias.ensure((size_t)B * sizeof(float));
-    B200_CUDA(cudaMemcpyAsync(ctx->mu_bias.p, h_mu_bias, (size_t)B * sizeof(float), cudaMemcpyHostToDevice, st));
+    ctx->mu_bias.ensure((size_t)a.B * sizeof(float));
+    B200_CUDA(cudaMemcpyAsync(ctx->mu_bias.p, h_mu_bias, (size_t)a.B * sizeof(float), cudaMemcpyHostToDevice, st));
     d_mu_bias = ctx->mu_bias.as<float>();
   }
-  ctx->keys.ensure((size_t)B * Tx_max * w.A * sizeof(float));
-  taco_keys_kernel<<<B * Tx_max, 128, w.E * sizeof(float), st>>>(d_memory, w.mem_k, B * Tx_max, w.E, w.A, ctx->keys.as<float>());
-  B200_CUDA(cudaGetLastError());
-  TacoArgs a{};
-  a.memory = d_memory; a.keys = ctx->keys.as<float>(); a.lengths = d_lengths;
-  a.B = B; a.Tx_max = Tx_max; a.max_steps = max_steps; a.window = window;
-  a.rng_mode = d.mode; a.seed = d.seed; a.utt_offset = d.utterance_offset; a.masks = d.d_masks;
-  a.frames = d_frames; a.stop = d_stop; a.align = d_align; a.nsteps = d_nsteps;
-  a.forced = d_forced;
-  if (B == 1 && ctx->tg_ok) {
-    // ONE sentence: the weight-stationary 128-block decoder (taco_grid.cuh).  The sentence length is needed on the host to size
-    // the exchange buffers; d_lengths is a device pointer, so Tx_max (the caller's padded length) bounds it and the kernel
-    // reads the true length itself.
-    const TacoGridModel& g = ctx->tgm;
-    const int Txp = (Tx_max + 3) & ~3;
+  ctx->keys.ensure((size_t)a.B * a.Tx_max * w.A * sizeof(float));
+  a.keys = ctx->keys.as<float>();
+  launch_taco_keys(w, a.memory, a.B * a.Tx_max, ctx->keys.as<float>(), st);
+  const TacoDecoder k = choose_taco_decoder(ctx, a.B, gta != nullptr, h_mu_bias != nullptr);
+  if (k == TacoDecoder::kGrid || k == TacoDecoder::kGridBiased) {
+    // The sentence length is needed on the host to size the exchange buffers; a.lengths is a device pointer, so Tx_max (the
+    // caller's padded length) bounds it and the kernel reads the true length itself.
+    const int Txp = (a.Tx_max + 3) & ~3;
     const size_t copy = (size_t)2048 + (size_t)kTgCtas * Txp;
     ctx->tg_vec.ensure(2 * copy * sizeof(float) + 64);
     int* d_err = reinterpret_cast<int*>(ctx->tg_vec.as<float>() + 2 * copy);
@@ -328,35 +264,56 @@ static int taco_decode_impl(b200tts_taco* ctx, const float* d_memory, const int3
     ga.wblob = ctx->tg_blob.as<float>();
     ga.vec = ctx->tg_vec.as<float>();
     ga.error = d_err;
-    ga.memory = d_memory; ga.keys = ctx->keys.as<float>();
-    ga.lengths = d_lengths;
-    ga.Tx = Tx_max; ga.Txp = Txp; ga.max_steps = max_steps; ga.window = window;
-    ga.rng_mode = d.mode; ga.seed = d.seed; ga.utt = d.utterance_offset; ga.masks = d.d_masks;
-    ga.forced = d_forced; ga.Tx_alloc = Tx_max;
-    ga.frames = d_frames; ga.stop = d_stop; ga.align = d_align; ga.nsteps = d_nsteps;
-    const size_t fl = (size_t)g.blob + (size_t)(w.P + w.E + w.U) + 2 * w.U + (w.U + w.E) + w.P + 128 + 24 * (size_t)Txp + 176;
-    const size_t smem = fl * sizeof(float);
+    ga.memory = a.memory; ga.keys = a.keys;
+    ga.lengths = a.lengths;
+    ga.Tx = a.Tx_max; ga.Txp = Txp; ga.max_steps = a.max_steps; ga.window = a.window;
+    ga.rng_mode = a.rng_mode; ga.seed = a.seed; ga.utt = a.utt_offset; ga.masks = a.masks;
+    ga.forced = a.forced; ga.Tx_alloc = a.Tx_max;
+    ga.frames = a.frames; ga.stop = a.stop; ga.align = a.align; ga.nsteps = a.nsteps;
+    const size_t smem = taco_grid_smem_bytes(ctx->tgm, Txp);
     REQUIRE(smem <= 227 * 1024, B200TTS_EINVAL, "taco_grid_kernel: shared memory budget exceeded");
-    const void* kernel = d_mu_bias ? (const void*)taco_grid_biased_kernel : (const void*)taco_grid_kernel;
+    const void* kernel = k == TacoDecoder::kGridBiased ? (const void*)taco_grid_biased_kernel : (const void*)taco_grid_kernel;
     B200_CUDA(cudaFuncSetAttribute(kernel, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)smem));
-    TacoGridModel gm = g;
+    TacoGridModel gm = ctx->tgm;
     void* args[] = {(void*)&gm, (void*)&ga, (void*)&d_mu_bias};
     B200_CUDA(cudaLaunchCooperativeKernel(kernel, dim3(kTgCtas), dim3(kTgThreads), args, smem, st));
-    taco_grid_finish_kernel<<<1, 1, 0, st>>>(d_err, d_nsteps);
+    taco_grid_finish_kernel<<<1, 1, 0, st>>>(d_err, a.nsteps);
     B200_CUDA(cudaGetLastError());
-    ctx->launches += 4;
-    return B200TTS_OK;
+    return;
   }
+  // Named in this order, the instantiations of taco_decoder_kernel keep their places in the module, and with them the code ptxas
+  // gives the grid kernels.
   const size_t smem = taco_decoder_smem_bytes(w);
-  if (d_mu_bias) {
+  if (k == TacoDecoder::kBatchBiased) {
     B200_CUDA(cudaFuncSetAttribute(taco_decoder_biased_kernel, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)smem));
-    taco_decoder_biased_kernel<<<B, kTacoThreads, smem, st>>>(w, a, d_mu_bias);
-  } else {
+    taco_decoder_biased_kernel<<<a.B, kTacoThreads, smem, st>>>(w, a, d_mu_bias);
+  } else if (k == TacoDecoder::kBatch) {
     B200_CUDA(cudaFuncSetAttribute(taco_decoder_kernel<false>, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)smem));
-    taco_decoder_kernel<false><<<B, kTacoThreads, smem, st>>>(w, a, TacoGtaArgs{});
+    taco_decoder_kernel<false><<<a.B, kTacoThreads, smem, st>>>(w, a, TacoGtaArgs{});
+  } else {
+    B200_CUDA(cudaFuncSetAttribute(taco_decoder_kernel<true>, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)smem));
+    taco_decoder_kernel<true><<<a.B, kTacoThreads, smem, st>>>(w, a, *gta);
   }
   B200_CUDA(cudaGetLastError());
-  ctx->launches += 2;
+}
+
+// free, forced (d_forced: state records) or biased (h_mu_bias: [B] host speaking-rate biases) decoding
+static int taco_decode_impl(b200tts_taco* ctx, const float* d_memory, const int32_t* d_lengths, int B, int Tx_max,
+                            const b200tts_taco_dropout* dropout, int max_steps, int window, const float* h_mu_bias,
+                            const float* d_forced, float* d_frames, float* d_stop, float* d_align, int32_t* d_nsteps, void* stream) {
+  API_BEGIN
+  REQUIRE(ctx && d_memory && d_lengths && d_frames && d_stop && d_nsteps, B200TTS_EINVAL, "null argument");
+  REQUIRE(B >= 1 && Tx_max >= 1 && Tx_max <= kTacoMaxTx && max_steps >= 1, B200TTS_EINVAL, "B, Tx_max (<= 512), max_steps out of range");
+  b200tts_taco_dropout d{};
+  if (dropout) d = *dropout;
+  require_dropout(d);
+  require_mu_bias(h_mu_bias, B);
+  TacoArgs a{};
+  a.memory = d_memory; a.lengths = d_lengths;
+  a.B = B; a.Tx_max = Tx_max; a.max_steps = max_steps; a.window = window;
+  a.rng_mode = d.mode; a.seed = d.seed; a.utt_offset = d.utterance_offset; a.masks = d.d_masks;
+  a.frames = d_frames; a.stop = d_stop; a.align = d_align; a.nsteps = d_nsteps; a.forced = d_forced;
+  launch_taco_decoder(ctx, a, nullptr, h_mu_bias, (cudaStream_t)stream);
   API_END
 }
 
@@ -402,27 +359,14 @@ extern "C" int b200tts_taco_decode_gta(b200tts_taco* ctx, const float* d_memory,
   REQUIRE(ctx && d_memory && d_lengths && dropout && d_targets && d_target_lengths && d_frames, B200TTS_EINVAL, "null argument");
   REQUIRE(B >= 1 && Tx_max >= 1 && Tx_max <= kTacoMaxTx && Ty_max >= 1, B200TTS_EINVAL, "B, Tx_max (<= 512), Ty_max out of range");
   const b200tts_taco_dropout d = *dropout;
-  REQUIRE(d.mode == B200TTS_TACO_DROPOUT_PHILOX || (d.mode == B200TTS_TACO_DROPOUT_EXT && d.d_masks), B200TTS_EINVAL,
-          "bad dropout descriptor");
-  DeviceGuard dg(ctx->device);
-  cudaStream_t st = (cudaStream_t)stream;
-  const TacoWeights& w = ctx->tw;
-  ctx->keys.ensure((size_t)B * Tx_max * w.A * sizeof(float));
-  taco_keys_kernel<<<B * Tx_max, 128, w.E * sizeof(float), st>>>(d_memory, w.mem_k, B * Tx_max, w.E, w.A, ctx->keys.as<float>());
-  B200_CUDA(cudaGetLastError());
-  // one CTA per sentence at every B: a batch job, so the single-sentence grid decoder is not taught the fed frame
+  require_dropout(d);
   TacoArgs a{};
-  a.memory = d_memory; a.keys = ctx->keys.as<float>(); a.lengths = d_lengths;
+  a.memory = d_memory; a.lengths = d_lengths;
   a.B = B; a.Tx_max = Tx_max; a.max_steps = Ty_max; a.window = 0;
   a.rng_mode = d.mode; a.seed = d.seed; a.utt_offset = d.utterance_offset; a.masks = d.d_masks;
   a.frames = d_frames; a.align = d_align;
-  TacoGtaArgs g{};
-  g.targets = d_targets; g.target_lengths = d_target_lengths;
-  const size_t smem = taco_decoder_smem_bytes(w);
-  B200_CUDA(cudaFuncSetAttribute(taco_decoder_kernel<true>, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)smem));
-  taco_decoder_kernel<true><<<B, kTacoThreads, smem, st>>>(w, a, g);
-  B200_CUDA(cudaGetLastError());
-  ctx->launches += 2;
+  const TacoGtaArgs g{d_targets, d_target_lengths};
+  launch_taco_decoder(ctx, a, &g, nullptr, (cudaStream_t)stream);
   API_END
 }
 
@@ -491,9 +435,7 @@ extern "C" int b200tts_taco_session_open_batch(b200tts_taco* ctx, const float* d
   float* rest = keys + keys_f;
   B200_CUDA(cudaMemcpyAsync(mem, d_memory, mem_f * sizeof(float), cudaMemcpyDeviceToDevice, st));
   B200_CUDA(cudaMemsetAsync(rest, 0, zero_f * sizeof(float), st));
-  taco_keys_kernel<<<n * Tx_max, 128, w.E * sizeof(float), st>>>(mem, w.mem_k, n * Tx_max, w.E, w.A, keys);
-  B200_CUDA(cudaGetLastError());
-  ctx->launches++;
+  launch_taco_keys(w, mem, n * Tx_max, keys, st);
   std::vector<std::unique_ptr<b200tts_taco_session>> ss(n);
   for (int i = 0; i < n; ++i) {
     ss[i].reset(new b200tts_taco_session());
@@ -572,7 +514,6 @@ extern "C" int b200tts_taco_session_run(b200tts_taco* ctx, b200tts_taco_session*
   int* d_status = ctx->sess_status.as<int>();
   for (int u = 0; u < m; ++u) io.row[u].status = d_status + 2 * u;
   launch_taco_sessions(ctx->tw, io, m, taco_decoder_smem_bytes(ctx->tw), st);
-  ctx->launches++;
   // where each decode stopped is decided on the device: wait for the slice and read the positions back
   int* h = static_cast<int*>(ctx->h_sess_status.p);
   B200_CUDA(cudaMemcpyAsync(h, d_status, (size_t)m * 2 * sizeof(int), cudaMemcpyDeviceToHost, st));
@@ -599,7 +540,6 @@ extern "C" int b200tts_taco_session_outputs(b200tts_taco_session* const* s, int 
   b200tts_taco* ctx = s[0]->ctx;
   DeviceGuard dg(ctx->device);
   launch_taco_session_outputs(g, n, T_max, ctx->tw.mels, d_frames, d_stop, d_nsteps, (cudaStream_t)stream);
-  ctx->launches++;
   API_END
 }
 
@@ -613,7 +553,6 @@ static void taco_launch_conv(b200tts_taco* ctx, const TacoConvW& cw, const float
   dim3 grid((Tmax + kConvTile - 1) / kConvTile, B);
   taco_conv_bn_kernel<<<grid, 256, smem, st>>>(a);
   B200_CUDA(cudaGetLastError());
-  ctx->launches++;
 }
 
 extern "C" int b200tts_taco_encode(b200tts_taco* ctx, const int32_t* d_ids, const int32_t* d_lengths, int B, int Tx_max, float* d_memory,
@@ -638,7 +577,6 @@ extern "C" int b200tts_taco_encode(b200tts_taco* ctx, const int32_t* d_ids, cons
   taco_bilstm_kernel<<<dim3(B, 2), kTacoThreads, smem, st>>>(a, d_lengths, Tx_max, Cin, U, ctx->enc_kfw, ctx->enc_bfw, ctx->enc_kbw,
                                                               ctx->enc_bbw, ctx->cfg.zoneout, d_memory);
   B200_CUDA(cudaGetLastError());
-  ctx->launches++;
   API_END
 }
 
@@ -664,6 +602,5 @@ extern "C" int b200tts_taco_postnet(b200tts_taco* ctx, const float* d_frames, co
   taco_postnet_proj_kernel<<<dim3(max_steps, B), 128, C * sizeof(float), st>>>(d_frames, a, d_nsteps, max_steps, C, M, ctx->post_pk,
                                                                                  ctx->post_pb, lo, hi, d_mel);
   B200_CUDA(cudaGetLastError());
-  ctx->launches++;
   API_END
 }

@@ -131,21 +131,13 @@ static StepWeights pack_original(b200tts_wavernn* ctx, const TensorMap& tm, Pack
   const float* Iw = need(tm, "I.weight", {R, nin})->data;
   size_t oI = pk.add((size_t)R * ldI);
   for (int r = 0; r < R; ++r) std::memcpy(&pk.h[oI + (size_t)r * ldI], Iw + (size_t)r * nin, sizeof(float) * nin);
-  auto copy = [&](const std::string& name, std::initializer_list<int64_t> shape) {
-    const b200tts_tensor* t = need(tm, name, shape);
-    size_t n = 1;
-    for (int64_t s : shape) n *= (size_t)s;
-    size_t off = pk.add(n);
-    std::memcpy(&pk.h[off], t->data, n * sizeof(float));
-    return off;
-  };
-  size_t oIb = copy("I.bias", {R});
-  size_t o_ih1 = copy("rnn1.weight_ih_l0", {3 * R, R}), o_hh1 = copy("rnn1.weight_hh_l0", {3 * R, R});
-  size_t o_bih1 = copy("rnn1.bias_ih_l0", {3 * R}), o_bhh1 = copy("rnn1.bias_hh_l0", {3 * R});
-  size_t o_ih2 = copy("rnn2.weight_ih_l0", {3 * R, R + AUX}), o_hh2 = copy("rnn2.weight_hh_l0", {3 * R, R});
-  size_t o_bih2 = copy("rnn2.bias_ih_l0", {3 * R}), o_bhh2 = copy("rnn2.bias_hh_l0", {3 * R});
-  size_t o_fc1 = copy("fc1.weight", {F, R + AUX}), o_fc1b = copy("fc1.bias", {F});
-  size_t o_fc2 = copy("fc2.weight", {F, F + AUX}), o_fc2b = copy("fc2.bias", {F});
+  size_t oIb = pk.copy(tm, "I.bias", {R});
+  size_t o_ih1 = pk.copy(tm, "rnn1.weight_ih_l0", {3 * R, R}), o_hh1 = pk.copy(tm, "rnn1.weight_hh_l0", {3 * R, R});
+  size_t o_bih1 = pk.copy(tm, "rnn1.bias_ih_l0", {3 * R}), o_bhh1 = pk.copy(tm, "rnn1.bias_hh_l0", {3 * R});
+  size_t o_ih2 = pk.copy(tm, "rnn2.weight_ih_l0", {3 * R, R + AUX}), o_hh2 = pk.copy(tm, "rnn2.weight_hh_l0", {3 * R, R});
+  size_t o_bih2 = pk.copy(tm, "rnn2.bias_ih_l0", {3 * R}), o_bhh2 = pk.copy(tm, "rnn2.bias_hh_l0", {3 * R});
+  size_t o_fc1 = pk.copy(tm, "fc1.weight", {F, R + AUX}), o_fc1b = pk.copy(tm, "fc1.bias", {F});
+  size_t o_fc2 = pk.copy(tm, "fc2.weight", {F, F + AUX}), o_fc2b = pk.copy(tm, "fc2.bias", {F});
   size_t o_fc3, o_fc3b;
   if (ctx->mol) {               // 30 rows padded with zero rows to NC = 32: the step kernels dot whole quads of rows
     const float* w = need(tm, "fc3.weight", {kMolParams, F})->data;
@@ -155,8 +147,8 @@ static StepWeights pack_original(b200tts_wavernn* ctx, const TensorMap& tm, Pack
     std::memcpy(&pk.h[o_fc3], w, sizeof(float) * kMolParams * F);
     std::memcpy(&pk.h[o_fc3b], b, sizeof(float) * kMolParams);
   } else {
-    o_fc3 = copy("fc3.weight", {NC, F});
-    o_fc3b = copy("fc3.bias", {NC});
+    o_fc3 = pk.copy(tm, "fc3.weight", {NC, F});
+    o_fc3b = pk.copy(tm, "fc3.bias", {NC});
   }
 
   // ---- MelResNet, transposed to [in][out]; BatchNorm (eval, eps 1e-5) folded to scale/shift in double ----
@@ -195,7 +187,7 @@ static StepWeights pack_original(b200tts_wavernn* ctx, const TensorMap& tm, Pack
   size_t o_cout = pk.add((size_t)C * O);
   for (int o = 0; o < O; ++o)
     for (int ci = 0; ci < C; ++ci) pk.h[o_cout + (size_t)ci * O + o] = cow[(size_t)o * C + ci];
-  size_t o_coutb = copy("upsample.resnet.conv_out.bias", {O});
+  size_t o_coutb = pk.copy(tm, "upsample.resnet.conv_out.bias", {O});
 
   // ---- composite FIR ----
   std::vector<std::vector<double>> taps(c.n_upsample);

@@ -198,6 +198,33 @@ def _host(x):
     return x.cpu().numpy() if hasattr(x, 'cpu') else np.asarray(x)
 
 
+def _session_rows(engine, max_rows, chunk_steps):
+    """Checks a streaming service's rows and chunk against its vocoder engine; True: the sessions run on the tensor cores."""
+    cap = int(getattr(engine, 'max_session_rows', 32))
+    if not 1 <= int(max_rows) <= cap:
+        raise ValueError(f'max_rows must be 1..{cap} (the most sessions one launch of this engine takes)')
+    if int(chunk_steps) < 1:
+        raise ValueError('chunk_steps must be >= 1')
+    tc = int(max_rows) > 32                  # the push kernel runs at most 32 sessions per launch
+    if tc and int(chunk_steps) % int(engine.hop):
+        raise ValueError(f'above 32 rows the sessions run on the tensor cores: chunk_steps must be a multiple of hop ({engine.hop})')
+    return tc
+
+
+def _advance(engine, active, chunk_steps):
+    """One launch over the (key, session) pairs `active` -> ([(key, wave piece, finished)], the pairs still active)."""
+    pieces = engine.advance([s for _, s in active], chunk_steps)
+    out, still = [], []
+    for (key, s), (_labels, wave) in zip(active, pieces):
+        finished = s.done
+        out.append((key, _host(wave), finished))
+        if finished:
+            s.close()
+        else:
+            still.append((key, s))
+    return out, still
+
+
 class StreamingVocoder:
     """Continuous batching of vocoder sessions on one engine.  `submit` queues requests; every `step` admits queued requests
     first come first served into free rows (at most `max_rows` sessions per launch), advances every session by up to
@@ -209,16 +236,9 @@ class StreamingVocoder:
     `chunk_steps` must be a multiple of the engine's hop."""
 
     def __init__(self, engine, seed=0, chunk_steps=2750, max_rows=32):
-        cap = int(getattr(engine, 'max_session_rows', 32))
-        if not 1 <= int(max_rows) <= cap:
-            raise ValueError(f'max_rows must be 1..{cap} (the most sessions one launch of this engine takes)')
-        if int(chunk_steps) < 1:
-            raise ValueError('chunk_steps must be >= 1')
+        self._tc = _session_rows(engine, max_rows, chunk_steps)
         self.engine, self.seed = engine, int(seed)
         self.chunk_steps, self.max_rows = int(chunk_steps), int(max_rows)
-        self._tc = self.max_rows > 32                       # the push kernel runs at most 32 sessions per launch
-        if self._tc and self.chunk_steps % int(engine.hop):
-            raise ValueError(f'above 32 rows the sessions run on the tensor cores: chunk_steps must be a multiple of hop ({engine.hop})')
         self._queue = collections.deque()       # (key, mel [T, feat], utterance id)
         self._active = []                       # (key, session) in admission order
 
@@ -250,16 +270,7 @@ class StreamingVocoder:
             self._active.append((key, self.engine.open_session(padded, seed=self.seed, utterance_id=uid, **kw)))
         if not self._active:
             return []
-        pieces = self.engine.advance([s for _, s in self._active], self.chunk_steps)
-        out, still = [], []
-        for (key, s), (_labels, wave) in zip(self._active, pieces):
-            finished = s.done
-            out.append((key, _host(wave), finished))
-            if finished:
-                s.close()
-            else:
-                still.append((key, s))
-        self._active = still
+        out, self._active = _advance(self.engine, self._active, self.chunk_steps)
         check = getattr(self.engine, 'check', None)
         if check is not None:
             check()                              # a timed-out run raises here instead of handing out NaN audio
@@ -294,11 +305,7 @@ class StreamingSynthesizer:
     single-sentence kernel."""
 
     def __init__(self, synth, engine, seed=0, chunk_steps=2750, max_rows=32, max_admit=None, decode_steps=None):
-        cap = int(getattr(engine, 'max_session_rows', 32))
-        if not 1 <= int(max_rows) <= cap:
-            raise ValueError(f'max_rows must be 1..{cap} (the most sessions one launch of this engine takes)')
-        if int(chunk_steps) < 1:
-            raise ValueError('chunk_steps must be >= 1')
+        self._tc = _session_rows(engine, max_rows, chunk_steps)
         if max_admit is not None and int(max_admit) < 1:
             raise ValueError('max_admit must be >= 1 (or None: as many as there are free rows)')
         self.synth, self.engine, self.seed = synth, engine, int(seed)
@@ -308,9 +315,6 @@ class StreamingSynthesizer:
             raise ValueError('decode_steps must be >= 1 (or None: the whole decode at admission)')
         self.decode_steps = None if decode_steps is None else int(decode_steps)
         self._decoding = []                     # (key, utterance id, decoder session) in admission order
-        self._tc = self.max_rows > 32                       # the push kernel runs at most 32 sessions per launch
-        if self._tc and self.chunk_steps % int(engine.hop):
-            raise ValueError(f'above 32 rows the sessions run on the tensor cores: chunk_steps must be a multiple of hop ({engine.hop})')
         self._queue = collections.deque()       # (key, text, utterance id, speaking-rate bias)
         self._active = []                       # (key, session) in admission order
         self._mels = {}                         # key -> (postnet output of its batch, row, frames)
@@ -411,17 +415,9 @@ class StreamingSynthesizer:
         for key in self._gone:
             self._mels.pop(key, None)
         empty = self._admit() if self.decode_steps is None else self._decode_slice()
-        out, still = [], []
+        out = []
         if self._active:
-            pieces = self.engine.advance([s for _, s in self._active], self.chunk_steps)
-            for (key, s), (_labels, wave) in zip(self._active, pieces):
-                finished = s.done
-                out.append((key, _host(wave), finished))
-                if finished:
-                    s.close()
-                else:
-                    still.append((key, s))
-        self._active = still
+            out, self._active = _advance(self.engine, self._active, self.chunk_steps)
         out += empty
         self._gone = [key for key, _piece, finished in out if finished]
         check = getattr(self.engine, 'check', None)

@@ -79,6 +79,36 @@ class TacoDecoderEngine:
     def _stream(self):
         return C.c_void_p(torch.cuda.current_stream(self.device).cuda_stream)
 
+    def _memory(self, memory, rows='B'):
+        """An encoder output [rows, Tx, enc_dim] -> contiguous float32 on this engine's device."""
+        m = torch.as_tensor(memory).to(device=self._dev(), dtype=torch.float32).contiguous()
+        if m.dim() != 3 or m.shape[2] != self.cfg['enc_dim']:
+            raise ValueError(f'memory must be [{rows}, Tx, {self.cfg["enc_dim"]}]')
+        return m
+
+    @staticmethod
+    def _lengths(lengths, B, Tx):
+        """Sentence lengths [B] in [1, Tx], or None (= Tx) -> int32 tensor."""
+        ln = torch.full((B,), Tx, dtype=torch.int32) if lengths is None else torch.as_tensor(lengths, dtype=torch.int32)
+        if tuple(ln.shape) != (B,) or B < 1 or int(ln.max()) > Tx or int(ln.min()) < 1:
+            raise ValueError('lengths must be [B] in [1, Tx]')
+        return ln
+
+    def _dropout(self, seed, utterance_offset, masks, B, steps):
+        """The prenet-dropout descriptor: PHILOX keyed by (seed, utterance_offset + b), or EXT when `masks`, uint8 keep flags
+        [B, steps, 2, prenet_units], are given.  Returns (descriptor, the masks on the device or None)."""
+        d = TacoDropout()
+        d.seed = int(seed) & 0xFFFFFFFFFFFFFFFF
+        d.utterance_offset = int(utterance_offset)
+        if masks is None:
+            return d, None
+        md = torch.as_tensor(masks).to(device=self._dev(), dtype=torch.uint8).contiguous()
+        if tuple(md.shape) != (B, steps, 2, self.cfg['prenet_units']):
+            raise ValueError(f'masks must be [{B}, {steps}, 2, {self.cfg["prenet_units"]}]')
+        d.mode = 1
+        d.d_masks = md.data_ptr()
+        return d, md
+
     def decode(self, memory, lengths=None, *, masks=None, seed=0, utterance_offset=0, max_steps=2000, window=False,
                want_align=True, forced_states=None, mu_bias=None):
         """memory [B, Tx, enc_dim] (tensor/ndarray); lengths [B] or None (= Tx).  masks: optional uint8 keep flags
@@ -89,30 +119,16 @@ class TacoDecoderEngine:
         mu_bias: speaking-rate bias, a scalar or one per sentence, each finite in [-1, 1] (b200tts_taco_decode_biased: the
         forward-attention speed bias of attention.py:163-165; positive is faster).  None or all zeros: the unbiased decoder."""
         dev = self._dev()
-        m = torch.as_tensor(memory).to(device=dev, dtype=torch.float32).contiguous()
-        if m.dim() != 3 or m.shape[2] != self.cfg['enc_dim']:
-            raise ValueError(f'memory must be [B, Tx, {self.cfg["enc_dim"]}]')
+        m = self._memory(memory)
         B, Tx, _ = m.shape
         bias = mu_bias_array(mu_bias, B)
-        ln = torch.full((B,), Tx, dtype=torch.int32) if lengths is None else torch.as_tensor(lengths, dtype=torch.int32)
-        if int(ln.max()) > Tx or int(ln.min()) < 1:
-            raise ValueError('lengths must be in [1, Tx]')
-        ln = ln.to(dev)
+        ln = self._lengths(lengths, B, Tx).to(dev)
         with torch.cuda.device(self.device):
             frames = torch.zeros(B, max_steps, self.cfg['num_mels'], device=dev, dtype=torch.float32)
             stop = torch.zeros(B, max_steps, device=dev, dtype=torch.float32)
             align = torch.zeros(B, max_steps, Tx, device=dev, dtype=torch.float32) if want_align else None
             nsteps = torch.zeros(B, device=dev, dtype=torch.int32)
-            d = TacoDropout()
-            d.seed = int(seed) & 0xFFFFFFFFFFFFFFFF
-            d.utterance_offset = int(utterance_offset)
-            md = None
-            if masks is not None:
-                md = torch.as_tensor(masks).to(device=dev, dtype=torch.uint8).contiguous()
-                if tuple(md.shape) != (B, max_steps, 2, self.cfg['prenet_units']):
-                    raise ValueError('masks must be [B, max_steps, 2, prenet_units]')
-                d.mode = 1
-                d.d_masks = md.data_ptr()
+            d, md = self._dropout(seed, utterance_offset, masks, B, max_steps)
             fs = None
             if forced_states is not None:
                 fs = torch.as_tensor(forced_states).to(device=dev, dtype=torch.float32).contiguous()
@@ -144,35 +160,21 @@ class TacoDecoderEngine:
         [B, Ty_max, 80] raw decoder outputs, align [B, Ty_max, Tx] or None, nsteps [B] int32) as CUDA tensors; rows at or
         beyond nsteps are zero."""
         dev = self._dev()
-        m = torch.as_tensor(memory).to(device=dev, dtype=torch.float32).contiguous()
-        if m.dim() != 3 or m.shape[2] != self.cfg['enc_dim']:
-            raise ValueError(f'memory must be [B, Tx, {self.cfg["enc_dim"]}]')
+        m = self._memory(memory)
         B, Tx, _ = m.shape
         tg = torch.as_tensor(targets).to(device=dev, dtype=torch.float32).contiguous()
         if tg.dim() != 3 or tg.shape[0] != B or tg.shape[2] != self.cfg['num_mels'] or tg.shape[1] < 1:
             raise ValueError(f'targets must be [{B}, Ty_max >= 1, {self.cfg["num_mels"]}]')
         Ty = tg.shape[1]
-        ln = torch.full((B,), Tx, dtype=torch.int32) if lengths is None else torch.as_tensor(lengths, dtype=torch.int32)
-        if tuple(ln.shape) != (B,) or int(ln.max()) > Tx or int(ln.min()) < 1:
-            raise ValueError('lengths must be [B] in [1, Tx]')
+        ln = self._lengths(lengths, B, Tx).to(dev)
         tl = torch.full((B,), Ty, dtype=torch.int32) if target_lengths is None else torch.as_tensor(target_lengths, dtype=torch.int32)
         if tuple(tl.shape) != (B,):
             raise ValueError('target_lengths must be [B]')
-        tl = tl.clamp(0, Ty)
-        ln, tl = ln.to(dev), tl.to(dev)
+        tl = tl.clamp(0, Ty).to(dev)
         with torch.cuda.device(self.device):
             frames = torch.zeros(B, Ty, self.cfg['num_mels'], device=dev, dtype=torch.float32)
             align = torch.zeros(B, Ty, Tx, device=dev, dtype=torch.float32) if want_align else None
-            d = TacoDropout()
-            d.seed = int(seed) & 0xFFFFFFFFFFFFFFFF
-            d.utterance_offset = int(utterance_offset)
-            md = None
-            if masks is not None:
-                md = torch.as_tensor(masks).to(device=dev, dtype=torch.uint8).contiguous()
-                if tuple(md.shape) != (B, Ty, 2, self.cfg['prenet_units']):
-                    raise ValueError('masks must be [B, Ty_max, 2, prenet_units]')
-                d.mode = 1
-                d.d_masks = md.data_ptr()
+            d, md = self._dropout(seed, utterance_offset, masks, B, Ty)
             _lib.check(self.lib.b200tts_taco_decode_gta(self._h, _ptr(m), _ptr(ln), B, Tx, C.byref(d), _ptr(tg), _ptr(tl), Ty,
                                                         _ptr(frames), _ptr(align), self._stream()))
             for t in (m, ln, tg, tl, md):
@@ -186,18 +188,14 @@ class TacoDecoderEngine:
         one per row, as in `decode`.  The memory is copied and its keys computed here, on the current stream; every session
         starts at step 0.  However `advance_decodes` cuts them, a session's frames, stop values and step count are bit for bit
         those `decode` gives its row at B >= 2 (one thread block per sentence) with utterance_offset = its id."""
-        dev = self._dev()
-        m = torch.as_tensor(memory).to(device=dev, dtype=torch.float32).contiguous()
-        if m.dim() != 3 or m.shape[2] != self.cfg['enc_dim']:
-            raise ValueError(f'memory must be [n, Tx, {self.cfg["enc_dim"]}]')
+        m = self._memory(memory, 'n')
         n, Tx, _ = m.shape
-        ln = np.full(n, Tx, dtype=np.int32) if lengths is None else np.ascontiguousarray(np.asarray(lengths).reshape(-1), dtype=np.int32)
+        ln = np.ascontiguousarray(self._lengths(lengths, n, Tx).cpu().numpy())
         uid = np.ascontiguousarray([int(i) & 0xFFFFFFFFFFFFFFFF for i in ids], dtype=np.uint64)
-        if len(ln) != n or len(uid) != n:
-            raise ValueError(f'need one length and one id per row ({n} rows)')
+        if len(uid) != n:
+            raise ValueError(f'need one id per row ({n} rows)')
         bias = mu_bias_array(mu_bias, n)
-        d = TacoDropout()
-        d.seed = int(seed) & 0xFFFFFFFFFFFFFFFF
+        d, _ = self._dropout(seed, 0, None, n, max_steps)
         handles = (C.c_void_p * max(n, 1))()
         with torch.cuda.device(self.device):
             _lib.check(self.lib.b200tts_taco_session_open_batch(
@@ -265,9 +263,7 @@ class TacoDecoderEngine:
         if i.dim() != 2:
             raise ValueError('ids must be [B, Tx]')
         B, Tx = i.shape
-        ln = torch.full((B,), Tx, dtype=torch.int32) if lengths is None else torch.as_tensor(lengths, dtype=torch.int32)
-        if tuple(ln.shape) != (B,) or B < 1 or int(ln.max()) > Tx or int(ln.min()) < 1:
-            raise ValueError('lengths must be [B] in [1, Tx]')
+        ln = self._lengths(lengths, B, Tx)
         if self.vocab is not None:                 # (without the encoder variables the library refuses the call itself)
             valid = torch.arange(Tx, device=i.device)[None, :] < ln.to(i.device)[:, None]
             if bool(((i < 0) | (i >= self.vocab))[valid].any()):

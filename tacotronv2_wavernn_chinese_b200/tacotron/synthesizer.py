@@ -58,19 +58,22 @@ class Synthesizer:
         self.engine = TacoDecoderEngine(w, device=device)
         return self
 
+    def _encode(self, texts):
+        """Pinyin strings -> (encoder output [B, Tx, enc_dim] CUDA tensor, lengths [B] int32 numpy), Tx the longest."""
+        seqs = [self.symbols.text_to_sequence(t) for t in texts]
+        lengths = np.array([len(s) for s in seqs], dtype=np.int32)
+        ids = np.zeros((len(seqs), int(lengths.max())), dtype=np.int32)
+        for b, s in enumerate(seqs):
+            ids[b, :len(s)] = s
+        return self.engine.encode(ids, lengths), lengths
+
     def mels(self, texts, seed=0, window=False, max_iters=None, utterance_offset=0, mu_bias=None):
         """Batch of pinyin strings -> (list of np.float32 mel [T_b, 80] scaled to [0,1] like the .npy the reference saves,
         dict with device tensors).  Each sentence decodes until its own stop token (reference graph is batch 1).
         mu_bias: speaking-rate bias, a scalar or one per text (TacoDecoderEngine.decode; positive speaks faster)."""
         mu_bias = mu_bias_array(mu_bias, len(texts))
-        seqs = [self.symbols.text_to_sequence(t) for t in texts]
-        B, Tx = len(seqs), max(len(s) for s in seqs)
-        ids = np.zeros((B, Tx), dtype=np.int32)
-        for b, s in enumerate(seqs):
-            ids[b, :len(s)] = s
-        lengths = np.array([len(s) for s in seqs], dtype=np.int32)
+        mem, lengths = self._encode(texts)
         eng = self.engine
-        mem = eng.encode(ids, lengths)
         ms = int(max_iters or self.max_iters)
         # the prenet-dropout Philox stream is keyed by the GLOBAL sentence index: a sentence's mel must not depend on
         # how the batch is sharded over ranks
@@ -83,7 +86,7 @@ class Synthesizer:
         stop = dec['stop'].cpu().numpy()
         mel_h = mel.cpu().numpy()
         out = []
-        for b in range(B):
+        for b in range(len(texts)):
             rounded = np.round(stop[b, :n[b]])
             target = int(np.argmax(rounded == 1)) if (rounded == 1).any() else int(n[b])       # :104-105
             out.append(unit_mel(mel_h[b, :target]))
@@ -95,18 +98,12 @@ class Synthesizer:
         dropout of sentence b is keyed by ids[b], an arbitrary global id, so a sentence's mel does not depend on which others
         share its batch.  Consecutive ids draw the PHILOX stream directly; otherwise each run of consecutive ids gets its keep
         flags from philox_masks, which by its contract equal that stream.  mu_bias: as in `mels`."""
-        seqs = [self.symbols.text_to_sequence(t) for t in texts]
         ids = [int(i) for i in ids]
-        if len(ids) != len(seqs) or not seqs:
+        if len(ids) != len(texts) or not texts:
             raise ValueError('need one id per text, and at least one text')
-        mu_bias = mu_bias_array(mu_bias, len(seqs))
-        B, Tx = len(seqs), max(len(s) for s in seqs)
-        tok = np.zeros((B, Tx), dtype=np.int32)
-        for b, s in enumerate(seqs):
-            tok[b, :len(s)] = s
-        lengths = np.array([len(s) for s in seqs], dtype=np.int32)
+        mu_bias = mu_bias_array(mu_bias, len(texts))
+        mem, lengths = self._encode(texts)
         eng = self.engine
-        mem = eng.encode(tok, lengths)
         ms = int(max_iters or self.max_iters)
         runs = [[ids[0], 1]]
         for i in ids[1:]:
@@ -128,15 +125,9 @@ class Synthesizer:
         to be advanced in slices with `engine.advance_decodes` and finished with `finish_decodes`.  Text b's prenet dropout is keyed
         by (seed, ids[b]) and its frames are bit for bit those of the batch decoder (`taco_decoder_kernel`) on this encoder output.
         A lone text therefore differs in bits from `decode_device`, which decodes a batch of one on the single-sentence kernel."""
-        seqs = [self.symbols.text_to_sequence(t) for t in texts]
-        if len(ids) != len(seqs) or not seqs:
+        if len(ids) != len(texts) or not texts:
             raise ValueError('need one id per text, and at least one text')
-        B, Tx = len(seqs), max(len(s) for s in seqs)
-        tok = np.zeros((B, Tx), dtype=np.int32)
-        for b, s in enumerate(seqs):
-            tok[b, :len(s)] = s
-        lengths = np.array([len(s) for s in seqs], dtype=np.int32)
-        mem = self.engine.encode(tok, lengths)
+        mem, lengths = self._encode(texts)
         return self.engine.open_decode_sessions(mem, lengths, ids, seed=seed, max_steps=int(max_iters or self.max_iters), window=window,
                                                 mu_bias=mu_bias)
 
@@ -168,28 +159,19 @@ class Synthesizer:
         keyed by (seed, utterance_offset + b, step, unit): a sentence's mel does not depend on the batch it is decoded in."""
         if len(texts) != len(targets) or not texts:
             raise ValueError('need one target mel per text, and at least one text')
-        seqs = [self.symbols.text_to_sequence(t) for t in texts]
         tg = [np.clip(np.asarray(t, dtype=np.float32), -MAX_ABS_VALUE, MAX_ABS_VALUE) for t in targets]
         for t in tg:
             if t.ndim != 2 or t.shape[1] != 80 or t.shape[0] < 1:
                 raise ValueError(f'target mels must be [T >= 1, 80], got {t.shape}')
-        B, Tx, Ty = len(seqs), max(len(s) for s in seqs), max(t.shape[0] for t in tg)
-        ids = np.zeros((B, Tx), dtype=np.int32)
-        tpad = np.zeros((B, Ty, 80), dtype=np.float32)
-        for b, (s, t) in enumerate(zip(seqs, tg)):
-            ids[b, :len(s)] = s
-            tpad[b, :t.shape[0]] = t
-        lengths = np.array([len(s) for s in seqs], dtype=np.int32)
         tlen = np.array([t.shape[0] for t in tg], dtype=np.int32)
+        tpad = np.zeros((len(tg), int(tlen.max()), 80), dtype=np.float32)
+        for b, t in enumerate(tg):
+            tpad[b, :t.shape[0]] = t
+        mem, lengths = self._encode(texts)
         eng = self.engine
-        mem = eng.encode(ids, lengths)
         dec = eng.decode_gta(mem, lengths, tpad, tlen, seed=seed, utterance_offset=utterance_offset)
         mel_h = eng.postnet(dec['frames'], dec['nsteps']).cpu().numpy()
-        out = []
-        for b in range(B):
-            m = np.clip(mel_h[b, :tlen[b]], -MAX_ABS_VALUE, MAX_ABS_VALUE)
-            out.append(np.clip((m + MAX_ABS_VALUE) / (2 * MAX_ABS_VALUE), 0, 1).astype(np.float32))
-        return out
+        return [unit_mel(mel_h[b, :tlen[b]]) for b in range(len(tg))]
 
     def synthesize_gta(self, text, mel_path, out_dir, idx, seed=0, utterance_offset=0):
         """wavernn_preprocess.py:72-120 `Synthesizer.synthesize(text, mel, out_dir, idx)`: Hanzi text (through get_pyin, :85),
