@@ -175,12 +175,14 @@ int b200tts_wavernn_fold_geometry(int T, int hop, int target, int overlap, int* 
 int b200tts_wavernn_generate_host(b200tts_wavernn* ctx, const float* h_mel, int B, int T, const b200tts_rng* rng,
                                   const b200tts_gen_opts* opts, int16_t* h_labels, double* h_wave);
 
-/* The Exp(1) noise the PHILOX mode uses for (utterance, step, class): d_q[n_steps][B][n_classes].
+/* The Exp(1) noise the PHILOX mode uses for (utterance, step, class): d_q[n_steps][B][n_classes], steps step0 ..
+ * step0 + n_steps - 1 with step0 >= 0 and step0 + n_steps <= 2^31 - 1 (else B200TTS_EINVAL, before any CUDA call).
  * Lets a test hand the production noise stream to the oracle. */
 int b200tts_philox_exponential(int device, uint64_t seed, uint64_t utterance_offset, int B, int step0, int n_steps,
                                int n_classes, float* d_q, void* stream);
 
-/* The uniforms the PHILOX mode of b200tts_wavernn_generate_mol draws for (utterance, step): d_u[n_steps][B][11]. */
+/* The uniforms the PHILOX mode of b200tts_wavernn_generate_mol draws for (utterance, step): d_u[n_steps][B][11], steps as
+ * b200tts_philox_exponential takes them. */
 int b200tts_philox_mol_uniform(int device, uint64_t seed, uint64_t utterance_offset, int B, int step0, int n_steps, float* d_u,
                                void* stream);
 
@@ -377,7 +379,8 @@ int b200tts_taco_session_run(b200tts_taco* ctx, b200tts_taco_session* const* s, 
 int b200tts_taco_session_outputs(b200tts_taco_session* const* s, int n, int T_max, float* d_frames, float* d_stop,
                                  int32_t* d_nsteps, void* stream);
 
-/* The keep flags the PHILOX dropout mode draws: d_masks [B][steps][2][prenet_units]. */
+/* The keep flags the PHILOX dropout mode draws: d_masks [B][steps][2][prenet_units], prenet_units a multiple of 4 as
+ * b200tts_taco_create requires. */
 int b200tts_taco_philox_masks(int device, uint64_t seed, uint64_t utterance_offset, int B, int steps, int prenet_units,
                               uint8_t* d_masks, void* stream);
 

@@ -20,8 +20,12 @@ struct Error : std::runtime_error {
   } while (0)
 
 // ---------------------------------------------------------------------------------------------
-// Philox4x32-10 (Salmon et al. 2011).  counter = (step, class/4, utt_lo, utt_hi), key = seed.
-// One call yields the noise of 4 consecutive classes of one (utterance, step).
+// Philox4x32-10 (Salmon et al. 2011), key = seed, counter = (word 0, word 1, utt_lo, utt_hi).  Every stream keyed by the same
+// (seed, utterance id) owns its own range of word 1, so no two streams ever read the same counter:
+//   WaveRNN RAW noise     (step,  class/4)                              [0, 2^13)   one call = 4 consecutive classes
+//   WaveRNN MOL uniforms  (step,  j = 0..2)                             [0, 3)      a model is RAW or MOL, never both
+//   Tacotron keep flags   (step,  0x40000000 | layer*P/4 + unit/4)      [2^30, 2^31)
+//   Griffin-Lim phase     (frame, 0x80000000 | bin/4)                   [2^31, 2^32)
 // ---------------------------------------------------------------------------------------------
 __host__ __device__ __forceinline__ void philox_round(uint32_t (&c)[4], uint32_t k0, uint32_t k1) {
   const uint32_t M0 = 0xD2511F53u, M1 = 0xCD9E8D57u;
@@ -58,6 +62,14 @@ __device__ __forceinline__ void philox_exp4(uint64_t seed, uint64_t utt, uint32_
   philox4x32_10(c, seed);
 #pragma unroll
   for (int i = 0; i < 4; ++i) q[i] = exp1_from_bits(c[i]);
+}
+
+// Tacotron prenet dropout (rate 0.5, always on): keep flag of unit `unit` of prenet layer `layer` (0 or 1, P units each) at
+// decoder step `step` of utterance `utt`.  The one place the flags' counter is decided: the decoders and the masks dump call it.
+__device__ __forceinline__ bool taco_keep_flag(uint64_t seed, uint64_t utt, int step, int layer, int unit, int P) {
+  uint32_t c[4] = {(uint32_t)step, 0x40000000u | (uint32_t)(layer * (P >> 2) + (unit >> 2)), (uint32_t)utt, (uint32_t)(utt >> 32)};
+  philox4x32_10(c, seed);
+  return (c[unit & 3] >> 31) != 0;
 }
 
 // ---------------------------------------------------------------------------------------------

@@ -41,8 +41,9 @@ __device__ __forceinline__ int gl_row_frames(const int* frames, int b, int Tmax)
   return T < 0 ? 0 : (T > Tmax ? Tmax : T);
 }
 
-// Uniform in [0,1) for (utterance, frame, bin); counter word 1 carries a tag bit so the stream is disjoint from the WaveRNN
-// sampling noise keyed with the same seed.  Shared by the frame kernel and b200tts_gl_philox_uniform (bit-identical dumps).
+// Uniform in [0,1) for (utterance, frame, bin); counter word 1 carries a tag bit so the stream is disjoint from the other
+// streams keyed with the same seed (the map is in common.cuh).  Shared by the frame kernel and b200tts_gl_philox_uniform
+// (bit-identical dumps).
 __device__ __forceinline__ float gl_philox_uniform(uint64_t seed, uint64_t utt, uint32_t frame, uint32_t bin) {
   uint32_t c[4] = {frame, 0x80000000u | (bin >> 2), (uint32_t)utt, (uint32_t)(utt >> 32)};
   philox4x32_10(c, seed);

@@ -40,9 +40,7 @@ __global__ void taco_philox_masks_kernel(unsigned long long seed, unsigned long 
     r /= 2;
     int step = (int)(r % steps);
     int b = (int)(r / steps);
-    uint32_t c[4] = {(uint32_t)step, (uint32_t)(layer * (P >> 2) + (j >> 2)), (uint32_t)(utt0 + b), (uint32_t)((utt0 + b) >> 32)};
-    philox4x32_10(c, seed);
-    masks[e] = (unsigned char)(c[j & 3] >> 31);
+    masks[e] = taco_keep_flag(seed, utt0 + b, step, layer, j, P) ? 1 : 0;
   }
 }
 

@@ -256,9 +256,7 @@ __device__ __forceinline__ void taco_decoder_run(const TacoWeights& W, const Tac
     for (int j = tid; j < P; j += kTacoThreads) {
       float keep;
       if (A.rng_mode == 0) {
-        uint32_t c[4] = {(uint32_t)step, (uint32_t)(j >> 2), (uint32_t)(A.utt_offset + b), (uint32_t)((A.utt_offset + b) >> 32)};
-        philox4x32_10(c, A.seed);
-        keep = (c[j & 3] >> 31) ? 1.f : 0.f;
+        keep = taco_keep_flag(A.seed, A.utt_offset + b, step, 0, j, P) ? 1.f : 0.f;
       } else {
         keep = A.masks[(((size_t)b * A.max_steps + step) * 2 + 0) * P + j] ? 1.f : 0.f;
       }
@@ -269,9 +267,7 @@ __device__ __forceinline__ void taco_decoder_run(const TacoWeights& W, const Tac
     for (int j = tid; j < P; j += kTacoThreads) {
       float keep;
       if (A.rng_mode == 0) {
-        uint32_t c[4] = {(uint32_t)step, (uint32_t)((P >> 2) + (j >> 2)), (uint32_t)(A.utt_offset + b), (uint32_t)((A.utt_offset + b) >> 32)};
-        philox4x32_10(c, A.seed);
-        keep = (c[j & 3] >> 31) ? 1.f : 0.f;
+        keep = taco_keep_flag(A.seed, A.utt_offset + b, step, 1, j, P) ? 1.f : 0.f;
       } else {
         keep = A.masks[(((size_t)b * A.max_steps + step) * 2 + 1) * P + j] ? 1.f : 0.f;
       }

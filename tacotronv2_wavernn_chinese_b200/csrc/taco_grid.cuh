@@ -234,9 +234,7 @@ __device__ __forceinline__ void taco_grid_run(const TacoGridModel& Md, const Tac
       const int j = 2 * c + tid;
       float keep;
       if (A.rng_mode == 0) {
-        uint32_t cc[4] = {(uint32_t)step, (uint32_t)(j >> 2), (uint32_t)A.utt, (uint32_t)(A.utt >> 32)};
-        philox4x32_10(cc, A.seed);
-        keep = (cc[j & 3] >> 31) ? 1.f : 0.f;
+        keep = taco_keep_flag(A.seed, A.utt, step, 0, j, P) ? 1.f : 0.f;
       } else {
         keep = A.masks[((size_t)step * 2 + 0) * P + j] ? 1.f : 0.f;
       }
@@ -260,9 +258,7 @@ __device__ __forceinline__ void taco_grid_run(const TacoGridModel& Md, const Tac
       const int j = 2 * c + tid;
       float keep;
       if (A.rng_mode == 0) {
-        uint32_t cc[4] = {(uint32_t)step, (uint32_t)((P >> 2) + (j >> 2)), (uint32_t)A.utt, (uint32_t)(A.utt >> 32)};
-        philox4x32_10(cc, A.seed);
-        keep = (cc[j & 3] >> 31) ? 1.f : 0.f;
+        keep = taco_keep_flag(A.seed, A.utt, step, 1, j, P) ? 1.f : 0.f;
       } else {
         keep = A.masks[((size_t)step * 2 + 1) * P + j] ? 1.f : 0.f;
       }

@@ -373,7 +373,7 @@ extern "C" int b200tts_taco_decode_gta(b200tts_taco* ctx, const float* d_memory,
 extern "C" int b200tts_taco_philox_masks(int device, uint64_t seed, uint64_t utterance_offset, int B, int steps, int prenet_units,
                                          uint8_t* d_masks, void* stream) {
   API_BEGIN
-  REQUIRE(d_masks && B >= 1 && steps >= 1 && prenet_units >= 4, B200TTS_EINVAL, "bad argument");
+  REQUIRE(d_masks && B >= 1 && steps >= 1 && prenet_units >= 4 && prenet_units % 4 == 0, B200TTS_EINVAL, "bad argument");
   DeviceGuard dg(device);
   size_t total = (size_t)B * steps * 2 * prenet_units;
   unsigned grid = (unsigned)std::min<size_t>((total + 255) / 256, 132 * 16);

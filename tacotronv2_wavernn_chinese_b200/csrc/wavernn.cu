@@ -1293,6 +1293,7 @@ extern "C" int b200tts_philox_exponential(int device, uint64_t seed, uint64_t ut
                                           int n_classes, float* d_q, void* stream) {
   API_BEGIN
   REQUIRE(d_q && B >= 1 && n_steps >= 1 && n_classes >= 4 && n_classes % 4 == 0 && step0 >= 0, B200TTS_EINVAL, "bad argument");
+  REQUIRE(n_steps <= INT_MAX - step0, B200TTS_EINVAL, "step0 + n_steps must not exceed 2^31 - 1");
   DeviceGuard dg(device);
   size_t total = (size_t)n_steps * B * (n_classes / 4);
   unsigned grid = (unsigned)std::min<size_t>((total + 255) / 256, 132 * 16);
@@ -1317,6 +1318,7 @@ extern "C" int b200tts_philox_mol_uniform(int device, uint64_t seed, uint64_t ut
                                           float* d_u, void* stream) {
   API_BEGIN
   REQUIRE(d_u && B >= 1 && n_steps >= 1 && step0 >= 0, B200TTS_EINVAL, "bad argument");
+  REQUIRE(n_steps <= INT_MAX - step0, B200TTS_EINVAL, "step0 + n_steps must not exceed 2^31 - 1");
   DeviceGuard dg(device);
   const size_t total = (size_t)n_steps * B;
   unsigned grid = (unsigned)std::min<size_t>((total + 255) / 256, 132 * 16);

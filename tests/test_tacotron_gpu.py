@@ -161,6 +161,25 @@ def test_philox_dropout_replay_and_batch_invariance():
     assert np.array_equal(pair['frames'].cpu().numpy()[0], a['frames'].cpu().numpy()[2])
 
 
+# (utterance_offset, window, mu_bias): ids across 2^32, the inference window, and both signs of a speaking-rate bias
+@pytest.mark.parametrize('offset,window,mu_bias', [(2 ** 32 - 3, False, None), (10, True, None), (10, False, 0.3),
+                                                   (10, False, -0.3)])
+def test_philox_dropout_every_decoder_kernel_draws_the_dumped_flags(offset, window, mu_bias):
+    """In Philox mode the batch kernel and the single-sentence grid kernel (their biased forms with a rate bias) draw, bit for
+    bit, what their EXT mode draws when fed b200tts_taco_philox_masks' dump of the same seed and ids."""
+    w = synth_taco_weights(7)
+    eng = _engine(w)
+    B, Tx, steps = 4, 30, 32
+    kw = dict(max_steps=steps, window=window, mu_bias=mu_bias)
+    mem = np.random.RandomState(3).uniform(-1, 1, (B, Tx, 512)).astype(np.float32)
+    masks = eng.philox_masks(77, offset, B, steps).cpu().numpy()
+    for rows in (slice(0, B), slice(2, 3)):                 # a batch (one block per sentence), one sentence (128-block decoder)
+        a = eng.decode(mem[rows], seed=77, utterance_offset=offset + rows.start, **kw)
+        b = eng.decode(mem[rows], masks=masks[rows], **kw)
+        for k in ('frames', 'stop', 'align', 'nsteps'):
+            assert np.array_equal(a[k].cpu().numpy(), b[k].cpu().numpy()), (rows, k)
+
+
 def test_decoder_error_behaviour():
     from tacotronv2_wavernn_chinese_b200._lib import B200TTSError
     from tacotronv2_wavernn_chinese_b200.tacotron.engine import TacoDecoderEngine
