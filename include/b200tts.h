@@ -212,7 +212,9 @@ int b200tts_wavernn_check(b200tts_wavernn* ctx);
  * session_open: a push session (session_open_kernel with kernel = B200TTS_KERNEL_AUTO).
  * session_open_kernel: d_mel [feat][T], T >= 21.  kernel: B200TTS_KERNEL_AUTO (push) or B200TTS_KERNEL_TC (tensor cores; refused
  *   where kernel=tc cannot run).  rng: PHILOX only, rng->utterance_offset is the utterance id (d_utterance_ids must be NULL).
- *   The conditioning tables are computed once, on `stream`, into memory the session owns.
+ *   A one-row b200tts_wavernn_session_open_batch of the mel (layout B200TTS_MEL_FEAT_T, T_max = T; T x max(feat_dims,
+ *   res_out_dims) must stay below 2^31): the conditioning tables are computed once, on `stream`, in three launches, into one
+ *   allocation of the session's table and state.
  * session_destroy: null-safe; waits for the runs still queued.  b200tts_wavernn_destroy frees the sessions still open.
  * session_info: next step, steps of the utterance (T*hop) and samples of its wave ((T-1)*hop); any pointer may be NULL.
  * session_run: n distinct sessions of ctx advance by min(max_steps, steps - pos) steps each in one launch (a finished session
@@ -234,9 +236,9 @@ int b200tts_wavernn_session_run(b200tts_wavernn* ctx, b200tts_wavernn_session* c
 int b200tts_wavernn_session_max_rows(const b200tts_wavernn* ctx);
 
 /* Batched open: n sessions in three launches whatever n is (mel preparation, MelResNet and the conditioning tables, each over the
- * rows' own frame counts), with no host copy of the mels.  Session i is bit for bit the session b200tts_wavernn_session_open_kernel
- * opens from row i's mel in [0, 1], zero-padded to max(h_frames[i], 21) frames, with the same seed, id, mu_law and kernel: its
- * pieces concatenate to that one-shot run.
+ * rows' own frame counts), with no host copy of the mels; b200tts_wavernn_session_open_kernel is its one-row case.  Session i is
+ * bit for bit the session b200tts_wavernn_session_open_kernel opens from row i's mel in [0, 1], zero-padded to max(h_frames[i], 21)
+ * frames, with the same seed, id, mu_law and kernel: its pieces concatenate to that one-shot run.
  *   d_mel, layout B200TTS_MEL_FEAT_T: [n][feat][T_max], in [0, 1].
  *          layout B200TTS_MEL_TACO:   [n][T_max][feat], the Tacotron postnet output, mapped on the device with the float32
  *          statements of the reference's synthesizer: m = clip(m, -max_abs_value, max_abs_value), clip((m + a) / (2a), 0, 1).

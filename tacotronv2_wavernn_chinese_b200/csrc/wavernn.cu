@@ -28,10 +28,9 @@ struct b200tts_wavernn_session {
   int T = 0, mu_law = 1;
   int64_t pos = 0, S = 0, wave_len = 0;     // next step; steps of the utterance; samples of its wave
   uint64_t seed = 0, id = 0;
-  DeviceBuf tab, state;                     // session_open(_kernel): memory of this session alone
-  std::shared_ptr<DeviceBuf> batch;         // session_open_batch: one allocation for the batch, freed with its last session
-  float* tab_p = nullptr;                   // the tables and the state, in `tab` / `state` or in `batch`
-  float* state_p = nullptr;
+  std::shared_ptr<DeviceBuf> mem;           // one allocation for the sessions opened together, freed with the last of them
+  float* tab = nullptr;                     // this session's tables and state, in `mem`
+  float* state = nullptr;
 };
 
 struct b200tts_wavernn {
@@ -608,18 +607,18 @@ static void launch_grid(b200tts_wavernn* ctx, const float* d_mel, const GenArgs&
 }
 
 // Conditioning tables [tab_rows][T+1][ncta][52] of the push and tensor-core kernels from the first `src_rows` utterances of the
-// mels / frame-rate aux, into `dst`, which is sized to hold them; table rows past the utterances are zero.
+// mels / frame-rate aux, into ctx->push_tab, which is sized to hold them; table rows past the utterances are zero.
 static const float* launch_cond_table(b200tts_wavernn* ctx, const float* d_mel, const float* aux_frames, int src_rows, int tab_rows,
-                                      int T, DeviceBuf& dst, cudaStream_t st) {
+                                      int T, cudaStream_t st) {
   const b200tts_wavernn_cfg& c = ctx->cfg;
   constexpr int FT = 8;
-  dst.ensure((size_t)tab_rows * (T + 1) * ctx->pm.ncta * kPushCondRows * sizeof(float));
+  ctx->push_tab.ensure((size_t)tab_rows * (T + 1) * ctx->pm.ncta * kPushCondRows * sizeof(float));
   dim3 grid((T + 1 + FT - 1) / FT, tab_rows);
   size_t smem = (size_t)(c.feat_dims + c.res_out_dims) * FT * sizeof(float);
-  push_cond_table_kernel<FT><<<grid, 256, smem, st>>>(ctx->pcw, d_mel, aux_frames, src_rows, T, dst.as<float>());
+  push_cond_table_kernel<FT><<<grid, 256, smem, st>>>(ctx->pcw, d_mel, aux_frames, src_rows, T, ctx->push_tab.as<float>());
   B200_CUDA(cudaGetLastError());
   ctx->launches++;
-  return dst.as<float>();
+  return ctx->push_tab.as<float>();
 }
 
 // ---- small-batch push kernel (wavernn_push.cuh) --------------------------------------------------------------------------
@@ -679,7 +678,7 @@ static void launch_push(b200tts_wavernn* ctx, const float* d_mel, const GenArgs&
   const int T = fold ? T0 : ua.T;
   const int tab_rows = fold ? 1 : (pack ? pack->n_utt : push_rows(rows)), src_rows = fold ? 1 : (pack ? pack->n_utt : rows);
   PushArgs a{};
-  a.tab = launch_cond_table(ctx, d_mel, ua.aux_frames, src_rows, tab_rows, T, ctx->push_tab, st);
+  a.tab = launch_cond_table(ctx, d_mel, ua.aux_frames, src_rows, tab_rows, T, st);
   a.B = pack ? pack->n_utt : rows; a.S = ua.S; a.T = T; a.steps = pack ? pack->steps : ua.steps;
   if (pack) { a.pack_utt = pack->utt; a.pack_start = pack->start; a.pack_segs = pack->segs; a.pack_rows = pack->rows; }
   a.row_stride = fold ? fold->stride : 0;
@@ -696,7 +695,7 @@ static void launch_tc(b200tts_wavernn* ctx, const float* d_mel, const GenArgs& u
   const int rows = ua.B, T = ua.T;
   const int ng = (rows + kTcRows - 1) / kTcRows;
   TcArgs a{};
-  if (!sess) a.tab = launch_cond_table(ctx, d_mel, ua.aux_frames, rows, rows, T, ctx->push_tab, st);
+  if (!sess) a.tab = launch_cond_table(ctx, d_mel, ua.aux_frames, rows, rows, T, st);
   ctx->tc_vec.ensure((size_t)TV_COUNT * ng * 2 * kTcVecBytes);
   ctx->tc_x1f.ensure((size_t)ng * 2 * kTcRows * 512 * sizeof(float));
   ctx->tc_win.ensure((size_t)ng * 2 * kTcWinCopies * kTcRows * 16 * sizeof(unsigned long long));
@@ -1038,6 +1037,18 @@ static void require_session_model(const b200tts_wavernn* ctx) {
   REQUIRE(ctx->pm.ok, B200TTS_EINVAL, "generation sessions need the push kernel (rnn_dims = fc_dims = 512 on >= 128 SMs)");
 }
 
+// The kernel and noise of a session open: kernel = AUTO (the push kernel) or TC where kernel=tc runs, and PHILOX noise (refused
+// with the message `noise`).  Returns whether the sessions run on the tensor cores.
+static bool require_session_kernel(const b200tts_wavernn* ctx, int kernel, const b200tts_rng& rng, const char* noise) {
+  REQUIRE(kernel == B200TTS_KERNEL_AUTO || kernel == B200TTS_KERNEL_TC, B200TTS_EINVAL,
+          "a session runs on kernel = AUTO (the push kernel) or TC (the tensor cores)");
+  const bool tc = kernel == B200TTS_KERNEL_TC;
+  REQUIRE(!tc || ctx->tc_ok, B200TTS_EINVAL, "tensor-core sessions need a model and device that run kernel=tc (rnn_dims = fc_dims = "
+                                             "512, 10-bit classes, hop_length x FIR taps <= 8192, >= 128 SMs)");
+  REQUIRE(rng.mode == B200TTS_RNG_PHILOX, B200TTS_EINVAL, noise);
+  return tc;
+}
+
 // The most sessions one run takes on ctx: a tensor-core run where that kernel runs, else a push run.
 extern "C" int b200tts_wavernn_session_max_rows(const b200tts_wavernn* ctx) {
   return ctx && ctx->tc_ok ? kTcSessRows : kPushMaxRows;
@@ -1048,73 +1059,15 @@ extern "C" int b200tts_wavernn_session_open(b200tts_wavernn* ctx, const float* d
   return b200tts_wavernn_session_open_kernel(ctx, d_mel, T, rng, mu_law, B200TTS_KERNEL_AUTO, out, stream);
 }
 
-extern "C" int b200tts_wavernn_session_open_kernel(b200tts_wavernn* ctx, const float* d_mel, int T, const b200tts_rng* rng,
-                                                   int mu_law, int kernel, b200tts_wavernn_session** out, void* stream) {
-  API_BEGIN
-  REQUIRE(ctx && d_mel && rng && out, B200TTS_EINVAL, "null argument");
-  *out = nullptr;
-  require_session_model(ctx);
-  REQUIRE(kernel == B200TTS_KERNEL_AUTO || kernel == B200TTS_KERNEL_TC, B200TTS_EINVAL,
-          "a session runs on kernel = AUTO (the push kernel) or TC (the tensor cores)");
-  const bool tc = kernel == B200TTS_KERNEL_TC;
-  REQUIRE(!tc || ctx->tc_ok, B200TTS_EINVAL, "tensor-core sessions need a model and device that run kernel=tc (rnn_dims = fc_dims = "
-                                             "512, 10-bit classes, hop_length x FIR taps <= 8192, >= 128 SMs)");
-  REQUIRE(rng->mode == B200TTS_RNG_PHILOX && !rng->d_utterance_ids, B200TTS_EINVAL,
-          "a session takes PHILOX noise keyed by (seed, rng->utterance_offset as the utterance id); d_utterance_ids must be NULL");
-  const int hop = ctx->cfg.hop_length;
-  REQUIRE(T >= 21, B200TTS_EINVAL, "T must be >= 21 frames: the reference's 20-hop fade-out (fatchord_version.py:256-258) fails below that");
-  REQUIRE((long long)T * hop <= INT_MAX, B200TTS_EINVAL, "utterance longer than 2^31 - 1 samples");
-  DeviceGuard dg(ctx->device);
-  const cudaStream_t st = (cudaStream_t)stream;
-  std::unique_ptr<b200tts_wavernn_session> s(new b200tts_wavernn_session());
-  s->ctx = ctx;
-  s->tc = tc;
-  s->T = T;
-  s->mu_law = mu_law ? 1 : 0;
-  s->S = (int64_t)T * hop;
-  s->wave_len = (int64_t)(T - 1) * hop;
-  s->seed = rng->seed;
-  s->id = rng->utterance_offset;
-  s->state.ensure((size_t)kSessStateFloats * sizeof(float));
-  // the conditioning of a one-shot run of this mel, once: MelResNet into the context's scratch, consumed in stream order by the
-  // tables, which the session owns (the next generate overwrites every scratch buffer)
-  ctx->aux_frames.ensure((size_t)T * ctx->cfg.res_out_dims * sizeof(float));
-  run_upsample(ctx, d_mel, 1, T, nullptr, ctx->aux_frames.as<float>(), nullptr, st);
-  s->tab_p = const_cast<float*>(launch_cond_table(ctx, d_mel, ctx->aux_frames.as<float>(), 1, 1, T, s->tab, st));
-  s->state_p = s->state.as<float>();
-  ctx->sessions.insert(s.get());
-  *out = s.release();
-  API_END
-}
-
-// n sessions in three launches (wavernn_open.cuh), bit for bit the sessions session_open_kernel opens one by one from the same mels.
-// Their tables and states share one allocation: a one-by-one open spends two cudaMalloc on every session (DESIGN 3.11.1).
-extern "C" int b200tts_wavernn_session_open_batch(b200tts_wavernn* ctx, const float* d_mel, int layout, float max_abs_value,
-                                                  const int32_t* h_frames, int n, int T_max, const b200tts_rng* rng, int mu_law,
-                                                  int kernel, b200tts_wavernn_session** out, void* stream) {
-  API_BEGIN
-  REQUIRE(ctx && d_mel && h_frames && rng && out, B200TTS_EINVAL, "null argument");
-  require_session_model(ctx);
-  REQUIRE(kernel == B200TTS_KERNEL_AUTO || kernel == B200TTS_KERNEL_TC, B200TTS_EINVAL,
-          "a session runs on kernel = AUTO (the push kernel) or TC (the tensor cores)");
-  const bool tc = kernel == B200TTS_KERNEL_TC;
-  REQUIRE(!tc || ctx->tc_ok, B200TTS_EINVAL, "tensor-core sessions need a model and device that run kernel=tc (rnn_dims = fc_dims = "
-                                             "512, 10-bit classes, hop_length x FIR taps <= 8192, >= 128 SMs)");
-  REQUIRE(rng->mode == B200TTS_RNG_PHILOX, B200TTS_EINVAL,
-          "sessions take PHILOX noise keyed by (seed, utterance id: d_utterance_ids[i], or utterance_offset + i)");
-  REQUIRE(layout == B200TTS_MEL_FEAT_T || layout == B200TTS_MEL_TACO, B200TTS_EINVAL,
-          "unknown mel layout (B200TTS_MEL_FEAT_T or B200TTS_MEL_TACO)");
-  REQUIRE(layout != B200TTS_MEL_TACO || (std::isfinite(max_abs_value) && max_abs_value > 0.f), B200TTS_EINVAL,
-          "max_abs_value must be positive and finite");
-  REQUIRE(n >= 1 && n <= b200tts_wavernn_session_max_rows(ctx), B200TTS_EINVAL, "n must be 1..session_max_rows");
-  REQUIRE(T_max >= 1, B200TTS_EINVAL, "T_max must be >= 1");
-  const int hop = ctx->cfg.hop_length, FEAT = ctx->cfg.feat_dims, O = ctx->cfg.res_out_dims, ncta = ctx->pm.ncta;
+// The rows of a session open from its mels' frame counts h_frames[n] (host): session i takes T = max(frames, 21) frames, zero-padded
+// to the 21 frames the 20-hop fade-out needs, as StreamingVocoder pads.  Their tables are placed by open_sessions.
+static OpenRows open_rows(const b200tts_wavernn* ctx, const int32_t* h_frames, int n, int T_max) {
+  const int hop = ctx->cfg.hop_length, FEAT = ctx->cfg.feat_dims, O = ctx->cfg.res_out_dims;
   OpenRows R{};
   R.n = n;
-  size_t tab_floats = 0;
   for (int i = 0; i < n; ++i) {
     REQUIRE(h_frames[i] >= 1 && h_frames[i] <= T_max, B200TTS_EINVAL, "every row needs 1..T_max frames");
-    const int T = std::max(h_frames[i], 21);     // zero-padded to the 21 frames the 20-hop fade-out needs, as StreamingVocoder pads
+    const int T = std::max(h_frames[i], 21);
     REQUIRE((long long)T * hop <= INT_MAX, B200TTS_EINVAL, "utterance longer than 2^31 - 1 samples");
     R.frames[i] = h_frames[i];
     R.T[i] = T;
@@ -1122,40 +1075,16 @@ extern "C" int b200tts_wavernn_session_open_batch(b200tts_wavernn* ctx, const fl
     R.f0[i + 1] = R.f0[i] + T;
     R.res0[i + 1] = R.res0[i] + (T + kOpenFT - 1) / kOpenFT;
     R.tab0[i + 1] = R.tab0[i] + (T + 1 + kOpenFT - 1) / kOpenFT;
-    tab_floats += (size_t)(T + 1) * ncta * kPushCondRows;
   }
-  DeviceGuard dg(ctx->device);
-  const cudaStream_t st = (cudaStream_t)stream;
-  std::vector<uint64_t> ids(n);
-  if (rng->d_utterance_ids) {       // the run kernels take each session's id as a parameter: read them back, in stream order
-    B200_CUDA(cudaMemcpyAsync(ids.data(), rng->d_utterance_ids, n * sizeof(uint64_t), cudaMemcpyDeviceToHost, st));
-    B200_CUDA(cudaStreamSynchronize(st));
-  } else {
-    for (int i = 0; i < n; ++i) ids[i] = rng->utterance_offset + (uint64_t)i;
-  }
-  // one allocation: the n tables, then the n states (each state 256-byte aligned)
-  const size_t state_floats = ((size_t)kSessStateFloats + 63) / 64 * 64;
-  auto block = std::make_shared<DeviceBuf>();
-  block->ensure((tab_floats + (size_t)n * state_floats) * sizeof(float));
-  float* base = block->as<float>();
-  std::vector<std::unique_ptr<b200tts_wavernn_session>> ss(n);
-  size_t off = 0;
-  for (int i = 0; i < n; ++i) {
-    ss[i].reset(new b200tts_wavernn_session());
-    b200tts_wavernn_session& s = *ss[i];
-    s.ctx = ctx;
-    s.tc = tc;
-    s.T = R.T[i];
-    s.mu_law = mu_law ? 1 : 0;
-    s.S = (int64_t)R.T[i] * hop;
-    s.wave_len = (int64_t)(R.T[i] - 1) * hop;
-    s.seed = rng->seed;
-    s.id = ids[i];
-    s.batch = block;
-    s.tab_p = R.tab[i] = base + off;
-    s.state_p = base + tab_floats + (size_t)i * state_floats;
-    off += (size_t)(R.T[i] + 1) * ncta * kPushCondRows;
-  }
+  return R;
+}
+
+// Opens the sessions of rows R (open_rows) from d_mel (`layout`, rows of T_max frames) in three launches (wavernn_open.cuh); session
+// i takes the utterance id ids[i].  Their tables and states share one allocation, freed with the last of them: a cudaMalloc is
+// most of a one-row open's time (DESIGN 3.11.1).  Checks nothing: its callers have.
+static void open_sessions(b200tts_wavernn* ctx, const float* d_mel, int layout, float max_abs_value, OpenRows R, int T_max,
+                          uint64_t seed, const uint64_t* ids, int mu_law, bool tc, b200tts_wavernn_session** out, cudaStream_t st) {
+  const int n = R.n, hop = ctx->cfg.hop_length, FEAT = ctx->cfg.feat_dims, O = ctx->cfg.res_out_dims, ncta = ctx->pm.ncta;
   // the prepared mels and MelResNet's output go to the context's scratch, consumed in stream order by the table launch
   const int frames = R.f0[n];
   ctx->mel_in.ensure((size_t)frames * FEAT * sizeof(float));
@@ -1172,14 +1101,83 @@ extern "C" int b200tts_wavernn_session_open_batch(b200tts_wavernn* ctx, const fl
     B200_CUDA(cudaFuncSetAttribute(melresnet_ragged_kernel<kOpenFT>, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)res_smem));
   melresnet_ragged_kernel<kOpenFT><<<R.res0[n], threads, res_smem, st>>>(ctx->rp, mel, R, aux);
   B200_CUDA(cudaGetLastError());
+  ctx->launches += 2;
+  // one allocation, made while those kernels run: the n tables, table i of T_i + 1 frames from frame f0[i] + i, then the n
+  // states (each 256-byte aligned)
+  const size_t tab_frame = (size_t)ncta * kPushCondRows, tab_floats = (size_t)(R.f0[n] + n) * tab_frame;
+  const size_t state_floats = ((size_t)kSessStateFloats + 63) / 64 * 64;
+  auto mem = std::make_shared<DeviceBuf>();
+  mem->ensure((tab_floats + (size_t)n * state_floats) * sizeof(float));
+  float* base = mem->as<float>();
+  std::vector<std::unique_ptr<b200tts_wavernn_session>> ss(n);
+  for (int i = 0; i < n; ++i) {
+    ss[i].reset(new b200tts_wavernn_session());
+    b200tts_wavernn_session& s = *ss[i];
+    s.ctx = ctx;
+    s.tc = tc;
+    s.T = R.T[i];
+    s.mu_law = mu_law ? 1 : 0;
+    s.S = (int64_t)R.T[i] * hop;
+    s.wave_len = (int64_t)(R.T[i] - 1) * hop;
+    s.seed = seed;
+    s.id = ids[i];
+    s.mem = mem;
+    s.tab = R.tab[i] = base + (size_t)(R.f0[i] + i) * tab_frame;
+    s.state = base + tab_floats + (size_t)i * state_floats;
+  }
   const size_t tab_smem = (size_t)(FEAT + O) * kOpenFT * sizeof(float);
   push_cond_table_ragged_kernel<kOpenFT><<<R.tab0[n], 256, tab_smem, st>>>(ctx->pcw, mel, aux, R);
   B200_CUDA(cudaGetLastError());
-  ctx->launches += 3;
+  ctx->launches++;
   for (int i = 0; i < n; ++i) {
     ctx->sessions.insert(ss[i].get());
     out[i] = ss[i].release();
   }
+}
+
+// A one-row batched open of the mel as it is (T >= 21 frames need no padding), with open_rows refusing one too long.
+extern "C" int b200tts_wavernn_session_open_kernel(b200tts_wavernn* ctx, const float* d_mel, int T, const b200tts_rng* rng,
+                                                   int mu_law, int kernel, b200tts_wavernn_session** out, void* stream) {
+  API_BEGIN
+  REQUIRE(ctx && d_mel && rng && out, B200TTS_EINVAL, "null argument");
+  *out = nullptr;
+  require_session_model(ctx);
+  const char* noise = "a session takes PHILOX noise keyed by (seed, rng->utterance_offset as the utterance id); d_utterance_ids "
+                      "must be NULL";
+  const bool tc = require_session_kernel(ctx, kernel, *rng, noise);
+  REQUIRE(!rng->d_utterance_ids, B200TTS_EINVAL, noise);
+  REQUIRE(T >= 21, B200TTS_EINVAL, "T must be >= 21 frames: the reference's 20-hop fade-out (fatchord_version.py:256-258) fails below that");
+  const OpenRows R = open_rows(ctx, &T, 1, T);
+  DeviceGuard dg(ctx->device);
+  open_sessions(ctx, d_mel, B200TTS_MEL_FEAT_T, 0.f, R, T, rng->seed, &rng->utterance_offset, mu_law, tc, out, (cudaStream_t)stream);
+  API_END
+}
+
+extern "C" int b200tts_wavernn_session_open_batch(b200tts_wavernn* ctx, const float* d_mel, int layout, float max_abs_value,
+                                                  const int32_t* h_frames, int n, int T_max, const b200tts_rng* rng, int mu_law,
+                                                  int kernel, b200tts_wavernn_session** out, void* stream) {
+  API_BEGIN
+  REQUIRE(ctx && d_mel && h_frames && rng && out, B200TTS_EINVAL, "null argument");
+  require_session_model(ctx);
+  const bool tc = require_session_kernel(
+      ctx, kernel, *rng, "sessions take PHILOX noise keyed by (seed, utterance id: d_utterance_ids[i], or utterance_offset + i)");
+  REQUIRE(layout == B200TTS_MEL_FEAT_T || layout == B200TTS_MEL_TACO, B200TTS_EINVAL,
+          "unknown mel layout (B200TTS_MEL_FEAT_T or B200TTS_MEL_TACO)");
+  REQUIRE(layout != B200TTS_MEL_TACO || (std::isfinite(max_abs_value) && max_abs_value > 0.f), B200TTS_EINVAL,
+          "max_abs_value must be positive and finite");
+  REQUIRE(n >= 1 && n <= b200tts_wavernn_session_max_rows(ctx), B200TTS_EINVAL, "n must be 1..session_max_rows");
+  REQUIRE(T_max >= 1, B200TTS_EINVAL, "T_max must be >= 1");
+  const OpenRows R = open_rows(ctx, h_frames, n, T_max);
+  DeviceGuard dg(ctx->device);
+  const cudaStream_t st = (cudaStream_t)stream;
+  std::vector<uint64_t> ids(n);
+  if (rng->d_utterance_ids) {       // the run kernels take each session's id as a parameter: read them back, in stream order
+    B200_CUDA(cudaMemcpyAsync(ids.data(), rng->d_utterance_ids, n * sizeof(uint64_t), cudaMemcpyDeviceToHost, st));
+    B200_CUDA(cudaStreamSynchronize(st));
+  } else {
+    for (int i = 0; i < n; ++i) ids[i] = rng->utterance_offset + (uint64_t)i;
+  }
+  open_sessions(ctx, d_mel, layout, max_abs_value, R, T_max, rng->seed, ids.data(), mu_law, tc, out, st);
   API_END
 }
 
@@ -1227,8 +1225,8 @@ extern "C" int b200tts_wavernn_session_run(b200tts_wavernn* ctx, b200tts_wavernn
   int steps = 0;
   for (int i = 0; i < n; ++i) {
     SessRow& r = io.row[i];
-    r.tab = s[i]->tab_p;
-    r.state = s[i]->state_p;
+    r.tab = s[i]->tab;
+    r.state = s[i]->state;
     r.seed = s[i]->seed;
     r.id = s[i]->id;
     r.T = s[i]->T;

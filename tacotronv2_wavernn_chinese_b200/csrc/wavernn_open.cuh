@@ -5,7 +5,7 @@
 //   melresnet_ragged_kernel<FT>    MelResNet over every row's tiles (melresnet_tile, as melresnet_kernel runs one row);
 //   push_cond_table_ragged_kernel  every row's [T+1][ncta][52] table (push_cond_table_tile), into the session's memory.
 // A tile of either ragged kernel finds its row by a binary search over the prefix sums of tiles per row, then computes exactly
-// what the one-row launch of b200tts_wavernn_session_open_kernel computes for that tile: same statements, same operands.
+// what melresnet_kernel / push_cond_table_kernel compute for that tile of a one-row launch: same statements, same operands.
 #pragma once
 #include "wavernn_push.cuh"
 #include "wavernn_upsample.cuh"
@@ -13,7 +13,7 @@
 namespace b200tts {
 
 constexpr int kOpenMaxRows = 256;   // kTcSessRows: the most sessions one run takes
-constexpr int kOpenFT = 8;          // frames per CTA of MelResNet and the tables, as the one-row open launches them
+constexpr int kOpenFT = 8;          // frames per CTA of MelResNet and the tables, as one-shot generation launches them
 
 struct OpenRows {                   // passed by value (6 KB of kernel parameters)
   int n;
